@@ -1,8 +1,8 @@
-# Convenience targets (the driver uses __graft_entry__.build(), which runs the same commands).
+# Convenience targets (__graft_entry__.build() runs the same commands).
 .PHONY: all lib oracle ref cpp test clean
 all: lib oracle cpp
 
-lib:            ## libsrtb_b200.so (nvcc, sm_100a only)
+lib:            ## libsrtb_b200.so (nvcc, sm_90a only)
 	simple-radio-telescope-backend_b200/csrc/build.sh
 
 oracle:         ## CPU oracle (test infrastructure)
@@ -14,7 +14,7 @@ ref:            ## the reference's own headers through the host SYCL shim (needs
 cpp: lib        ## C++ pipe framework tests + pipeline_main (the reference's main.cpp wiring on the re-hosted pipes)
 	$(MAKE) -C tests/cpp all
 
-test:           ## CPU-only suite; add `-m gpu` on a B200
+test:           ## CPU-only suite; add `-m gpu` on an H100
 	python -m pytest tests -q -m "not gpu"
 
 clean:

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
 """bench.py — Gsamples/s of 8-bit baseband through the full coherent-dedispersion chain
-(unpack -> fft_r2c -> rfi_s1 -> dedisperse -> watfft -> rfi_s2 -> signal_detect) on B200,
+(unpack -> fft_r2c -> rfi_s1 -> dedisperse -> watfft -> rfi_s2 -> signal_detect) on H100,
 with per-stage achieved HBM GB/s against the measured copy peak, next to the restated
 reference CPU path timed on the same box.
 
-Contract (driver): python bench.py --gpus N --steps K --warmup W [--impl reference]
+Usage: python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
   * a "step" = one block of synthetic baseband through the whole chain on each rank;
   * workload = BASELINE.json configs[2], the J1644-4559 shape the north star names: dual-polarisation
     8-bit, 2^26 samples per stream per block, 400 MHz, DM 562.05, C = 2^11 channels (rows of 2^14 time
@@ -21,13 +21,16 @@ Contract (driver): python bench.py --gpus N --steps K --warmup W [--impl referen
     of its detector result (and of positive series) are inside the timed region;
   * `roofline` = the dominant kernel of the block path (the one-kernel waterfall group: s1 + chirp + waterfall FFT + SK +
     column sums): its compulsory bytes per launch / its launch time, CUDA events inside the library on the launching
-    stream, vs the measured copy peak (MEASURED_PEAKS.json hbm_gbs, else 6650 fallback); `traffic` = its DRAM bytes per
+    stream, vs the measured copy peak (MEASURED_PEAKS.json hbm_gbs, else the data sheet's 3350); `traffic` = its DRAM bytes per
     launch from the committed ncu capture; `roofline.fused` has every kernel group of the block path against the bytes
     THEY must move; `stages` every per-pipe C-ABI stage alone (SURVEY.md §8d bytes); `roofline.chain` the whole block on
     three byte counts (unfused algorithmic, the launched kernels' sweep bytes, measured DRAM bytes);
   * `cpu_baseline` = the CPU oracle (port of the reference operators, OpenMP, all host cores) on a bounded
     sample of the same workload (rank 0, N = 1 only).
 --impl reference times that CPU path alone (rank 0) with the same JSON shape.
+--dump-outputs DIR writes what the last timed step returned to its caller as DIR/<name>.npy (rank 0): the detector
+result headers of every stream and a fixed, seeded sample of each stream's dynamic spectrum (at most 64 MiB in all).
+The synthetic blocks are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -42,9 +45,9 @@ import time
 from pathlib import Path
 
 # The two lanes of a context rely on the driver giving their CUDA streams separate hardware work queues. With NCCL in
-# the process (torchrun, N > 1) and this variable unset the lanes were seen to alias (config 3: 120 instead of 131
-# Gsamples/s per GPU); 8 — the documented default — set explicitly restores it, 1 serialises them, 32 co-schedules the
-# big sweeps and is slower (profiles/r02s_connections.md). Must be in the environment before CUDA initialises.
+# the process (torchrun, N > 1) and this variable unset the lanes can alias; 8 — the documented default — set
+# explicitly keeps them apart, 1 serialises them, 32 co-schedules the big sweeps. Must be in the environment before CUDA
+# initialises.
 os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "8")
 
 ROOT = Path(__file__).resolve().parent
@@ -124,7 +127,7 @@ def hbm_peak():
             return float(json.loads(p.read_text())["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3; not measured)"
 
 
 # kernels of each per-pipe stage, for summing the ncu DRAM traffic of profiles/traffic.json
@@ -268,8 +271,8 @@ def synth_block_with_pulse(n: int, streams: int, seed: int, w: dict) -> np.ndarr
 
 def bind_to_gpu_numa_node(torch, device_index: int):
     """Multi-rank runs: keep this rank's thread (and with it the pinned host blocks it allocates from now on) on the
-    NUMA node its GPU hangs off — eight ranks pulling 55 GB/s each out of host memory otherwise depend on where the
-    scheduler happened to start them (8 GPUs: 430 against 270 Gsamples/s end to end, profiles/r02t_scaling.md).
+    NUMA node its GPU hangs off — ranks pulling tens of GB/s each out of host memory otherwise depend on where the
+    scheduler happened to start them.
     Returns the node, or None when the topology cannot be read (nothing is changed then)."""
     try:
         pr = torch.cuda.get_device_properties(device_index)
@@ -292,10 +295,10 @@ def bind_to_gpu_numa_node(torch, device_index: int):
 
 
 class RankSync:
-    """Plumbing between the ranks of one node. The default process group is NCCL, as the launch contract says, but it
+    """Plumbing between the ranks of one node. The default process group is NCCL, as torchrun launches expect, but it
     is created lazily and this path has no data-path collective, so NO NCCL communicator exists while blocks are timed:
-    barriers and the max-over-ranks go through a gloo group on host scalars. (A communicator in the process costs the
-    two-lane path up to 8 %: its streams take hardware work queues, profiles/r02s_connections.md.) NCCL is exercised
+    barriers and the max-over-ranks go through a gloo group on host scalars. (A communicator in the process can slow
+    the two-lane path: its streams take hardware work queues.) NCCL is exercised
     once, after everything is measured, by close(). SRTB_BENCH_EAGER_NCCL=1 restores an eager communicator and NCCL
     barriers for comparison."""
 
@@ -553,7 +556,7 @@ class Harness:
         self.fmt = srtb_b200.FORMAT_BY_NAME[w["fmt"]]
         self.streams = srtb_b200.FORMAT_STREAMS[self.fmt]
         self.block_bytes = self.n * self.streams * abs(w["bits"]) // 8
-        self.ring = max(2, min(16, (288 << 20) // self.block_bytes))      # > L2 (126 MB) of distinct input
+        self.ring = max(2, min(16, (288 << 20) // self.block_bytes))      # > L2 (50 MB) of distinct input
         self.stream = torch.cuda.current_stream()
         self.extra_streams = [torch.cuda.Stream() for _ in range(max(0, n_contexts - 1))]
         self.ctxs = [srtb_b200.Context(local_rank, self.stream.cuda_stream)] + \
@@ -592,6 +595,7 @@ class Harness:
         self.detections = 0
         self.blocks_with_detection = 0
         self._tickets = []
+        self.last_output = None   # (detector results, device pointers of the dynamic spectra) of the last block collected
 
     def close(self):
         for c in self.ctxs:
@@ -603,7 +607,8 @@ class Harness:
 
     def _collect(self):
         c, t = self._tickets.pop(0)
-        res = c.collect_block(t)
+        res, _, spectra = c.collect_block_ex(t)
+        self.last_output = (res, spectra)
         found = sum(int(r.signal_count[b]) for r in res for b in range(r.n_boxcars))
         self.detections += found
         self.blocks_with_detection += 1 if found else 0
@@ -671,16 +676,18 @@ def run_dm_sweep(args, torch, srtb_b200, w, wname, rank, local_rank, world, dist
     H = Harness(torch, srtb_b200, wname, w, 1, rank, local_rank, inject_pulse=True)
     ctx, dms = H.ctxs[0], w["dms"]
     by_dm = np.zeros(len(dms), np.int64)
+    last = []
 
     def step(i, host):
         blk = (H.host_blocks if host else H.dev_blocks)[i % H.ring]
         res = ctx.process_block_dm_sweep(H.cfg, blk, H.block_bytes, dms, on_device=not host)
+        last[:] = res
         for j, per_stream in enumerate(res):
             by_dm[j] += sum(int(r.signal_count[b]) for r in per_stream for b in range(r.n_boxcars))
 
     for i in range(max(args.warmup, 3)):
         step(i, False)
-    steps = max(4, min(args.steps, 40))
+    steps = args.steps
     sampler = ClockSampler(local_rank)
     if rank == 0:
         sampler.start()
@@ -689,6 +696,11 @@ def run_dm_sweep(args, torch, srtb_b200, w, wname, rank, local_rank, world, dist
     ms = H.timed(lambda i: step(i, False), steps, dist) / steps
     launches = H.launch_count - l0
     found = by_dm.copy()
+    if args.dump_outputs and rank == 0:
+        out = Path(args.dump_outputs)
+        out.mkdir(parents=True, exist_ok=True)
+        dump_detect_results(out, [r for per_stream in last for r in per_stream])   # rows: (trial DM, stream)
+        np.save(out / "detect_dm.npy", np.repeat(np.asarray(dms, np.float64), len(last[0])))
     for i in range(3):
         step(i, True)
     ms_e2e = float(np.median([H.timed(lambda i: step(i, True), steps, dist) / steps for _ in range(3)]))
@@ -795,6 +807,43 @@ def run_udp_stream(args, torch, w, wname, rank, local_rank, world, dist):
     return 0
 
 
+DUMP_SPECTRUM_POINTS = 1 << 21   # per stream: 16 MiB of float32 (re, im) pairs, four streams at most
+DUMP_SEED = 20261015
+
+
+def dump_detect_results(out_dir: Path, results, prefix: str = "detect"):
+    """detector result headers, one row per stream (a list of DetectResult), as float64 arrays"""
+    nb = max([int(r.n_boxcars) for r in results] + [1])
+    cols = {"zero_count": lambda r: [r.zero_count], "time_series_count": lambda r: [r.time_series_count],
+            "detect_enabled": lambda r: [r.detect_enabled], "n_boxcars": lambda r: [r.n_boxcars],
+            "boxcar_length": lambda r: r.boxcar_length[:nb], "series_length": lambda r: r.series_length[:nb],
+            "signal_count": lambda r: r.signal_count[:nb], "variance": lambda r: r.variance[:nb],
+            "threshold": lambda r: r.threshold[:nb]}
+    for name, get in cols.items():
+        np.save(out_dir / f"{prefix}_{name}.npy", np.array([list(get(r)) for r in results], np.float64))
+
+
+def dump_block_outputs(torch, out_dir: str, last_output, n: int):
+    """the last timed block as its caller receives it: detector results per stream, and its dynamic spectra (n / 2
+    complex64 points per stream, [channel][time]) at a fixed, seeded sample of DUMP_SPECTRUM_POINTS indices"""
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    results, spectra = last_output
+    dump_detect_results(out, results)
+    nc = n // 2
+    k = min(nc, DUMP_SPECTRUM_POINTS)
+    idx = np.sort(np.random.default_rng(DUMP_SEED).choice(nc, size=k, replace=False))
+    d_idx = torch.from_numpy(idx).cuda()
+
+    class DeviceSpectrum:   # the library's buffer seen as a [nc][2] float32 tensor, no copy
+        def __init__(self, ptr):
+            self.__cuda_array_interface__ = {"shape": (nc, 2), "typestr": "<f4", "data": (ptr, False), "version": 3}
+
+    sample = np.stack([torch.as_tensor(DeviceSpectrum(ptr), device="cuda")[d_idx].cpu().numpy() for ptr in spectra])
+    np.save(out / "spectrum_sample.npy", sample)
+    np.save(out / "spectrum_sample_index.npy", idx.astype(np.float64))
+
+
 def main():
     claim_stdout()
     ap = argparse.ArgumentParser()
@@ -808,6 +857,8 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-pulse", action="store_true", help="noise-only blocks (no injected dispersed pulse)")
     ap.add_argument("--stage-iters", type=int, default=5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32 / float64)")
     ap.add_argument("--contexts", type=int, default=int(os.environ.get("SRTB_BENCH_CONTEXTS", "0")),
                     help="contexts per GPU that blocks alternate over (0 = 1 for multi-stream blocks of >= 2^26 samples, whose "
                          "streams the context overlaps itself; else 6 up to 2^24-sample blocks, 4 up to 2^27, 2 above)")
@@ -836,6 +887,8 @@ def main():
     if wname == "config4":
         return run_dm_sweep(args, torch, srtb_b200, w, wname, rank, local_rank, world, dist)
     if wname == "config5":
+        if args.dump_outputs:
+            raise SystemExit("bench.py: --dump-outputs is not available for config5 (its timed path is the executable)")
         return run_udp_stream(args, torch, w, wname, rank, local_rank, world, dist)
 
     n_ctx = args.contexts if args.contexts > 0 else default_contexts(w)
@@ -859,6 +912,8 @@ def main():
         sampler.snapshot()          # short run: take one sample while the GPU is still under load
     ms_per_step = ms_total / args.steps
     value = samples_per_step / (ms_per_step * 1e-3) / 1e9
+    if args.dump_outputs and rank == 0:
+        dump_block_outputs(torch, args.dump_outputs, H.last_output, n)
 
     # ---- end to end from pinned host memory (`e2e`)
     H.warm(H.step_e2e, args.warmup)
@@ -874,7 +929,7 @@ def main():
     if len(H.ctxs) > 1:
         extra, H.ctxs, H.extra_streams = (H.ctxs[1:], H.extra_streams), H.ctxs[:1], []
         H.warm(H.step_device, args.warmup)
-        ms1 = H.timed(H.step_device, max(10, args.steps // 2), dist) / max(10, args.steps // 2)
+        ms1 = H.timed(H.step_device, args.steps, dist) / args.steps
         single = {"value": samples_per_step / (ms1 * 1e-3) / 1e9, "unit": UNIT, "ms_per_step": ms1, "contexts_per_gpu": 1}
         H.ctxs, H.extra_streams = H.ctxs + extra[0], extra[1]
     else:
@@ -1004,7 +1059,7 @@ def main():
         torch.cuda.empty_cache()
         w2 = WORKLOADS[args.secondary]
         H2 = Harness(torch, srtb_b200, args.secondary, w2, default_contexts(w2), rank, local_rank, inject_pulse=False)
-        steps2 = max(args.steps, 200)
+        steps2 = args.steps
         H2.warm(H2.step_device, args.warmup)
         ms2 = H2.timed(H2.step_device, steps2, dist) / steps2
         H2.warm(H2.step_e2e, args.warmup)

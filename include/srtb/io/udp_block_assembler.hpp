@@ -105,11 +105,13 @@ class block_assembler {
                   pkt.data() + Backend::packet_header_size, packet_data_size);
       received++;
     };
-    if (carry_.has_value()) {  // a packet of this block that arrived while the previous one was closing
+    if (carry_.has_value()) {  // a packet past the previous block that arrived while that one was closing
       const uint64_t c = Backend::parse_counter(*carry_);
       if (!begin_counter.has_value()) begin_counter = c;
       if (c >= begin_counter.value() && c < begin_counter.value() + count) place(*carry_, c);
-      carry_.reset();
+      // a packet more than one block ahead (after a long gap) waits for its own block; this one is all gap
+      if (c >= begin_counter.value() + count) closed = true;
+      else carry_.reset();
     }
     while (!closed) {
       std::span<const std::byte> pkt;

@@ -17,7 +17,7 @@ namespace srtb {
 namespace pipeline {
 
 /** how a pipe thread waits on an empty (or full) queue: spin briefly — a block spends tens of microseconds per
- *  stage on a B200, while sleep_for(1 us) really sleeps ~60 us (timer slack) — then fall back to the reference's
+ *  stage on the GPU, while sleep_for(1 us) really sleeps ~60 us (timer slack) — then fall back to the reference's
  *  sleep of thread_query_work_wait_time ns (pipe_io.hpp:45). */
 struct queue_backoff {
   static constexpr int spin_limit = 2048;

@@ -1,4 +1,4 @@
-/* srtb_b200.h — C ABI of libsrtb_b200.so: the B200-native drop-in for srtb's
+/* srtb_b200.h — C ABI of libsrtb_b200.so: the H100-native drop-in for srtb's
  * baseband -> single-pulse hot path
  *   unpack -> fft_1d_r2c -> rfi_mitigation_s1 -> dedisperse -> watfft_1d_c2c
  *          -> rfi_mitigation_s2 -> signal_detect

@@ -799,6 +799,14 @@ void srtb_oracle_set_threads(int n) {
 #endif
 }
 
+// count_signal of one series (signal_detect.hpp:32-72): elements above snr * sqrt(mean(v^2))
+uint64_t srtb_oracle_count_signal(const float* v, size_t n, float snr) {
+  float var = 0, thr = 0;
+  uint64_t cnt = 0;
+  count_signal(v, n, snr, &var, &thr, &cnt);
+  return cnt;
+}
+
 int srtb_oracle_num_threads(void) {
 #if defined(_OPENMP)
   return omp_get_max_threads();

@@ -19,9 +19,11 @@
 //     signalled on its own mbarrier. Shared memory holds THREE half-row buffers that
 //     rotate: while row r is transformed in two of them, the first half of row r + 1 lands in the third, and its
 //     second half follows into the buffer row r frees first — stage 0 consumes chunk i while chunks i + 1.. arrive;
-//   * the detector's column sums (one accumulator per time sample, 64 KiB for 2^14) live in TENSOR MEMORY, not in
-//     shared memory: every thread owns 32 cells of its warp's TMEM lane quadrant (tcgen05.ld / tcgen05.st,
-//     SASS LDTM / STTM) — the tensor cores have no work on this path, their 256 KiB accumulator file does;
+//   * the detector's column sums (one accumulator per time sample, 64 KiB for 2^14) fit neither in shared memory
+//     (three half rows and the tables take 209 KiB of the 227 KiB a block may have) nor in registers (the
+//     butterflies use all 128 a thread gets at 512 threads): every thread owns 32 cells of its CTA's partial row in
+//     global memory, read and written back once per row with an L2 evict-last policy, so the row stays in L2
+//     (grid x ts_count x 4 bytes: 8 MiB per lane on 132 SMs, against 50 MB) while the spectrum streams past it;
 //   * twiddles: stage 0 from W_L^j by repeated multiplication, stages 1 and 2 from small shared-memory tables;
 //   * the chirp phase is evaluated in fp64 like the reference; 1/f comes from one correctly rounded reciprocal per
 //     thread and Newton steps from the neighbouring bin: one step when (B1*df/f)^2 <= 2^-52 (the reciprocal is then
@@ -44,45 +46,26 @@ struct bigrow {
   static constexpr int NT = L / 32;         // threads: 32 points each
   static constexpr int NW = NT / 32;
   static constexpr int CTAS = (LOGL == 13) ? 2 : 1;
-  static constexpr int TMEM_COLS = NW * 8;  // 32 accumulator cells per thread: (NW / 4) column blocks of 32 per lane quadrant
   static constexpr int TABN = B1 + 15 * B2 + 15 * R3;  // W_L^j | W_B1^{i j} [15][B2] | W_B2^{i j} [15][R3]
   static constexpr size_t off_tab = 3 * (size_t)HALF * sizeof(float2);
   static constexpr size_t off_mbar = off_tab + (size_t)TABN * sizeof(float2);
-  static constexpr size_t off_red = off_mbar + 24 * 8 + 64;   // 3 buffers x 8 chunk barriers, TMEM base address
+  static constexpr size_t off_red = off_mbar + 24 * 8;   // 3 buffers x 8 chunk barriers
   static constexpr size_t bytes = off_red + 4 * 32 * sizeof(float);
 };
 
-// ---- tensor memory as an accumulator file: 32 consecutive columns of the calling thread's TMEM lane
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
+// ---- column-sum cells in global memory, kept in L2 across the rows a CTA adds into them
+__device__ __forceinline__ uint64_t l2_evict_last_policy() {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(pol));
+  return pol;
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float (&v)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-      "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-      "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-      "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-      "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-      "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-      "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-      "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-      : "memory");
-  asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
+__device__ __forceinline__ float ld_l2_keep(const float* a, uint64_t pol) {
+  float v;
+  asm volatile("ld.global.L2::cache_hint.f32 %0, [%1], %2;" : "=f"(v) : "l"(a), "l"(pol));
+  return v;
+}
+__device__ __forceinline__ void st_l2_keep(float* a, float v, uint64_t pol) {
+  asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(a), "f"(v), "l"(pol) : "memory");
 }
 
 // a[i] *= w^i, i = 1..15 (powers at most four multiplications deep)
@@ -144,32 +127,21 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
   float2* const T1 = T0 + B1;
   float2* const T2 = T1 + 15 * B2;
   uint64_t* const mbar = reinterpret_cast<uint64_t*>(smraw + C::off_mbar);  // [3 buffers][8 chunks]
-  uint32_t* const tmem_base_s = reinterpret_cast<uint32_t*>(smraw + C::off_mbar + 24 * 8);
   float* const red = reinterpret_cast<float*>(smraw + C::off_red);  // [2 slots][s2 | s4][32]
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
 
   for (int i = tid; i < C::TABN; i += NT) T0[i] = __ldg(&tabs[i]);
   if (tid < 24) mbar_init(&mbar[tid], 1);
   if (tid == 0) fence_mbar_init();
-  uint32_t my_tmem = 0;
-  if constexpr (SK) {
-    if (wid == 0) {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_base_s)),
-                   "n"(C::TMEM_COLS));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-  }
   __syncthreads();
-  if constexpr (SK) {
-    asm volatile("tcgen05.fence::after_thread_sync;");
-    // this thread's 32 column-sum cells: lane `lane` of quadrant wid & 3, columns 32 (wid >> 2) .. + 31
-    my_tmem = *tmem_base_s + ((uint32_t)(32 * (wid & 3)) << 16) + (uint32_t)((wid >> 2) * 32);
-    float z[32];
-#pragma unroll
-    for (int i = 0; i < 32; i++) z[i] = 0.f;
-    tmem_st32(my_tmem, z);
-  }
+  // this thread's 32 column-sum cells: time samples kcell + 256 (c >> 1) + 4096 (c & 1) of the CTA's partial row,
+  // natural order; cells past ts_count are dropped. Only this thread ever touches them.
+  const int kcell = (lane & 15) + 16 * (((wid & 7) << 1) | (lane >> 4)) + 8192 * (wid >> 3);
+  float* const cells = skp.partial + (size_t)blockIdx.x * skp.ts_count + kcell;
+  auto cell_live = [&](int c) { return (unsigned)(kcell + 256 * (c >> 1) + 4096 * (c & 1)) < skp.ts_count; };
+  auto cell = [&](int c) { return cells + 256 * (c >> 1) + 4096 * (c & 1); };
+  uint64_t keep_pol = 0;
+  if constexpr (SK) keep_pol = l2_evict_last_policy();
 
   // warp 0, lanes 0..7: fetch half a row (chunks d0 = 8 which .. 8 which + 7) into half buffer hb, one bulk copy per
   // chunk, each signalled on its own mbarrier
@@ -189,7 +161,12 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
   };
   if (blockIdx.x < nrows) prefetch_phase(blockIdx.x);  // the table is a constant of the run: no dependency to wait for
   pdl_launch_dependents();
-  pdl_wait();  // tables, barriers and tensor memory were set up while the preceding kernel drained
+  pdl_wait();  // tables and barriers were set up while the preceding kernel drained
+  if constexpr (SK) {
+#pragma unroll
+    for (int c = 0; c < 32; c++)
+      if (cell_live(c)) st_l2_keep(cell(c), 0.f, keep_pol);
+  }
   float limit = 0.f;
   if constexpr (CHIRP) limit = cp.threshold * __ldg(cp.mean);
 
@@ -336,7 +313,11 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
       }
     }
     bool zap = false;
+    float acc[SK ? 32 : 1];
     if constexpr (SK) {
+      // the row's column sums are fetched now, so that L2 latency overlaps the SK reduction below
+#pragma unroll
+      for (int c = 0; c < 32; c++) acc[c] = cell_live(c) ? ld_l2_keep(cell(c), keep_pol) : 0.f;
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
         s2 += __shfl_xor_sync(0xffffffffu, s2, o);
@@ -376,8 +357,6 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
           o[256 * i2 + 4096] = make_float2(0.f, 0.f);
         }
       } else {
-        float acc[SK ? 32 : 1];
-        if constexpr (SK) tmem_ld32(my_tmem, acc);
 #pragma unroll
         for (int i2 = 0; i2 < 16; i2++) {
           const float4 q = *reinterpret_cast<const float4*>(base + i2 * R3);
@@ -388,7 +367,11 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
             acc[2 * i2 + 1] += q.z * q.z + q.w * q.w;
           }
         }
-        if constexpr (SK) tmem_st32(my_tmem, acc);
+        if constexpr (SK) {
+#pragma unroll
+          for (int c = 0; c < 32; c++)
+            if (cell_live(c)) st_l2_keep(cell(c), acc[c], keep_pol);
+        }
       }
     }
     __syncthreads();  // the row's buffers are free: second half of the next row, first half of the one after
@@ -397,22 +380,6 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
       if (nxt < nrows) issue_half(nxt, 1, hA);     // B of row it + 1 is A of row it
       if (nxt2 < nrows) issue_half(nxt2, 0, hB);   // A of row it + 2 is B of row it
     }
-  }
-  if constexpr (SK) {
-    // column sums of the surviving rows this CTA transformed: one partial row per CTA, natural order
-    float acc[32];
-    tmem_ld32(my_tmem, acc);
-    const int pd0 = lane & 15, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
-    float* const dst = skp.partial + (size_t)blockIdx.x * skp.ts_count;
-#pragma unroll
-    for (int c = 0; c < 32; c++) {
-      const unsigned k = (unsigned)(pd0 + 16 * pd1 + 256 * (c >> 1) + 4096 * (2 * sel + (c & 1)));
-      if (k < skp.ts_count) dst[k] = acc[c];
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;");
-    __syncthreads();
-    if (wid == 0)
-      asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(*tmem_base_s), "n"(C::TMEM_COLS));
   }
 }
 

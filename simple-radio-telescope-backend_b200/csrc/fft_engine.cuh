@@ -1,4 +1,4 @@
-// fft_engine.cuh — hand-written sm_100a FFT passes (no cuFFT on the hot path).
+// fft_engine.cuh — hand-written sm_90a FFT passes (no cuFFT on the hot path).
 //
 // Replaces the vendor-FFT call sites of the reference:
 //   R2C  : userspace/include/srtb/fft/cufft_like_wrapper.hpp:183-191 (cufftExecR2C)
@@ -470,7 +470,7 @@ struct trans_io {
 // TMA (cp.async.bulk) + mbarrier helpers
 // ---------------------------------------------------------------------------------
 // programmatic dependent launch (griddepcontrol): a kernel launched with the stream-serialisation attribute may start
-// while its predecessor drains; everything it does before pdl_wait() (shared-memory tables, barrier and TMEM set-up)
+// while its predecessor drains; everything it does before pdl_wait() (shared-memory tables, barrier set-up)
 // overlaps the predecessor's tail, everything after sees the predecessor's results. No-ops in a normal launch.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

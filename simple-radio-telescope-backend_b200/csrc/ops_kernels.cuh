@@ -1,4 +1,4 @@
-// ops_kernels.cuh — the non-FFT kernels of the path, hand-written for sm_100a.
+// ops_kernels.cuh — the non-FFT kernels of the path, hand-written for sm_90a.
 // All are HBM-bound streaming kernels: 16-byte vector accesses, fully coalesced,
 // grid sized as a multiple of the SM count, reductions by warp shuffles.
 // Reference operators are cited per kernel (S/ = userspace/include/srtb/).

@@ -33,7 +33,7 @@ struct srtb_b200_ctx {
   std::recursive_mutex mu;
   int device = 0;
   cudaStream_t stream = nullptr;
-  int sm_count = 148;
+  int sm_count = 132;
   std::string err;
   uint64_t launches = 0;
   std::set<const void*> configured;  // kernels whose smem attribute is set on this device
@@ -230,7 +230,7 @@ struct stage_scope {
 
 extern "C" {
 
-const char* srtb_b200_version(void) { return "srtb_b200 0.1 (sm_100a)"; }
+const char* srtb_b200_version(void) { return "srtb_b200 0.1 (sm_90a)"; }
 
 int srtb_b200_ctx_create(int device, void* cuda_stream, srtb_b200_ctx** out) {
   srtb_b200_ctx* ctx = nullptr;
@@ -649,11 +649,11 @@ static bool make_tensor_map(tensor_map_blob* out, const void* base, int rank, co
   return true;
 }
 
-// Programmatic dependent launch along the block path: each kernel's set-up (tables into shared memory, barriers, tensor
-// memory) overlaps its predecessor's tail; every such kernel calls pdl_wait() before touching anything a predecessor
-// produces. Measured (profiles/r02_pdl.md): +4 % on 2^24-sample blocks, whose kernels last 20-60 us, and -1..-4 % on
-// 2^26-sample blocks, where the early-resident CTAs of the next kernel only take shared memory from the running one.
-// Hence: on for blocks up to 2^25 samples, off above; SRTB_B200_PDL=0 / 1 forces it.
+// Programmatic dependent launch along the block path: each kernel's set-up (tables into shared memory, barriers) overlaps
+// its predecessor's tail; every such kernel calls pdl_wait() before touching anything a predecessor produces. It pays
+// where kernels are short (2^24-sample blocks) and can cost where they are long, since the
+// early-resident CTAs of the next kernel only take shared memory from the running one. Hence: on for blocks up to 2^25
+// samples, off above; SRTB_B200_PDL=0 / 1 forces it.
 static bool use_pdl(const srtb_b200_ctx* ctx) {
   static const int forced = [] {
     const char* e = std::getenv("SRTB_B200_PDL");
@@ -2207,8 +2207,8 @@ static int block_enqueue(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, 
       constexpr double D = 4.148808e3;
       row_chirp_params cp{(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)cfg->dm,
                           ctx->mean, cfg->mitigate_rfi_average_method_threshold, coef, 0};
-      // (no phase table here: the long-row column sweep is DRAM-bound and the 4 extra bytes per bin cost more than
-      // the fp64 evaluation they would replace — measured 74 against 77 Gsamples/s at 2^29 bins)
+      // (no phase table here: the long-row column sweep is DRAM-bound, and the 4 extra bytes per bin a table costs
+      // outweigh the fp64 evaluation it would replace)
       const int rc = watfft_long_fused(ctx, s, reinterpret_cast<float2*>(buf), reinterpret_cast<const float2*>(buf), L, batch,
                                        reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                        cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,

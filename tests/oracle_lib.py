@@ -94,6 +94,8 @@ class Oracle:
         L.srtb_oracle_signal_detect.argtypes = [P, SZ, SZ, SZ, F, F, SZ, C.POINTER(DetectResult), P]
         L.srtb_oracle_chain.argtypes = [P, C.POINTER(ChainConfig), P, C.POINTER(DetectResult), P, P]
         L.srtb_oracle_num_threads.restype = I
+        L.srtb_oracle_count_signal.restype = C.c_uint64
+        L.srtb_oracle_count_signal.argtypes = [P, SZ, F]
 
     # ---- unpack
     def window(self, window, i, n):
@@ -242,6 +244,10 @@ class Oracle:
                                         series.ctypes.data, stage_s.ctypes.data)
         assert rc == 0
         return work, res, series, stage_s
+
+    def count_signal(self, v, snr):
+        v = np.ascontiguousarray(v, dtype=np.float32)
+        return int(self.lib.srtb_oracle_count_signal(v.ctypes.data, v.size, snr))
 
     def set_threads(self, n: int):
         self.lib.srtb_oracle_set_threads(int(n))

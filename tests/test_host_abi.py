@@ -26,16 +26,16 @@ def test_library_exports_every_declared_symbol():
     exported = set(re.findall(r"\bT (srtb_b200_[a-z0-9_]+)", out))
     assert set(names) <= exported, sorted(set(names) - exported)
     assert set(names) == set(srtb_b200.SYMBOLS), "python binding and header disagree"
-    assert b"sm_100a" in lib.srtb_b200_version()
+    assert b"sm_90a" in lib.srtb_b200_version()
 
 
-def test_library_is_sm100a_only():
+def test_library_is_sm90a_only():
     import srtb_b200
     r = subprocess.run(["cuobjdump", "-lelf", str(srtb_b200.LIB_PATH)], capture_output=True, text=True)
     if r.returncode != 0:
         pytest.skip("cuobjdump unavailable")
     archs = set(re.findall(r"sm_\d+a?", r.stdout))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
 def test_no_cpu_fallback():
@@ -94,10 +94,9 @@ def test_cpp_host_next(tmp_path):
     import numpy as np
     d = ROOT / "tests" / "cpp"
     subprocess.run(["make", "-C", str(d), "test_host_next"], check=True, capture_output=True)
-    # with the reference tree at hand its two shipped .cfg files are parsed verbatim (they cannot travel to the GPU box)
-    ref = Path("/root/reference/userspace")
-    extra = [str(ref)] if (ref / "srtb_config.cfg").exists() and (ref / "srtb_config_1644-4559.cfg").exists() else []
-    r = subprocess.run([str(d / "test_host_next"), str(tmp_path), *extra], capture_output=True, text=True, timeout=120,
+    # the original project's two shipped .cfg files, stored verbatim under tests/golden, are parsed as they stand
+    r = subprocess.run([str(d / "test_host_next"), str(tmp_path), str(ROOT / "tests" / "golden")], capture_output=True,
+                       text=True, timeout=120,
                        env={"SRTB_LOG_LEVEL": "1", "PATH": "/usr/bin:/bin"})
     assert r.returncode == 0 and "host next ok" in r.stdout, r.stderr[-2000:]
     a = np.load(tmp_path / "srtb_test.npy")
