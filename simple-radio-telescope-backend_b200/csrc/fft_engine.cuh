@@ -833,11 +833,8 @@ __device__ __forceinline__ void stage_compute16_row(float2 (&v)[16], int u, cons
   }
 }
 
-#ifndef SRTB_ROW16_CHIRP_MIN_BLOCKS
-#define SRTB_ROW16_CHIRP_MIN_BLOCKS 3
-#endif
 template <int LOGL, int T, bool FWD, bool SK = false, bool CHIRP = false>
-__global__ void __launch_bounds__(((1 << LOGL) / 16) * T, CHIRP ? SRTB_ROW16_CHIRP_MIN_BLOCKS : 3)
+__global__ void __launch_bounds__(((1 << LOGL) / 16) * T, 3)
     fft_row16_tma_kernel(const float2* __restrict__ in, float2* __restrict__ out, size_t nrows,
                          const float2* __restrict__ tw, row_sk_params skp, row_chirp_params cp) {
   using SC = sched16<LOGL>;

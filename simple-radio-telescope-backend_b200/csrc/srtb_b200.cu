@@ -26,22 +26,11 @@ using namespace srtb_b200;
 
 static thread_local std::string g_last_error;
 
-struct srtb_b200_ctx {
-  // a context may be shared by the threads of a pipeline (the reference hands one sycl::queue to every pipe): every
-  // C-ABI entry takes this lock, so the planning state below (tables, scratch sizes, kernel attributes) is never
-  // mutated concurrently. Recursive because the block entries call the stage entries.
-  std::recursive_mutex mu;
-  int device = 0;
+// what one chain of kernels writes through: the data streams of a block are independent until their result headers
+// are read back, so a context runs the odd-numbered ones on a second lane with its own CUDA stream and scratch (one
+// lane's kernel tails and small detector kernels overlap the other lane's FFT sweeps)
+struct lane_state {
   cudaStream_t stream = nullptr;
-  int sm_count = 132;
-  std::string err;
-  uint64_t launches = 0;
-  std::set<const void*> configured;  // kernels whose smem attribute is set on this device
-  std::map<const void*, int> occupancy;  // resident CTAs per SM of the persistent kernels
-  // FFT
-  float2* tw[13] = {nullptr};
-  std::map<int, float2*> bigtw;  // log2(n_i) -> [3 << q]
-  float2* bigrow_tab[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [logl - 13][forward] whole-row kernel tables
   void* fft_scratch = nullptr;
   size_t fft_scratch_bytes = 0;
   // s1
@@ -49,13 +38,42 @@ struct srtb_b200_ctx {
   unsigned* ticket = nullptr;
   unsigned* detect_ticket = nullptr;  // last-CTA ticket of the detector's column-sum kernel
   float* mean = nullptr;
-  // detect (slots = streams in flight)
+  // detect
   float* colsum_partial = nullptr;
   size_t colsum_partial_elems = 0;
-  float* series[4] = {nullptr, nullptr, nullptr, nullptr};
-  size_t series_elems = 0;
   float* acc = nullptr;
   size_t acc_elems = 0;
+  // long waterfall rows: per-tile SK statistics of the last sweep, per-row zap flags
+  void* long_stats = nullptr;
+  size_t long_stats_bytes = 0;
+  void* long_zap = nullptr;
+  size_t long_zap_bytes = 0;
+};
+
+struct srtb_b200_ctx {
+  // a context may be shared by the threads of a pipeline (the reference hands one sycl::queue to every pipe): every
+  // C-ABI entry takes this lock, so the planning state below (tables, scratch sizes, kernel attributes) is never
+  // mutated concurrently. Recursive because the block entries call the stage entries.
+  std::recursive_mutex mu;
+  int device = 0;
+  int sm_count = 132;
+  std::string err;
+  uint64_t launches = 0;
+  std::set<const void*> configured;  // kernels whose smem attribute is set on this device
+  std::map<const void*, int> occupancy;  // resident CTAs per SM of the persistent kernels
+  // the lane the launch code writes through, and the other one. lane_swap() exchanges them, so the launch code itself
+  // is lane-agnostic. The first lane's stream is the caller's; the second lane (created on first use) owns its stream.
+  lane_state lane, alt;
+  bool alt_ready = false, on_alt = false;
+  int lanes = 1;  // SRTB_B200_LANES (default 2): CUDA streams per context the data streams of a block are spread over
+  cudaEvent_t lane_fork = nullptr, lane_join = nullptr;
+  // FFT
+  float2* tw[13] = {nullptr};
+  std::map<int, float2*> bigtw;  // log2(n_i) -> [3 << q]
+  float2* bigrow_tab[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [logl - 13][forward] whole-row kernel tables
+  // detect (slots = streams in flight)
+  float* series[4] = {nullptr, nullptr, nullptr, nullptr};
+  size_t series_elems = 0;
   detect_dev_result* d_res = nullptr;
   detect_dev_result* h_res = nullptr;  // pinned, 4 slots
   size_t slot_time_count[4] = {0, 0, 0, 0};
@@ -65,7 +83,6 @@ struct srtb_b200_ctx {
   size_t slot_baseband_bytes[SRTB_B200_RING_SLOTS] = {0};
   cudaEvent_t slot_h2d[SRTB_B200_RING_SLOTS] = {nullptr}, slot_done[SRTB_B200_RING_SLOTS] = {nullptr};
   int slot_streams[SRTB_B200_RING_SLOTS] = {0};
-  size_t slot_L[SRTB_B200_RING_SLOTS] = {0};
   bool slot_busy[SRTB_B200_RING_SLOTS] = {false};
   cudaEvent_t slot_done_alt[SRTB_B200_RING_SLOTS] = {nullptr};  // second lane's completion of the slot's block
   bool slot_alt_used[SRTB_B200_RING_SLOTS] = {false};
@@ -83,11 +100,6 @@ struct srtb_b200_ctx {
   size_t sweep_buf_bytes = 0;
   void* sweep_res = nullptr;
   size_t sweep_res_bytes = 0;
-  // long waterfall rows: per-tile SK statistics of the last sweep, per-row zap flags
-  void* long_stats = nullptr;
-  size_t long_stats_bytes = 0;
-  void* long_zap = nullptr;
-  size_t long_zap_bytes = 0;
   // optional per-stage timing (srtb_b200_stage_stats)
   bool stats_on = false;
   cudaEvent_t stat_ev[SRTB_B200_STAGE_COUNT][2] = {};
@@ -106,50 +118,35 @@ struct srtb_b200_ctx {
   float* chirp_tab = nullptr;
   size_t chirp_tab_bytes = 0;
   double chirp_tab_key[6] = {0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm
-  // second lane: the data streams of one block are independent until their result headers are read back, so the
-  // odd-numbered ones run on a second CUDA stream of this context with their own scratch (one lane's kernel tails and
-  // small detector kernels overlap the other lane's FFT sweeps). lane_swap() exchanges every member a stream's chain
-  // writes through with the copy kept here, so the launch code itself is lane-agnostic.
-  struct lane_state {
-    cudaStream_t stream = nullptr;
-    void* fft_scratch = nullptr;
-    size_t fft_scratch_bytes = 0;
-    double* partial = nullptr;
-    unsigned* ticket = nullptr;
-    unsigned* detect_ticket = nullptr;
-    float* mean = nullptr;
-    float* colsum_partial = nullptr;
-    size_t colsum_partial_elems = 0;
-    float* acc = nullptr;
-    size_t acc_elems = 0;
-    void* long_stats = nullptr;
-    size_t long_stats_bytes = 0;
-    void* long_zap = nullptr;
-    size_t long_zap_bytes = 0;
-  } alt;
-  bool alt_ready = false, on_alt = false;
-  int lanes = 1;  // SRTB_B200_LANES (default 2): CUDA streams per context the data streams of a block are spread over
-  cudaEvent_t lane_fork = nullptr, lane_join = nullptr;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
-  auto& a = ctx->alt;
-  std::swap(ctx->stream, a.stream);
-  std::swap(ctx->fft_scratch, a.fft_scratch);
-  std::swap(ctx->fft_scratch_bytes, a.fft_scratch_bytes);
-  std::swap(ctx->partial, a.partial);
-  std::swap(ctx->ticket, a.ticket);
-  std::swap(ctx->detect_ticket, a.detect_ticket);
-  std::swap(ctx->mean, a.mean);
-  std::swap(ctx->colsum_partial, a.colsum_partial);
-  std::swap(ctx->colsum_partial_elems, a.colsum_partial_elems);
-  std::swap(ctx->acc, a.acc);
-  std::swap(ctx->acc_elems, a.acc_elems);
-  std::swap(ctx->long_stats, a.long_stats);
-  std::swap(ctx->long_stats_bytes, a.long_stats_bytes);
-  std::swap(ctx->long_zap, a.long_zap);
-  std::swap(ctx->long_zap_bytes, a.long_zap_bytes);
+  std::swap(ctx->lane, ctx->alt);
   ctx->on_alt = !ctx->on_alt;
+}
+
+// the fixed-size device state of a lane (its stream is set by the caller)
+static cudaError_t lane_alloc(lane_state* l) {
+  cudaError_t e = cudaMalloc(&l->partial, sizeof(double) * 4096);
+  if (e == cudaSuccess) e = cudaMalloc(&l->ticket, sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMemset(l->ticket, 0, sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMalloc(&l->detect_ticket, sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMemset(l->detect_ticket, 0, sizeof(unsigned));
+  if (e == cudaSuccess) e = cudaMalloc(&l->mean, sizeof(float));
+  return e;
+}
+
+// every device buffer of a lane; not its stream
+static void lane_free(lane_state* l) {
+  cudaFree(l->fft_scratch);
+  cudaFree(l->partial);
+  cudaFree(l->ticket);
+  cudaFree(l->detect_ticket);
+  cudaFree(l->mean);
+  cudaFree(l->colsum_partial);
+  cudaFree(l->acc);
+  cudaFree(l->long_stats);
+  cudaFree(l->long_zap);
 }
 
 #define API_LOCK(c)                                         \
@@ -173,7 +170,7 @@ static int fail(srtb_b200_ctx* ctx, int code, const std::string& msg) {
 
 // both lanes of the context idle (before anything either of them may still use is freed)
 static int sync_lanes(srtb_b200_ctx* ctx) {
-  CK(cudaStreamSynchronize(ctx->stream));
+  CK(cudaStreamSynchronize(ctx->lane.stream));
   if (ctx->alt_ready) CK(cudaStreamSynchronize(ctx->alt.stream));
   return 0;
 }
@@ -191,6 +188,14 @@ static int ensure(srtb_b200_ctx* ctx, void** p, size_t* have, size_t want_bytes)
     return fail(ctx, SRTB_B200_E_NOMEM, std::string("cudaMalloc(") + std::to_string(want_bytes) +
                                             "): " + cudaGetErrorString(e));
   *have = want_bytes;
+  return 0;
+}
+
+// the lane's partial column sums of the detector, grown to at least `elems` floats
+static int ensure_colsum_partial(srtb_b200_ctx* ctx, size_t elems) {
+  size_t have = ctx->lane.colsum_partial_elems * sizeof(float);
+  if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->lane.colsum_partial), &have, elems * sizeof(float))) return rc;
+  ctx->lane.colsum_partial_elems = have / sizeof(float);
   return 0;
 }
 
@@ -221,10 +226,10 @@ struct stage_scope {
     }
     ctx->stat_bytes[stage] = bytes;
     ctx->stat_have[stage] = true;
-    cudaEventRecord(ctx->stat_ev[stage][0], ctx->stream);
+    cudaEventRecord(ctx->stat_ev[stage][0], ctx->lane.stream);
   }
   ~stage_scope() {
-    if (ctx) cudaEventRecord(ctx->stat_ev[stage][1], ctx->stream);
+    if (ctx) cudaEventRecord(ctx->stat_ev[stage][1], ctx->lane.stream);
   }
 };
 
@@ -244,15 +249,10 @@ int srtb_b200_ctx_create(int device, void* cuda_stream, srtb_b200_ctx** out) {
   if (device < 0 || device >= count) return fail(nullptr, SRTB_B200_E_INVALID, "ctx_create: bad device index");
   ctx = new srtb_b200_ctx();
   ctx->device = device;
-  ctx->stream = static_cast<cudaStream_t>(cuda_stream);
+  ctx->lane.stream = static_cast<cudaStream_t>(cuda_stream);
   e = cudaSetDevice(device);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device);
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->partial, sizeof(double) * 4096);
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->ticket, sizeof(unsigned));
-  if (e == cudaSuccess) e = cudaMemset(ctx->ticket, 0, sizeof(unsigned));
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->detect_ticket, sizeof(unsigned));
-  if (e == cudaSuccess) e = cudaMemset(ctx->detect_ticket, 0, sizeof(unsigned));
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->mean, sizeof(float));
+  if (e == cudaSuccess) e = lane_alloc(&ctx->lane);
   if (e == cudaSuccess) e = cudaMalloc(&ctx->d_res, sizeof(detect_dev_result) * 4);
   if (e == cudaSuccess) e = cudaMemset(ctx->d_res, 0, sizeof(detect_dev_result) * 4);
   if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_res, sizeof(detect_dev_result) * 4 * (1 + SRTB_B200_RING_SLOTS));
@@ -271,20 +271,13 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   if (!ctx) return 0;
   cudaSetDevice(ctx->device);
   if (ctx->on_alt) lane_swap(ctx);
-  cudaStreamSynchronize(ctx->stream);
+  cudaStreamSynchronize(ctx->lane.stream);
   if (ctx->alt_ready) {
     cudaStreamSynchronize(ctx->alt.stream);
-    cudaFree(ctx->alt.fft_scratch);
-    cudaFree(ctx->alt.partial);
-    cudaFree(ctx->alt.ticket);
-    cudaFree(ctx->alt.detect_ticket);
-    cudaFree(ctx->alt.mean);
-    cudaFree(ctx->alt.colsum_partial);
-    cudaFree(ctx->alt.acc);
-    cudaFree(ctx->alt.long_stats);
-    cudaFree(ctx->alt.long_zap);
     cudaStreamDestroy(ctx->alt.stream);
   }
+  lane_free(&ctx->lane);
+  lane_free(&ctx->alt);
   if (ctx->lane_fork) cudaEventDestroy(ctx->lane_fork);
   if (ctx->lane_join) cudaEventDestroy(ctx->lane_join);
   for (auto& p : ctx->tw)
@@ -292,21 +285,12 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   for (auto& kv : ctx->bigtw) cudaFree(kv.second);
   for (auto& a : ctx->bigrow_tab)
     for (auto& p : a) cudaFree(p);
-  cudaFree(ctx->fft_scratch);
-  cudaFree(ctx->partial);
-  cudaFree(ctx->ticket);
-  cudaFree(ctx->detect_ticket);
-  cudaFree(ctx->mean);
-  cudaFree(ctx->colsum_partial);
   for (auto& p : ctx->series) cudaFree(p);
-  cudaFree(ctx->acc);
   cudaFree(ctx->d_res);
   cudaFreeHost(ctx->h_res);
   cudaFree(ctx->d_baseband);
   cudaFree(ctx->sweep_buf);
   cudaFree(ctx->sweep_res);
-  cudaFree(ctx->long_stats);
-  cudaFree(ctx->long_zap);
   cudaFree(ctx->chirp_tab);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
     cudaFree(ctx->slot_baseband[i]);
@@ -328,7 +312,7 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
 int srtb_b200_ctx_set_stream(srtb_b200_ctx* ctx, void* cuda_stream) {
   API_LOCK(ctx);
   if (!ctx) return fail(nullptr, SRTB_B200_E_INVALID, "set_stream: ctx is null");
-  ctx->stream = static_cast<cudaStream_t>(cuda_stream);
+  ctx->lane.stream = static_cast<cudaStream_t>(cuda_stream);
   return 0;
 }
 
@@ -337,8 +321,8 @@ int srtb_b200_synchronize(srtb_b200_ctx* ctx) {
   cudaStream_t s0, s1 = nullptr;
   {
     API_LOCK(ctx);  // the wait itself runs unlocked: other threads keep enqueueing meanwhile
-    s0 = ctx->on_alt ? ctx->alt.stream : ctx->stream;
-    if (ctx->alt_ready) s1 = ctx->on_alt ? ctx->stream : ctx->alt.stream;
+    s0 = ctx->on_alt ? ctx->alt.stream : ctx->lane.stream;
+    if (ctx->alt_ready) s1 = ctx->on_alt ? ctx->lane.stream : ctx->alt.stream;
   }
   CK(cudaStreamSynchronize(s0));
   if (s1) CK(cudaStreamSynchronize(s1));
@@ -382,11 +366,11 @@ static int launch_unpack_simple(srtb_b200_ctx* ctx, const void* d_in, float* out
   const bool aligned = ((reinterpret_cast<uintptr_t>(d_in) & 15u) == 0) &&
                        ((reinterpret_cast<uintptr_t>(out) & 15u) == 0);
   if (!aligned) {
-    unpack_simple_scalar_kernel<BITS><<<grid_for(ctx, n, 256), 256, 0, ctx->stream>>>(d_in, out, n, window);
+    unpack_simple_scalar_kernel<BITS><<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(d_in, out, n, window);
   } else if (window == 0) {
-    unpack_simple_kernel<BITS, false><<<grid_for(ctx, n / 16 + 1, 256), 256, 0, ctx->stream>>>(d_in, out, n, window);
+    unpack_simple_kernel<BITS, false><<<grid_for(ctx, n / 16 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, out, n, window);
   } else {
-    unpack_simple_kernel<BITS, true><<<grid_for(ctx, n / 16 + 1, 256), 256, 0, ctx->stream>>>(d_in, out, n, window);
+    unpack_simple_kernel<BITS, true><<<grid_for(ctx, n / 16 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, out, n, window);
   }
   ctx->launches++;
   CK(cudaGetLastError());
@@ -395,7 +379,7 @@ static int launch_unpack_simple(srtb_b200_ctx* ctx, const void* d_in, float* out
 
 template <int BITS>
 static int launch_unpack_il2(srtb_b200_ctx* ctx, const void* d_in, float* o1, float* o2, size_t n, int window) {
-  unpack_interleaved2_kernel<BITS><<<grid_for(ctx, n / 4 + 1, 256), 256, 0, ctx->stream>>>(d_in, o1, o2, n, window);
+  unpack_interleaved2_kernel<BITS><<<grid_for(ctx, n / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, o1, o2, n, window);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -464,14 +448,14 @@ extern "C" int srtb_b200_unpack(srtb_b200_ctx* ctx, const void* d_in, size_t in_
     case SRTB_B200_FORMAT_NAOCPSR_SNAP1:
       if (bits != -8)
         return fail(ctx, SRTB_B200_E_UNSUPPORTED, "naocpsr_snap1 requires baseband_input_bits = -8");
-      unpack_snap1_kernel<<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->stream>>>(d_in, d_out[0], d_out[1], out_count, window);
+      unpack_snap1_kernel<<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, d_out[0], d_out[1], out_count, window);
       break;
     case SRTB_B200_FORMAT_GZNUPSR_A1_2:
-      unpack_gznupsr_kernel<2><<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->stream>>>(
+      unpack_gznupsr_kernel<2><<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(
           d_in, d_out[0], d_out[1], nullptr, nullptr, out_count, window);
       break;
     case SRTB_B200_FORMAT_GZNUPSR_A1_4:
-      unpack_gznupsr_kernel<4><<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->stream>>>(
+      unpack_gznupsr_kernel<4><<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(
           d_in, d_out[0], d_out[1], d_out[2], d_out[3], out_count, window);
       break;
   }
@@ -492,8 +476,8 @@ static int get_stage_twiddles(srtb_b200_ctx* ctx, int logl, const float2** out) 
       h[j] = make_float2((float)std::cos(a), (float)std::sin(a));
     }
     CK(cudaMalloc(&ctx->tw[logl], L * sizeof(float2)));
-    CK(cudaMemcpyAsync(ctx->tw[logl], h.data(), L * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaMemcpyAsync(ctx->tw[logl], h.data(), L * sizeof(float2), cudaMemcpyHostToDevice, ctx->lane.stream));
+    CK(cudaStreamSynchronize(ctx->lane.stream));
   }
   *out = ctx->tw[logl];
   return 0;
@@ -513,8 +497,8 @@ static int get_big_twiddles(srtb_b200_ctx* ctx, int logn, big_twiddle* out) {
       }
     float2* d = nullptr;
     CK(cudaMalloc(&d, h.size() * sizeof(float2)));
-    CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->lane.stream));
+    CK(cudaStreamSynchronize(ctx->lane.stream));
     it = ctx->bigtw.emplace(logn, d).first;
   }
   out->tab = it->second;
@@ -533,7 +517,7 @@ static int launch_pass(srtb_b200_ctx* ctx, const IO& io, unsigned grid, size_t e
   }
   const float2* tw = nullptr;
   if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-  kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->stream>>>(io, tw);
+  kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(io, tw);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -544,23 +528,12 @@ template <int LOGL>
 struct row_t {
   static constexpr int value = (LOGL >= 11) ? 1 : (1 << (11 - LOGL));
 };
-#ifndef SRTB_COL_T
-#define SRTB_COL_T 16
-#endif
 template <int LOGL>
 struct col_t {
-  static constexpr int value = (LOGL <= 8) ? SRTB_COL_T : ((SRTB_COL_T < 8) ? SRTB_COL_T : 8);
+  static constexpr int value = (LOGL <= 8) ? 16 : 8;
 };
 
-// sixteen-points-per-thread row kernels (L = 256, 1024, 2048, 4096); SRTB_B200_ROW16=0 selects the
-// eight-point kernels (A/B measurements)
-static bool use_row16() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_ROW16");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
+// sixteen-points-per-thread row kernels (L = 256 .. 4096); shorter rows take the eight-point kernel
 template <int LOGL>
 struct has_row16 {
   static constexpr bool value = (LOGL >= 8 && LOGL <= 12);
@@ -570,7 +543,7 @@ template <int LOGL, bool FWD>
 static int launch_row(srtb_b200_ctx* ctx, const float2* in, float2* out, size_t nrows) {
   constexpr int T = row_t<LOGL>::value;
   if constexpr (has_row16<LOGL>::value) {
-    if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0 && use_row16()) {
+    if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0) {
       constexpr int T16 = row16_t<LOGL>::value, threads = ((1 << LOGL) / 16) * T16;
       auto kern = fft_row16_tma_kernel<LOGL, T16, FWD>;
       constexpr size_t smem = row16_smem<LOGL, T16>::bytes;
@@ -584,8 +557,7 @@ static int launch_row(srtb_b200_ctx* ctx, const float2* in, float2* out, size_t 
       CK(cudaGetLastError());
       return 0;
     }
-  }
-  if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0) {
+  } else if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0) {
     // persistent TMA-fed kernel (cp.async.bulk needs 16-byte aligned rows)
     auto kern = fft_row_tma_kernel<LOGL, T, FWD>;
     constexpr size_t smem = row_tma_smem<LOGL, T>::bytes;
@@ -601,7 +573,7 @@ static int launch_row(srtb_b200_ctx* ctx, const float2* in, float2* out, size_t 
     if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
     const size_t ntiles = (nrows + T - 1) / T;
     const unsigned grid = (unsigned)std::min<size_t>(ntiles, (size_t)ctx->sm_count * ctx->occupancy[key]);
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->stream>>>(in, out, nrows, tw, row_sk_params{});
+    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(in, out, nrows, tw, row_sk_params{});
     ctx->launches++;
     CK(cudaGetLastError());
     return 0;
@@ -653,26 +625,19 @@ static bool make_tensor_map(tensor_map_blob* out, const void* base, int rank, co
 // its predecessor's tail; every such kernel calls pdl_wait() before touching anything a predecessor produces. It pays
 // where kernels are short (2^24-sample blocks) and can cost where they are long, since the
 // early-resident CTAs of the next kernel only take shared memory from the running one. Hence: on for blocks up to 2^25
-// samples, off above; SRTB_B200_PDL=0 / 1 forces it.
-static bool use_pdl(const srtb_b200_ctx* ctx) {
-  static const int forced = [] {
-    const char* e = std::getenv("SRTB_B200_PDL");
-    return e ? (e[0] == '0' ? 0 : 1) : -1;
-  }();
-  return forced >= 0 ? forced == 1 : ctx->pdl_auto;
-}
+// samples, off above and outside a block.
 template <typename... KArgs, typename... Args>
 static cudaError_t launch_pdl(srtb_b200_ctx* ctx, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
-  cfg.stream = ctx->stream;
+  cfg.stream = ctx->lane.stream;
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = use_pdl(ctx) ? 1 : 0;
+  cfg.numAttrs = ctx->pdl_auto ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
@@ -693,36 +658,19 @@ static int persistent_grid(srtb_b200_ctx* ctx, K kern, int threads, size_t smem,
 }
 
 // three-sweep factorisation of 2^q: the first sweep takes ceil(q/3); of the rest the longer half goes to the
-// LAST sweep (2^23 = 2^8 * 2^7 * 2^8) so that the transposing pass runs as 16 x 16; SRTB_B200_PLAN_878=0
-// gives the longer half to the middle sweep instead (8, 8, 7)
-static bool plan_last_long() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_PLAN_878");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
-// SRTB_B200_PLAN_FIRST_SHORT=1: give the FIRST sweep the short factor (2^25 = 2^8 * 2^9 * 2^8 instead of 2^9 * 2^8 * 2^8):
-// the raw-byte first sweep then runs 256-point columns of 16 neighbours (64-byte raw segments for two streams)
-static bool plan_first_short() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_PLAN_FIRST_SHORT");
-    return e && e[0] == '1';
-  }();
-  return on;
-}
+// LAST sweep (2^23 = 2^8 * 2^7 * 2^8) so that the transposing pass runs as 16 x 16
 static void plan3(int q, int* l1, int* l2, int* l3) {
-  *l1 = plan_first_short() ? q / 3 : (q + 2) / 3;
+  *l1 = (q + 2) / 3;
   const int big = (q - *l1 + 1) / 2, small = q - *l1 - big;
   // the fused R2C last sweep exists up to L = 256: keep the last factor <= 8 when one of the two is
-  const bool last_big = plan_last_long() && big <= 8;
+  const bool last_big = big <= 8;
   *l2 = last_big ? small : big;
   *l3 = last_big ? big : small;
 }
 
 // 2^27 points and above: four sweeps of L <= 256 (all on the sixteen-point kernels, each near the HBM roofline)
 // beat three sweeps with 512/1024-point columns; the last factor is 7 or 8 so the fused R2C last sweep applies.
-// 27 = 7+7+6+7, 28 = 7+7+7+7, 29 = 7+7+7+8, 30 = 8+7+7+8. SRTB_B200_FOUR_SWEEPS=0 keeps three sweeps.
+// 27 = 7+7+6+7, 28 = 7+7+7+7, 29 = 7+7+7+8, 30 = 8+7+7+8. Unaligned data or no TMA keeps three sweeps.
 static void plan4(int q, int* l) {
   l[3] = (q >= 29) ? 8 : 7;
   int r = q - l[3];
@@ -730,35 +678,14 @@ static void plan4(int q, int* l) {
   l[1] = (r - l[0] + 1) / 2;
   l[2] = r - l[0] - l[1];
 }
-static bool use_col16();
-static encode_tiled_fn get_encode_tiled();
 static bool four_sweeps(int q, const void* ptr) {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_FOUR_SWEEPS");
-    return !(e && e[0] == '0');
-  }();
-  return on && q >= 27 && q <= 30 && use_col16() && get_encode_tiled() != nullptr &&
-         (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0;
-}
-
-// sixteen-points-per-thread column kernels (radix 16 x 16 / 16 x 8) for L = 256 / 128; SRTB_B200_COL16=0
-// selects the eight-point kernels instead (A/B measurements)
-static bool use_col16() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_COL16");
-    return !(e && e[0] == '0');
-  }();
-  return on;
+  return q >= 27 && q <= 30 && get_encode_tiled() != nullptr && (reinterpret_cast<uintptr_t>(ptr) & 15u) == 0;
 }
 
 // wide tiles (32 neighbouring columns = 256-byte segments) for the 128-point column sweep of very long transforms,
-// whose row stride is megabytes: fewer DRAM page openings / TLB entries per byte. SRTB_B200_WIDE_COL=0 disables.
+// whose row stride is megabytes: fewer DRAM page openings / TLB entries per byte
 static bool wide_col(size_t A, size_t L, size_t B) {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_WIDE_COL");
-    return !(e && e[0] == '0');
-  }();
-  return on && B >= ((size_t)1 << 14) && A * L * B >= ((size_t)1 << 26);
+  return B >= ((size_t)1 << 14) && A * L * B >= ((size_t)1 << 26);
 }
 
 template <int LOGL, bool FWD, int TT = col_t<LOGL>::value>
@@ -766,7 +693,7 @@ static int launch_col_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, siz
                           const row_chirp_params* chirp = nullptr) {
   constexpr int T = TT, L = 1 << LOGL;
   if constexpr (LOGL == 7 && TT == col_t<LOGL>::value) {
-    if (use_col16() && wide_col(A, L, B) && !chirp) return launch_col_tma<LOGL, FWD, 32>(ctx, in, out, A, B, done);
+    if (wide_col(A, L, B) && !chirp) return launch_col_tma<LOGL, FWD, 32>(ctx, in, out, A, B, done);
   }
   *done = false;
   if ((reinterpret_cast<uintptr_t>(in) & 15u) || A * L >= ((size_t)1 << 31) || B >= ((size_t)1 << 31)) return 0;
@@ -783,35 +710,30 @@ static int launch_col_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, siz
   const size_t ntiles = A * (B / T);
   unsigned grid = 1;
   if constexpr (LOGL >= 7 && LOGL <= 9) {
-    if (use_col16()) {
-      auto kern16 = fft_col16_tma_kernel<LOGL, T, FWD>;
-      constexpr int threads = col16_threads<LOGL, T>::value;
-      const size_t smem16 = col16_smem<LOGL, T, false>::bytes(btw.q);
-      if (int rc = persistent_grid(ctx, kern16, threads, smem16, col16_smem<LOGL, T, false>::bytes(10), ntiles, &grid)) return rc;
-      if constexpr (!FWD) {
-        if (chirp) {  // s1 + chirp applied as the tile is read (long waterfall rows)
-          auto kernc = fft_col16_tma_kernel<LOGL, T, FWD, 0, true>;
-          if (int rc = persistent_grid(ctx, kernc, threads, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-          CK(launch_pdl(ctx, kernc, dim3(grid), dim3(threads), smem, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
-                        raw_params{}, *chirp));
-          ctx->launches++;
-          CK(cudaGetLastError());
-          *done = true;
-          return 0;
-        }
+    auto kern16 = fft_col16_tma_kernel<LOGL, T, FWD>;
+    constexpr int threads = col16_threads<LOGL, T>::value;
+    const size_t smem16 = col16_smem<LOGL, T, false>::bytes(btw.q);
+    if (int rc = persistent_grid(ctx, kern16, threads, smem16, col16_smem<LOGL, T, false>::bytes(10), ntiles, &grid)) return rc;
+    if constexpr (!FWD) {
+      if (chirp) {  // s1 + chirp applied as the tile is read (long waterfall rows)
+        auto kernc = fft_col16_tma_kernel<LOGL, T, FWD, 0, true>;
+        if (int rc = persistent_grid(ctx, kernc, threads, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
+        CK(launch_pdl(ctx, kernc, dim3(grid), dim3(threads), smem, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
+                      raw_params{}, *chirp));
+        ctx->launches++;
+        CK(cudaGetLastError());
+        *done = true;
+        return 0;
       }
-      CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
-                    raw_params{}, row_chirp_params{}));
-      ctx->launches++;
-      CK(cudaGetLastError());
-      *done = true;
-      return 0;
     }
+    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
+                  raw_params{}, row_chirp_params{}));
+  } else {
+    if (chirp) return 0;  // the chirp-on-load sweep exists for the sixteen-point kernel only
+    auto kern = fft_col_tma_kernel<LOGL, T, FWD>;
+    if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
+    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, raw_params{});
   }
-  if (chirp) return 0;  // the chirp-on-load sweep exists for the sixteen-point kernel only
-  auto kern = fft_col_tma_kernel<LOGL, T, FWD>;
-  if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-  kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, raw_params{});
   ctx->launches++;
   CK(cudaGetLastError());
   *done = true;
@@ -831,7 +753,7 @@ template <int LOGL, int RAW, int TT = col_t<LOGL>::value>
 static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2* out, size_t B, bool* done) {
   constexpr int T = TT, L = 1 << LOGL;
   if constexpr (LOGL == 7 && TT == col_t<LOGL>::value) {
-    if (use_col16() && wide_col(1, L, B)) return launch_col_tma_raw<LOGL, RAW, 32>(ctx, src, out, B, done);
+    if (wide_col(1, L, B)) return launch_col_tma_raw<LOGL, RAW, 32>(ctx, src, out, B, done);
   }
   *done = false;
   if ((reinterpret_cast<uintptr_t>(src.base) & 15u) || B >= ((size_t)1 << 29)) return 0;
@@ -853,31 +775,24 @@ static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2*
   unsigned grid = 1;
   const raw_params rp{src.G, src.o0, src.o1, src.delta, (int)row_bytes, src.bits};
   if constexpr (LOGL >= 7 && LOGL <= 9) {
-    if (use_col16()) {
-      auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
-      constexpr int threads = col16_threads<LOGL, T>::value;
-      constexpr size_t smem16 = raw16_smem<LOGL, T>::bytes;  // inter-sweep tables stay in global memory here
-      if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
-      CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
-                    row_chirp_params{}));
-      ctx->launches++;
-      CK(cudaGetLastError());
-      *done = true;
-      return 0;
-    }
-  }
-  if constexpr (RAW == 3) {
+    auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
+    constexpr int threads = col16_threads<LOGL, T>::value;
+    constexpr size_t smem16 = raw16_smem<LOGL, T>::bytes;  // inter-sweep tables stay in global memory here
+    if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
+    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
+                  row_chirp_params{}));
+  } else if constexpr (RAW == 3) {
     return 0;  // packed samples: sixteen-point kernel only
   } else {
     if (src.delta) return 0;
     auto kern = fft_col_tma_kernel<LOGL, T, true, RAW>;
     if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp);
-    ctx->launches++;
-    CK(cudaGetLastError());
-    *done = true;
-    return 0;
+    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp);
   }
+  ctx->launches++;
+  CK(cudaGetLastError());
+  *done = true;
+  return 0;
 }
 
 static int dispatch_col_raw(srtb_b200_ctx* ctx, int logl, const raw_source& src, float2* out, size_t B, bool* done) {
@@ -913,31 +828,22 @@ static int launch_trans_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, s
   if (!make_tensor_map(&tm, in, 3, dims, strides, box)) return 0;
   const float2* tw = nullptr;
   if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-  if constexpr ((LOGL == 7 || LOGL == 8) && T == 16) {
-    if (use_col16()) {
-      auto kern16 = fft_trans16_tma_kernel<LOGL, T, FWD>;
-      constexpr int threads = T * (L / 16);
-      const size_t smem16 = tile_tma_smem<LOGL, T>::bytes(0);
-      const size_t k1tiles16 = L1 / T, ntiles16 = batch * S * k1tiles16;
-      unsigned grid16 = 1;
-      if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles16, &grid16)) return rc;
-      kern16<<<grid16, threads, smem16, ctx->stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
-                                                     (uint32_t)k1tiles16, (uint32_t)ntiles16, tw, (uint32_t)rest_inner,
-                                                     tile_stats);
-      ctx->launches++;
-      CK(cudaGetLastError());
-      *done = true;
-      return 0;
-    }
-  }
-  if (rest_inner > 1) return 0;  // only the sixteen-point kernel knows the four-sweep row order
-  auto kern = fft_trans_tma_kernel<LOGL, T, FWD>;
   const size_t smem = tile_tma_smem<LOGL, T>::bytes(0);
   const size_t k1tiles = L1 / T, ntiles = batch * S * k1tiles;
   unsigned grid = 1;
-  if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
-  kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
-                                                                  (uint32_t)k1tiles, (uint32_t)ntiles, tw, tile_stats);
+  if constexpr (LOGL == 7 || LOGL == 8) {
+    auto kern16 = fft_trans16_tma_kernel<LOGL, T, FWD>;
+    constexpr int threads = T * (L / 16);
+    if (int rc = persistent_grid(ctx, kern16, threads, smem, smem, ntiles, &grid)) return rc;
+    kern16<<<grid, threads, smem, ctx->lane.stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1, (uint32_t)k1tiles,
+                                                      (uint32_t)ntiles, tw, (uint32_t)rest_inner, tile_stats);
+  } else {
+    if (rest_inner > 1) return 0;  // only the sixteen-point kernel knows the four-sweep row order
+    auto kern = fft_trans_tma_kernel<LOGL, T, FWD>;
+    if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
+    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
+                                                                         (uint32_t)k1tiles, (uint32_t)ntiles, tw, tile_stats);
+  }
   ctx->launches++;
   CK(cudaGetLastError());
   *done = true;
@@ -1020,14 +926,7 @@ static int dispatch_trans(srtb_b200_ctx* ctx, int logl, const float2* in, float2
 }
 
 // ---- whole-row waterfall kernel (fft_bigrow.cuh): rows of 2^13 / 2^14 points held in one CTA's shared memory.
-// SRTB_B200_BIGROW=0 keeps the two-sweep column + transposing plan for these lengths (A/B measurements).
-static bool use_bigrow() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_BIGROW");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
+// Unaligned rows of these lengths take the two-sweep column + transposing plan.
 
 template <int LOGL>
 static int get_bigrow_tables(srtb_b200_ctx* ctx, bool fwd, const float2** out) {
@@ -1046,8 +945,8 @@ static int get_bigrow_tables(srtb_b200_ctx* ctx, bool fwd, const float2** out) {
     for (int i = 1; i < 16; i++)
       for (int j = 0; j < C::R3; j++) h[C::B1 + 15 * C::B2 + (i - 1) * C::R3 + j] = w(C::B2, (size_t)i * j);
     CK(cudaMalloc(&d, h.size() * sizeof(float2)));
-    CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->lane.stream));
+    CK(cudaStreamSynchronize(ctx->lane.stream));
   }
   *out = d;
   return 0;
@@ -1067,11 +966,8 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
     if (int rc = persistent_grid(ctx, kern, C::NT, smem, smem, nrows, &grid)) return rc;
     row_sk_params p{};
     if (with_sk) {
-      size_t have = ctx->colsum_partial_elems * sizeof(float);
-      if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->colsum_partial), &have, (size_t)grid * sk->ts_count * sizeof(float)))
-        return rc;
-      ctx->colsum_partial_elems = have / sizeof(float);
-      sk->partial = ctx->colsum_partial;
+      if (int rc = ensure_colsum_partial(ctx, (size_t)grid * sk->ts_count)) return rc;
+      sk->partial = ctx->lane.colsum_partial;
       p = *sk;
     }
     CK(launch_pdl(ctx, kern, dim3(grid), dim3(C::NT), smem, in, out, (unsigned)nrows, tabs, p, chirp ? *chirp : row_chirp_params{}));
@@ -1117,13 +1013,13 @@ static int fft_c2c_impl(srtb_b200_ctx* ctx, float2* x, size_t n, size_t batch) {
   const int q = ilog2(n);
   if (q == 0) return 0;
   if (q <= 2) {
-    tiny_fft_kernel<FWD><<<(unsigned)((batch + 255) / 256), 256, 0, ctx->stream>>>(x, q, batch);
+    tiny_fft_kernel<FWD><<<(unsigned)((batch + 255) / 256), 256, 0, ctx->lane.stream>>>(x, q, batch);
     ctx->launches++;
     CK(cudaGetLastError());
     return 0;
   }
   if (q <= 12) return dispatch_row<FWD>(ctx, q, x, x, batch);
-  if ((q == 13 || q == 14) && use_bigrow() && (reinterpret_cast<uintptr_t>(x) & 15u) == 0) {
+  if ((q == 13 || q == 14) && (reinterpret_cast<uintptr_t>(x) & 15u) == 0) {
     // one sweep: the whole row in shared memory (in place: a CTA reads its row completely before it stores it)
     return q == 13 ? launch_bigrow<13, FWD>(ctx, x, x, batch, nullptr, nullptr, nullptr)
                    : launch_bigrow<14, FWD>(ctx, x, x, batch, nullptr, nullptr, nullptr);
@@ -1131,8 +1027,8 @@ static int fft_c2c_impl(srtb_b200_ctx* ctx, float2* x, size_t n, size_t batch) {
   if (q > 30) return fail(ctx, SRTB_B200_E_SIZE, "fft: length above 2^30 not supported");
   if (batch * n > ((size_t)1 << 32) * 4)
     return fail(ctx, SRTB_B200_E_SIZE, "fft: batch * length too large");
-  if (int rc = ensure(ctx, &ctx->fft_scratch, &ctx->fft_scratch_bytes, batch * n * sizeof(float2))) return rc;
-  float2* s = static_cast<float2*>(ctx->fft_scratch);
+  if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, batch * n * sizeof(float2))) return rc;
+  float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
   if (q <= 20) {
     const int l1 = (q + 1) / 2, l2 = q - l1;
     const size_t L1 = (size_t)1 << l1, L2 = (size_t)1 << l2;
@@ -1196,19 +1092,10 @@ extern "C" int srtb_b200_fft_r2c_inplace(srtb_b200_ctx* ctx, float* d_inout, siz
     return fft_r2c_with_power_mean(ctx, d_inout, n_real);  // multi-sweep sizes: split fused into the last sweep
   float2* H = reinterpret_cast<float2*>(d_inout);
   if (int rc = fft_c2c_impl<true>(ctx, H, M, 1)) return rc;
-  r2c_post_kernel<false><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->stream>>>(H, M, nullptr, nullptr, nullptr);
+  r2c_post_kernel<false><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(H, M, nullptr, nullptr, nullptr);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
-}
-
-// SRTB_B200_TRANS16=0: eight-point fused last pass; SRTB_B200_PLAN_878=0: factor 2^23 as 8,8,7 instead of 8,7,8
-static bool use_trans16() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_TRANS16");
-    return !(e && e[0] == '0');
-  }();
-  return on;
 }
 
 // launch of the fused last pass + split (LOGL <= 8 keeps two [2T][L] tiles double-buffered in smem)
@@ -1229,26 +1116,21 @@ static int launch_trans_r2c(srtb_b200_ctx* ctx, const float2* in, float2* out, s
   constexpr size_t smem = trans_r2c_smem<LOGL, T>::bytes;
   const size_t tiles_per_rest = L1 / (2 * T) + 1, ntiles = S * tiles_per_rest;
   unsigned grid = 1;
-  bool launched = false;
   if constexpr (LOGL == 7 || LOGL == 8) {
-    if (use_trans16()) {
-      auto kern16 = fft_trans_r2c16_tma_kernel<LOGL, T>;
-      constexpr int threads = 2 * T * (L / 16);
-      if (int rc = persistent_grid(ctx, kern16, threads, smem, smem, ntiles, &grid)) return rc;
-      grid = std::min<unsigned>(grid, 2048);
-      CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem, tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
-                    (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw, ctx->partial, (uint32_t)rest_inner));
-      launched = true;
-    }
-  }
-  if (!launched && rest_inner > 1) return 0;  // four-sweep row order: sixteen-point kernel only
-  if (!launched) {
+    auto kern16 = fft_trans_r2c16_tma_kernel<LOGL, T>;
+    constexpr int threads = 2 * T * (L / 16);
+    if (int rc = persistent_grid(ctx, kern16, threads, smem, smem, ntiles, &grid)) return rc;
+    grid = std::min<unsigned>(grid, 2048);
+    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem, tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
+                  (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw, ctx->lane.partial, (uint32_t)rest_inner));
+  } else {
+    if (rest_inner > 1) return 0;  // four-sweep row order: sixteen-point kernel only
     auto kern = fft_trans_r2c_tma_kernel<LOGL, T>;
     if (int rc = persistent_grid(ctx, kern, 2 * pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
     grid = std::min<unsigned>(grid, 2048);
-    kern<<<grid, 2 * pass_threads<LOGL, T>::value, smem, ctx->stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
+    kern<<<grid, 2 * pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
                                                                         (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw,
-                                                                        ctx->partial);
+                                                                        ctx->lane.partial);
   }
   ctx->launches++;
   CK(cudaGetLastError());
@@ -1256,8 +1138,8 @@ static int launch_trans_r2c(srtb_b200_ctx* ctx, const float2* in, float2* out, s
     const size_t pairs = ((A << LOGL) / L1) / 2 + 1;
     const unsigned fgrid = (unsigned)std::min<size_t>((pairs + 255) / 256, 2048);
     if (grid + fgrid > 4096) return fail(ctx, SRTB_B200_E_SIZE, "r2c: partial buffer too small");
-    CK(launch_pdl(ctx, r2c_col0_fixup_kernel, dim3(fgrid), dim3(256), 0, out, (size_t)(A << LOGL), (size_t)L1, ctx->partial,
-                  (unsigned)grid, ctx->ticket, ctx->mean));
+    CK(launch_pdl(ctx, r2c_col0_fixup_kernel, dim3(fgrid), dim3(256), 0, out, (size_t)(A << LOGL), (size_t)L1, ctx->lane.partial,
+                  (unsigned)grid, ctx->lane.ticket, ctx->lane.mean));
   }
   ctx->launches++;
   CK(cudaGetLastError());
@@ -1265,7 +1147,7 @@ static int launch_trans_r2c(srtb_b200_ctx* ctx, const float2* in, float2* out, s
   return 0;
 }
 
-// R2C whose split pass also leaves mean(|X_k|^2, k < N/2) in ctx->mean (used by process_block:
+// R2C whose split pass also leaves mean(|X_k|^2, k < N/2) in ctx->lane.mean (used by process_block:
 // the s1 statistic costs no extra sweep). For multi-pass sizes the split is fused into the last FFT
 // pass (fft_trans_r2c_tma_kernel), so the packed transform costs P sweeps instead of P + 1.
 static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_real, const raw_source* raw,
@@ -1276,11 +1158,11 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
   const int q = ilog2(M);
   if (q >= 13 && q <= 30 && M >= 2) {
     // same factorisation as fft_c2c_impl
-    if (four_sweeps(q, d_inout) && use_trans16()) {
+    if (four_sweeps(q, d_inout)) {
       int l[4];
       plan4(q, l);
-      if (int rc = ensure(ctx, &ctx->fft_scratch, &ctx->fft_scratch_bytes, M * sizeof(float2))) return rc;
-      float2* s = static_cast<float2*>(ctx->fft_scratch);
+      if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, M * sizeof(float2))) return rc;
+      float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
       const size_t L1 = (size_t)1 << l[0], L2 = (size_t)1 << l[1], L3 = (size_t)1 << l[2], L4 = (size_t)1 << l[3];
       bool first_done = false;
       if (raw && raw->base) {
@@ -1308,8 +1190,8 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
     }
     const int llast = l3 ? l3 : l2;
     if (llast >= 6 && llast <= 8 && get_encode_tiled()) {
-      if (int rc = ensure(ctx, &ctx->fft_scratch, &ctx->fft_scratch_bytes, M * sizeof(float2))) return rc;
-      float2* s = static_cast<float2*>(ctx->fft_scratch);
+      if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, M * sizeof(float2))) return rc;
+      float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
       const size_t L1 = (size_t)1 << l1, L2 = (size_t)1 << l2, L3 = (size_t)1 << l3;
       bool first_done = false;
       if (raw && raw->base) {
@@ -1335,7 +1217,7 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
       // tensor map refused: finish with the plain last pass + split kernel
       if (int rc2 = dispatch_trans<true>(ctx, llast, s, H, 1, A, L1)) return rc2;
       const unsigned grid = std::min<unsigned>(grid_for(ctx, M / 2 + 1, 256), 4096);
-      r2c_post_kernel<true><<<grid, 256, 0, ctx->stream>>>(H, M, ctx->partial, ctx->ticket, ctx->mean);
+      r2c_post_kernel<true><<<grid, 256, 0, ctx->lane.stream>>>(H, M, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean);
       ctx->launches++;
       CK(cudaGetLastError());
       return 0;
@@ -1344,7 +1226,7 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
   if (raw && raw->base) return SRTB_B200_E_UNSUPPORTED;  // fused unpack needs the multi-pass TMA route
   if (int rc = fft_c2c_impl<true>(ctx, H, M, 1)) return rc;
   const unsigned grid = std::min<unsigned>(grid_for(ctx, M / 2 + 1, 256), 4096);
-  r2c_post_kernel<true><<<grid, 256, 0, ctx->stream>>>(H, M, ctx->partial, ctx->ticket, ctx->mean);
+  r2c_post_kernel<true><<<grid, 256, 0, ctx->lane.stream>>>(H, M, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -1414,64 +1296,6 @@ extern "C" int srtb_b200_rfi_range_to_bins(float f1, float f2, float freq_low, f
   return 0;
 }
 
-extern "C" int srtb_b200_rfi_s1(srtb_b200_ctx* ctx, void* d_x, size_t count, float avg_threshold,
-                                float norm_coef, const size_t* h_bin_ranges, size_t n_ranges,
-                                float* d_mean_out) {
-  API_LOCK(ctx);
-  if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: null argument");
-  if (count == 0) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: zero count");
-  if (n_ranges && !h_bin_ranges) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: null ranges");
-  CK(cudaSetDevice(ctx->device));
-  stage_scope stats_(ctx, SRTB_B200_STAGE_RFI_S1, 24.0 * (double)count);
-  float2* x = static_cast<float2*>(d_x);
-  const unsigned grid = std::min<unsigned>(grid_for(ctx, count / 2 + 1, 256), 4096);
-  power_sum_kernel<<<grid, 256, 0, ctx->stream>>>(x, count, ctx->partial, ctx->ticket, ctx->mean);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  if (d_mean_out) CK(cudaMemcpyAsync(d_mean_out, ctx->mean, sizeof(float), cudaMemcpyDeviceToDevice, ctx->stream));
-  rfi_s1_apply_kernel<<<grid_for(ctx, count / 2 + 1, 256), 256, 0, ctx->stream>>>(x, count, ctx->mean, avg_threshold, norm_coef);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  for (size_t r0 = 0; r0 < n_ranges; r0 += 16) {
-    bin_ranges br;
-    const size_t nr = std::min<size_t>(16, n_ranges - r0);
-    size_t longest = 1;
-    for (size_t r = 0; r < nr; r++) {
-      const size_t lo = h_bin_ranges[2 * (r0 + r)], hi = h_bin_ranges[2 * (r0 + r) + 1];
-      if (!(lo <= hi && hi < count)) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: bin range out of bounds");
-      br.lo[r] = lo;
-      br.hi[r] = hi;
-      longest = std::max(longest, hi - lo + 1);
-    }
-    dim3 g(grid_for(ctx, longest, 256), (unsigned)nr);
-    rfi_zero_ranges_kernel<<<g, 256, 0, ctx->stream>>>(x, br);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
-  return 0;
-}
-
-// ------------------------------------------------------------------------------------
-// dedisperse
-// ------------------------------------------------------------------------------------
-extern "C" int srtb_b200_dedisperse(srtb_b200_ctx* ctx, void* d_x, size_t count, float f_min, float f_c,
-                                    float df, float dm) {
-  API_LOCK(ctx);
-  if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "dedisperse: null argument");
-  if (count == 0) return 0;
-  CK(cudaSetDevice(ctx->device));
-  stage_scope stats_(ctx, SRTB_B200_STAGE_DEDISPERSE, 16.0 * (double)count);
-  constexpr double D = 4.148808e3;  // coherent_dedispersion.hpp:67
-  const double ddm = (D * 1e6) * (double)dm;
-  dedisperse_kernel<false><<<grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, ctx->stream>>>(
-      static_cast<const float2*>(d_x), static_cast<float2*>(d_x), count, (double)f_min, (double)df, (double)f_c, ddm, nullptr, 0.f, 1.f);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return 0;
-}
-
-// s1 (mean -> zap/normalise) and the chirp in two kernels instead of three: power sum, then one
-// fused apply + chirp sweep, then the manual zap (zero * chirp = zero, so the order is equivalent)
 // mitigate_rfi_manual (rfi_mitigation.hpp:97-158): zero the listed bin ranges, 16 ranges per launch
 static int zero_bin_ranges(srtb_b200_ctx* ctx, float2* x, const std::vector<size_t>& bins) {
   for (size_t r0 = 0; r0 < bins.size() / 2; r0 += 16) {
@@ -1491,20 +1315,59 @@ static int zero_bin_ranges(srtb_b200_ctx* ctx, float2* x, const std::vector<size
   return 0;
 }
 
-static int rfi_s1_dedisperse_fused(srtb_b200_ctx* ctx, float2* x, size_t count, float avg_threshold, float coef,
-                                   const std::vector<size_t>& bins, float f_min, float f_c, float df, float dm,
-                                   bool mean_ready, const float2* src = nullptr) {
-  if (!src) src = x;  // in place unless a separate (kept) spectrum is given
-  if (!mean_ready) {
-    const unsigned grid = std::min<unsigned>(grid_for(ctx, count / 2 + 1, 256), 4096);
-    power_sum_kernel<<<grid, 256, 0, ctx->stream>>>(x, count, ctx->partial, ctx->ticket, ctx->mean);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
+extern "C" int srtb_b200_rfi_s1(srtb_b200_ctx* ctx, void* d_x, size_t count, float avg_threshold,
+                                float norm_coef, const size_t* h_bin_ranges, size_t n_ranges,
+                                float* d_mean_out) {
+  API_LOCK(ctx);
+  if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: null argument");
+  if (count == 0) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: zero count");
+  if (n_ranges && !h_bin_ranges) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: null ranges");
+  const std::vector<size_t> bins(h_bin_ranges, h_bin_ranges + 2 * n_ranges);
+  for (size_t r = 0; r < n_ranges; r++)
+    if (!(bins[2 * r] <= bins[2 * r + 1] && bins[2 * r + 1] < count))
+      return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: bin range out of bounds");
+  CK(cudaSetDevice(ctx->device));
+  stage_scope stats_(ctx, SRTB_B200_STAGE_RFI_S1, 24.0 * (double)count);
+  float2* x = static_cast<float2*>(d_x);
+  const unsigned grid = std::min<unsigned>(grid_for(ctx, count / 2 + 1, 256), 4096);
+  power_sum_kernel<<<grid, 256, 0, ctx->lane.stream>>>(x, count, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  if (d_mean_out) CK(cudaMemcpyAsync(d_mean_out, ctx->lane.mean, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
+  rfi_s1_apply_kernel<<<grid_for(ctx, count / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(x, count, ctx->lane.mean, avg_threshold, norm_coef);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return zero_bin_ranges(ctx, x, bins);
+}
+
+// ------------------------------------------------------------------------------------
+// dedisperse
+// ------------------------------------------------------------------------------------
+extern "C" int srtb_b200_dedisperse(srtb_b200_ctx* ctx, void* d_x, size_t count, float f_min, float f_c,
+                                    float df, float dm) {
+  API_LOCK(ctx);
+  if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "dedisperse: null argument");
+  if (count == 0) return 0;
+  CK(cudaSetDevice(ctx->device));
+  stage_scope stats_(ctx, SRTB_B200_STAGE_DEDISPERSE, 16.0 * (double)count);
+  constexpr double D = 4.148808e3;  // coherent_dedispersion.hpp:67
+  const double ddm = (D * 1e6) * (double)dm;
+  dedisperse_kernel<false><<<grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, ctx->lane.stream>>>(
+      static_cast<const float2*>(d_x), static_cast<float2*>(d_x), count, (double)f_min, (double)df, (double)f_c, ddm, nullptr, 0.f, 1.f);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// s1 (mean -> zap/normalise) and the chirp in two kernels instead of three: power sum, then one
+// fused apply + chirp sweep, then the manual zap (zero * chirp = zero, so the order is equivalent). The mean is
+// already in the lane's `mean` (left there by the R2C); src is the spectrum read, x the one written (may be equal).
+static int rfi_s1_dedisperse_fused(srtb_b200_ctx* ctx, float2* x, const float2* src, size_t count, float avg_threshold,
+                                   float coef, const std::vector<size_t>& bins, float f_min, float f_c, float df, float dm) {
   constexpr double D = 4.148808e3;
   const double ddm = (D * 1e6) * (double)dm;
-  dedisperse_kernel<true><<<grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, ctx->stream>>>(
-      src, x, count, (double)f_min, (double)df, (double)f_c, ddm, ctx->mean, avg_threshold, coef);
+  dedisperse_kernel<true><<<grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, ctx->lane.stream>>>(
+      src, x, count, (double)f_min, (double)df, (double)f_c, ddm, ctx->lane.mean, avg_threshold, coef);
   ctx->launches++;
   CK(cudaGetLastError());
   return zero_bin_ranges(ctx, x, bins);
@@ -1528,6 +1391,17 @@ extern "C" size_t srtb_b200_nsamps_reserved(size_t baseband_input_count, size_t 
 // ------------------------------------------------------------------------------------
 // RFI stage 2 (spectral kurtosis)
 // ------------------------------------------------------------------------------------
+// a channel is kept when its SK estimate over M time samples lies in [lo, hi]
+struct sk_range {
+  float lo, hi;
+};
+static sk_range sk_bounds(float sk_threshold, size_t M) {
+  const float M_ = static_cast<float>(M);
+  float hi = sk_threshold, lo = 2 - sk_threshold;
+  if (lo > hi) std::swap(lo, hi);
+  return {lo * ((M_ - 1) / (M_ + 1)) + 1, hi * ((M_ - 1) / (M_ + 1)) + 1};
+}
+
 extern "C" int srtb_b200_rfi_s2_sk(srtb_b200_ctx* ctx, void* d_x, size_t time_count, size_t chan_count,
                                    float sk_threshold, float* d_sk_out) {
   API_LOCK(ctx);
@@ -1535,11 +1409,8 @@ extern "C" int srtb_b200_rfi_s2_sk(srtb_b200_ctx* ctx, void* d_x, size_t time_co
   if (time_count == 0 || chan_count == 0) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s2: zero size");
   CK(cudaSetDevice(ctx->device));
   stage_scope stats_(ctx, SRTB_B200_STAGE_RFI_S2, 8.0 * (double)time_count * (double)chan_count);
-  const float M_ = static_cast<float>(time_count);
-  float hi = sk_threshold, lo = 2 - sk_threshold;
-  if (lo > hi) std::swap(lo, hi);
-  const float lo_ = lo * ((M_ - 1) / (M_ + 1)) + 1, hi_ = hi * ((M_ - 1) / (M_ + 1)) + 1;
-  sk_kernel<<<(unsigned)chan_count, 256, 0, ctx->stream>>>(static_cast<float2*>(d_x), time_count, lo_, hi_, d_sk_out);
+  const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
+  sk_kernel<<<(unsigned)chan_count, 256, 0, ctx->lane.stream>>>(static_cast<float2*>(d_x), time_count, lo_, hi_, d_sk_out);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -1564,17 +1435,23 @@ static int detect_prepare(srtb_b200_ctx* ctx, int slot, size_t time_count, size_
     ctx->series_elems = series_need;
   }
   {
-    size_t have = ctx->acc_elems * sizeof(float);
-    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->acc), &have, time_count * sizeof(float))) return rc;
-    ctx->acc_elems = have / sizeof(float);
+    size_t have = ctx->lane.acc_elems * sizeof(float);
+    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->lane.acc), &have, time_count * sizeof(float))) return rc;
+    ctx->lane.acc_elems = have / sizeof(float);
   }
-  {
-    size_t have = ctx->colsum_partial_elems * sizeof(float);
-    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->colsum_partial), &have, need_partial_elems * sizeof(float)))
-      return rc;
-    ctx->colsum_partial_elems = have / sizeof(float);
-  }
-  return 0;
+  return ensure_colsum_partial(ctx, need_partial_elems);
+}
+
+// channel rows in chunks for colsum_partial_kernel: about 8 CTAs per SM in all, at most 128 chunks
+struct colsum_chunks {
+  size_t ctas_per_chunk, rows_per_chunk, chunks;
+};
+static colsum_chunks colsum_geometry(const srtb_b200_ctx* ctx, size_t samples_per_row, size_t chan_count) {
+  const size_t ctas_per_chunk = (samples_per_row + 511) / 512;
+  size_t chunks = std::max<size_t>(1, (size_t)ctx->sm_count * 8 / ctas_per_chunk);
+  chunks = std::min(chunks, std::min<size_t>(128, chan_count));
+  const size_t rows_per_chunk = (chan_count + chunks - 1) / chunks;
+  return {ctas_per_chunk, rows_per_chunk, (chan_count + rows_per_chunk - 1) / rows_per_chunk};
 }
 
 // column-sum reduction over `chunks` partial rows, zero count, scan, boxcar ladder
@@ -1587,14 +1464,14 @@ static int detect_tail(srtb_b200_ctx* ctx, int slot, const float2* x, size_t tim
   float* const host_series = ctx->host_series_dst ? ctx->host_series_dst + (size_t)slot * SRTB_B200_MAX_BOXCARS * time_count : nullptr;
   stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_DETECT_TAIL, 4.0 * (double)chunks * (double)ts_count);
   CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>((ts_count + 31) / 32, (size_t)ctx->sm_count)),
-                dim3(1024), 0, (const float*)ctx->colsum_partial, ts_count, chunks, ctx->series[slot], ctx->acc, x, zero_stride,
-                chan_count, chan_thr, max_boxcar, ctx->detect_ticket, ctx->d_res + slot));
+                dim3(1024), 0, (const float*)ctx->lane.colsum_partial, ts_count, chunks, ctx->series[slot], ctx->lane.acc, x, zero_stride,
+                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot));
   ctx->launches++;
   CK(cudaGetLastError());
   // one CTA per possible boxcar; CTAs beyond n_boxcars (known only on the device) exit at once
   unsigned max_nb = 1;
   for (size_t b = 2; b <= max_boxcar && b < ts_count && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2) max_nb++;
-  CK(launch_pdl(ctx, detect_boxcar_kernel, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count, (const float*)ctx->acc,
+  CK(launch_pdl(ctx, detect_boxcar_kernel, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count, (const float*)ctx->lane.acc,
                 ts_count, snr, ctx->d_res + slot, host_series));
   ctx->launches++;
   CK(cudaGetLastError());
@@ -1606,82 +1483,54 @@ static int detect_enqueue(srtb_b200_ctx* ctx, int slot, const float2* x, size_t 
                           size_t chan_count, size_t time_reserved_count, float snr, float chan_thr,
                           size_t max_boxcar) {
   const size_t ts_count = (time_count <= time_reserved_count) ? time_count : time_count - time_reserved_count;
-  const size_t ctas_per_chunk = (ts_count + 511) / 512;
-  size_t chunks = std::max<size_t>(1, (size_t)ctx->sm_count * 8 / ctas_per_chunk);
-  chunks = std::min(chunks, std::min<size_t>(128, chan_count));
-  const size_t rows_per_chunk = (chan_count + chunks - 1) / chunks;
-  chunks = (chan_count + rows_per_chunk - 1) / rows_per_chunk;
-  if (int rc = detect_prepare(ctx, slot, time_count, chunks * ts_count)) return rc;
-  CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->stream));
-  dim3 g((unsigned)ctas_per_chunk, (unsigned)chunks);
-  colsum_partial_kernel<<<g, 256, 0, ctx->stream>>>(const_cast<float2*>(x), time_count, chan_count, ts_count, rows_per_chunk,
-                                                    ctx->colsum_partial, nullptr);
+  const colsum_chunks cg = colsum_geometry(ctx, ts_count, chan_count);
+  if (int rc = detect_prepare(ctx, slot, time_count, cg.chunks * ts_count)) return rc;
+  CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  dim3 g((unsigned)cg.ctas_per_chunk, (unsigned)cg.chunks);
+  colsum_partial_kernel<<<g, 256, 0, ctx->lane.stream>>>(const_cast<float2*>(x), time_count, chan_count, ts_count,
+                                                         cg.rows_per_chunk, ctx->lane.colsum_partial, nullptr);
   ctx->launches++;
   CK(cudaGetLastError());
-  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, chunks, snr, chan_thr, max_boxcar);
+  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr, max_boxcar);
 }
 
 // watfft (backward C2C of every channel row) with spectral kurtosis + the detector's partial column
 // sums fused into its epilogue: the dynamic spectrum is written once and not read again until the
 // candidate sink. Used by process_block when one CTA holds a whole row (L = 512 .. 4096).
-// s1 + chirp folded into the waterfall kernel's load (process_block, L = 1024..4096): SRTB_B200_FUSE_CHIRP=0 keeps
-// the separate dedisperse kernel
-static bool use_fused_chirp() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_FUSE_CHIRP");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
+// s1 + chirp folded into the waterfall kernel's load: the sixteen-point row kernels (L = 1024..4096) and the
+// whole-row kernel (L = 8192, 16384)
 static bool chirp_fusable(size_t time_count) {
-  if (!use_fused_chirp()) return false;
-  if (time_count == 8192 || time_count == 16384) return use_bigrow();
-  return use_row16() && (time_count == 1024 || time_count == 2048 || time_count == 4096);
+  return time_count == 1024 || time_count == 2048 || time_count == 4096 || time_count == 8192 || time_count == 16384;
 }
 
 template <int LOGL>
 static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, float lo_, float hi_, size_t ts_count,
                             size_t* chunks_out, const row_chirp_params* chirp = nullptr, const float2* src = nullptr) {
   if (!src) src = x;  // in place unless the input spectrum is kept (DM sweep)
-  if constexpr (has_row16<LOGL>::value && LOGL >= 10) {
-    if (use_row16()) {
-      constexpr int T16 = row16_t<LOGL>::value, threads = ((1 << LOGL) / 16) * T16;
-      auto kern = chirp ? fft_row16_tma_kernel<LOGL, T16, false, true, true> : fft_row16_tma_kernel<LOGL, T16, false, true, false>;
-      constexpr size_t smem = row16_smem<LOGL, T16>::bytes;
-      const size_t ntiles = (chan_count + T16 - 1) / T16;
-      unsigned grid = 1;
-      if (int rc = persistent_grid(ctx, kern, threads, smem, smem, ntiles, &grid)) return rc;
-      size_t have = ctx->colsum_partial_elems * sizeof(float);
-      if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->colsum_partial), &have, (size_t)grid * ts_count * sizeof(float)))
-        return rc;
-      ctx->colsum_partial_elems = have / sizeof(float);
-      const float2* tw = nullptr;
-      if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-      row_sk_params p{lo_, hi_, ctx->colsum_partial, (unsigned)ts_count};
-      CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem, src, x, chan_count, tw, p, chirp ? *chirp : row_chirp_params{}));
-      ctx->launches++;
-      CK(cudaGetLastError());
-      *chunks_out = grid;
-      return 0;
-    }
-  }
-  if (chirp || src != x) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: fused chirp needs the sixteen-point row kernel");
-  constexpr int T = row_t<LOGL>::value;
-  auto kern = fft_row_tma_kernel<LOGL, T, false, true>;
-  constexpr size_t smem = row_tma_smem<LOGL, T>::bytes;
-  const size_t ntiles = (chan_count + T - 1) / T;
   unsigned grid = 1;
-  if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
-  {
-    size_t have = ctx->colsum_partial_elems * sizeof(float);
-    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->colsum_partial), &have, (size_t)grid * ts_count * sizeof(float)))
-      return rc;
-    ctx->colsum_partial_elems = have / sizeof(float);
-  }
   const float2* tw = nullptr;
-  if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-  row_sk_params p{lo_, hi_, ctx->colsum_partial, (unsigned)ts_count};
-  kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->stream>>>(x, x, chan_count, tw, p);
+  if constexpr (LOGL >= 10) {  // sixteen-point row kernel; L = 512 has the eight-point one only
+    constexpr int T16 = row16_t<LOGL>::value, threads = ((1 << LOGL) / 16) * T16;
+    auto kern = chirp ? fft_row16_tma_kernel<LOGL, T16, false, true, true> : fft_row16_tma_kernel<LOGL, T16, false, true, false>;
+    constexpr size_t smem = row16_smem<LOGL, T16>::bytes;
+    const size_t ntiles = (chan_count + T16 - 1) / T16;
+    if (int rc = persistent_grid(ctx, kern, threads, smem, smem, ntiles, &grid)) return rc;
+    if (int rc = ensure_colsum_partial(ctx, (size_t)grid * ts_count)) return rc;
+    if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
+    row_sk_params p{lo_, hi_, ctx->lane.colsum_partial, (unsigned)ts_count};
+    CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem, src, x, chan_count, tw, p, chirp ? *chirp : row_chirp_params{}));
+  } else {
+    if (chirp || src != x) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: fused chirp needs the sixteen-point row kernel");
+    constexpr int T = row_t<LOGL>::value;
+    auto kern = fft_row_tma_kernel<LOGL, T, false, true>;
+    constexpr size_t smem = row_tma_smem<LOGL, T>::bytes;
+    const size_t ntiles = (chan_count + T - 1) / T;
+    if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
+    if (int rc = ensure_colsum_partial(ctx, (size_t)grid * ts_count)) return rc;
+    if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
+    row_sk_params p{lo_, hi_, ctx->lane.colsum_partial, (unsigned)ts_count};
+    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(x, x, chan_count, tw, p);
+  }
   ctx->launches++;
   CK(cudaGetLastError());
   *chunks_out = grid;
@@ -1696,11 +1545,8 @@ static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_
   if (int rc = detect_prepare(ctx, slot, time_count, 1)) return rc;
   // the result header is zeroed here unless the block path did it for every stream up front (a memset between two
   // kernels would break their programmatic-dependent-launch chain)
-  if (!ctx->res_zeroed) CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->stream));
-  const float M_ = static_cast<float>(time_count);
-  float hi = sk_threshold, lo = 2 - sk_threshold;
-  if (lo > hi) std::swap(lo, hi);
-  const float lo_ = lo * ((M_ - 1) / (M_ + 1)) + 1, hi_ = hi * ((M_ - 1) / (M_ + 1)) + 1;
+  if (!ctx->res_zeroed) CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
   size_t chunks = 0;
   int rc = 0;
   std::unique_ptr<stage_scope> stats_(new stage_scope(ctx, SRTB_B200_STAGE_FUSED_WATERFALL, 16.0 * (double)time_count * (double)chan_count));
@@ -1751,14 +1597,10 @@ static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_
 //   decide   one thread per channel folds its tiles and takes the SK decision
 //   sums     the detector's partial column sums, zeroing the flagged rows on the way (one read of the spectrum)
 // i.e. 20 bytes per sample instead of the 32 of dedisperse + two-sweep waterfall + SK + column sums.
-static bool long_fusable(size_t time_count, const float2* x) {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_LONG_FUSED");
-    return !(e && e[0] == '0');
-  }();
+// (16-byte aligned spectra only)
+static bool long_fusable(size_t time_count) {
   const int q = ilog2(time_count);
-  return on && use_fused_chirp() && use_col16() && is_pow2(time_count) && q >= 15 && q <= 18 && get_encode_tiled() &&
-         (reinterpret_cast<uintptr_t>(x) & 15u) == 0;
+  return is_pow2(time_count) && q >= 15 && q <= 18 && get_encode_tiled();
 }
 
 static int watfft_long_fused(srtb_b200_ctx* ctx, int slot, float2* x, const float2* src, size_t time_count,
@@ -1768,14 +1610,14 @@ static int watfft_long_fused(srtb_b200_ctx* ctx, int slot, float2* x, const floa
   const int q = ilog2(time_count);
   const int l1 = (q + 1) / 2, l2 = q - l1;
   const size_t L1 = (size_t)1 << l1, L2 = (size_t)1 << l2;
-  if (int rc = ensure(ctx, &ctx->fft_scratch, &ctx->fft_scratch_bytes, chan_count * time_count * sizeof(float2))) return rc;
-  float2* s = static_cast<float2*>(ctx->fft_scratch);
+  if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, chan_count * time_count * sizeof(float2))) return rc;
+  float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
   const size_t T_last = (l2 <= 8) ? 16 : 8;  // rows per tile of the last sweep (col_t)
   const size_t tiles_per_row = L1 / T_last;
-  if (int rc = ensure(ctx, &ctx->long_stats, &ctx->long_stats_bytes, chan_count * tiles_per_row * sizeof(float2))) return rc;
-  if (int rc = ensure(ctx, &ctx->long_zap, &ctx->long_zap_bytes, chan_count)) return rc;
-  float2* stats = static_cast<float2*>(ctx->long_stats);
-  unsigned char* zap = static_cast<unsigned char*>(ctx->long_zap);
+  if (int rc = ensure(ctx, &ctx->lane.long_stats, &ctx->lane.long_stats_bytes, chan_count * tiles_per_row * sizeof(float2))) return rc;
+  if (int rc = ensure(ctx, &ctx->lane.long_zap, &ctx->lane.long_zap_bytes, chan_count)) return rc;
+  float2* stats = static_cast<float2*>(ctx->lane.long_stats);
+  unsigned char* zap = static_cast<unsigned char*>(ctx->lane.long_zap);
   row_chirp_params cp = chirp;
   {
     // Newton steps for 1/f between a thread's consecutive points, U * B = (L1 / 16) * L2 bins apart
@@ -1804,28 +1646,22 @@ static int watfft_long_fused(srtb_b200_ctx* ctx, int slot, float2* x, const floa
   }
   if (rc) return rc;
   if (!done) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: long fused plan needs the TMA last sweep");
-  const float M_ = static_cast<float>(time_count);
-  float hi = sk_threshold, lo = 2 - sk_threshold;
-  if (lo > hi) std::swap(lo, hi);
-  const float lo_ = lo * ((M_ - 1) / (M_ + 1)) + 1, hi_ = hi * ((M_ - 1) / (M_ + 1)) + 1;
-  sk_decide_kernel<<<(unsigned)((chan_count + 255) / 256), 256, 0, ctx->stream>>>(stats, (unsigned)tiles_per_row, chan_count,
-                                                                             M_, lo_, hi_, zap);
+  const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
+  sk_decide_kernel<<<(unsigned)((chan_count + 255) / 256), 256, 0, ctx->lane.stream>>>(
+      stats, (unsigned)tiles_per_row, chan_count, static_cast<float>(time_count), lo_, hi_, zap);
   ctx->launches++;
   CK(cudaGetLastError());
   // partial column sums (all time samples are visited so that flagged rows are zeroed completely)
-  const size_t ctas_per_chunk = (time_count + 511) / 512;
-  size_t chunks = std::max<size_t>(1, (size_t)ctx->sm_count * 8 / ctas_per_chunk);
-  chunks = std::min(chunks, std::min<size_t>(128, chan_count));
-  const size_t rows_per_chunk = (chan_count + chunks - 1) / chunks;
-  chunks = (chan_count + rows_per_chunk - 1) / rows_per_chunk;
-  if (int rc2 = detect_prepare(ctx, slot, time_count, chunks * ts_count)) return rc2;
-  if (!ctx->res_zeroed) CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->stream));
-  dim3 g((unsigned)ctas_per_chunk, (unsigned)chunks);
-  colsum_partial_kernel<<<g, 256, 0, ctx->stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, ctx->colsum_partial, zap);
+  const colsum_chunks cg = colsum_geometry(ctx, time_count, chan_count);
+  if (int rc2 = detect_prepare(ctx, slot, time_count, cg.chunks * ts_count)) return rc2;
+  if (!ctx->res_zeroed) CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  dim3 g((unsigned)cg.ctas_per_chunk, (unsigned)cg.chunks);
+  colsum_partial_kernel<<<g, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, cg.rows_per_chunk,
+                                                         ctx->lane.colsum_partial, zap);
   ctx->launches++;
   CK(cudaGetLastError());
   stats_.reset();
-  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, chunks, snr, chan_thr, max_boxcar);
+  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr, max_boxcar);
 }
 
 // s2 (spectral kurtosis) + the detector's first column-sum stage in one sweep; used by process_block
@@ -1835,7 +1671,7 @@ static bool sk_detect_fusable(size_t time_count) {
 }
 // waterfall FFT + SK + column sums in one kernel (no chirp): the row kernels above plus the whole-row kernel
 static bool watfft_sk_fusable(size_t time_count) {
-  return sk_detect_fusable(time_count) || ((time_count == 8192 || time_count == 16384) && use_bigrow());
+  return sk_detect_fusable(time_count) || time_count == 8192 || time_count == 16384;
 }
 static int sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_t time_count, size_t chan_count,
                            size_t time_reserved_count, float sk_threshold, float snr, float chan_thr,
@@ -1844,16 +1680,13 @@ static int sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_t time_
   const size_t rows_per_chunk = std::max<size_t>(1, chan_count / ((size_t)ctx->sm_count * 4));
   const size_t chunks = (chan_count + rows_per_chunk - 1) / rows_per_chunk;
   if (int rc = detect_prepare(ctx, slot, time_count, chunks * ts_count)) return rc;
-  CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->stream));
-  const float M_ = static_cast<float>(time_count);
-  float hi = sk_threshold, lo = 2 - sk_threshold;
-  if (lo > hi) std::swap(lo, hi);
-  const float lo_ = lo * ((M_ - 1) / (M_ + 1)) + 1, hi_ = hi * ((M_ - 1) / (M_ + 1)) + 1;
+  CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
   switch (time_count / 512) {
-    case 1: sk_colsum_kernel<1><<<(unsigned)chunks, 256, 0, ctx->stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->colsum_partial); break;
-    case 2: sk_colsum_kernel<2><<<(unsigned)chunks, 256, 0, ctx->stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->colsum_partial); break;
-    case 4: sk_colsum_kernel<4><<<(unsigned)chunks, 256, 0, ctx->stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->colsum_partial); break;
-    default: sk_colsum_kernel<8><<<(unsigned)chunks, 256, 0, ctx->stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->colsum_partial); break;
+    case 1: sk_colsum_kernel<1><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
+    case 2: sk_colsum_kernel<2><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
+    case 4: sk_colsum_kernel<4><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
+    default: sk_colsum_kernel<8><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
   }
   ctx->launches++;
   CK(cudaGetLastError());
@@ -1870,16 +1703,16 @@ static int detect_collect(srtb_b200_ctx* ctx, int slot, srtb_b200_detect_result*
     for (int b = 0; b < h_result->n_boxcars; b++) {
       if (copy_all || h_result->signal_count[b] > 0) {
         CK(cudaMemcpyAsync(h_series + (size_t)b * stride, ctx->series[slot] + (size_t)b * stride,
-                           h_result->series_length[b] * sizeof(float), cudaMemcpyDeviceToHost, ctx->stream));
+                           h_result->series_length[b] * sizeof(float), cudaMemcpyDeviceToHost, ctx->lane.stream));
         any = true;
       }
     }
-    if (any) CK(cudaStreamSynchronize(ctx->stream));
+    if (any) CK(cudaStreamSynchronize(ctx->lane.stream));
   } else if (h_series && copy_all) {
     // detection disabled: still hand back the mean-removed time series
     CK(cudaMemcpyAsync(h_series, ctx->series[slot], h_result->time_series_count * sizeof(float),
-                       cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
+                       cudaMemcpyDeviceToHost, ctx->lane.stream));
+    CK(cudaStreamSynchronize(ctx->lane.stream));
   }
   return 0;
 }
@@ -1896,25 +1729,22 @@ extern "C" int srtb_b200_signal_detect(srtb_b200_ctx* ctx, const void* d_x, size
   if (int rc = detect_enqueue(ctx, 0, static_cast<const float2*>(d_x), time_count, chan_count,
                               time_reserved_count, snr_threshold, channel_threshold, max_boxcar_length))
     return rc;
-  CK(cudaMemcpyAsync(ctx->h_res, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_res, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
+  CK(cudaStreamSynchronize(ctx->lane.stream));
   return detect_collect(ctx, 0, h_result, h_series, copy_all);
 }
 
 // ---- alternates of the refft path: spectra laid out [time][frequency] ------------------------------------------
 static int sk_v1_enqueue(srtb_b200_ctx* ctx, float2* x, size_t fft_bins, size_t time_counts, float sk_threshold,
                          float* d_sk_out) {
-  if (int rc = ensure(ctx, &ctx->long_zap, &ctx->long_zap_bytes, fft_bins)) return rc;
-  unsigned char* zap = static_cast<unsigned char*>(ctx->long_zap);
-  const float M_ = static_cast<float>(time_counts);
-  float hi = sk_threshold, lo = 2 - sk_threshold;
-  if (lo > hi) std::swap(lo, hi);
-  const float lo_ = lo * ((M_ - 1) / (M_ + 1)) + 1, hi_ = hi * ((M_ - 1) / (M_ + 1)) + 1;
-  sk_v1_stats_kernel<<<(unsigned)((fft_bins + 31) / 32), 256, 0, ctx->stream>>>(x, fft_bins, time_counts, lo_, hi_, zap, d_sk_out);
+  if (int rc = ensure(ctx, &ctx->lane.long_zap, &ctx->lane.long_zap_bytes, fft_bins)) return rc;
+  unsigned char* zap = static_cast<unsigned char*>(ctx->lane.long_zap);
+  const auto [lo_, hi_] = sk_bounds(sk_threshold, time_counts);
+  sk_v1_stats_kernel<<<(unsigned)((fft_bins + 31) / 32), 256, 0, ctx->lane.stream>>>(x, fft_bins, time_counts, lo_, hi_, zap, d_sk_out);
   ctx->launches++;
   CK(cudaGetLastError());
   const unsigned gy = (unsigned)std::max<size_t>(1, std::min<size_t>(time_counts, 64));
-  sk_v1_zero_kernel<<<dim3((unsigned)((fft_bins + 255) / 256), gy), 256, 0, ctx->stream>>>(x, fft_bins, time_counts, zap);
+  sk_v1_zero_kernel<<<dim3((unsigned)((fft_bins + 255) / 256), gy), 256, 0, ctx->lane.stream>>>(x, fft_bins, time_counts, zap);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -1942,15 +1772,15 @@ extern "C" int srtb_b200_signal_detect_v1(srtb_b200_ctx* ctx, void* d_x, size_t 
   // one value per spectrum; then the same tail as the v2 detector (mean removal, scan, boxcars) on a series of
   // batch_size values, masked channels counted over the first spectrum
   if (int rc = detect_prepare(ctx, 0, batch_size, batch_size)) return rc;
-  CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result), ctx->stream));
-  rowsum_norm_kernel<<<(unsigned)((batch_size + 7) / 8), 256, 0, ctx->stream>>>(x, count_per_batch, batch_size, ctx->colsum_partial);
+  CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  rowsum_norm_kernel<<<(unsigned)((batch_size + 7) / 8), 256, 0, ctx->lane.stream>>>(x, count_per_batch, batch_size, ctx->lane.colsum_partial);
   ctx->launches++;
   CK(cudaGetLastError());
   if (int rc = detect_tail(ctx, 0, x, batch_size, count_per_batch, batch_size, 1, snr_threshold, channel_threshold,
                            max_boxcar_length, /*zero_stride=*/1))
     return rc;
-  CK(cudaMemcpyAsync(ctx->h_res, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_res, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
+  CK(cudaStreamSynchronize(ctx->lane.stream));
   return detect_collect(ctx, 0, h_result, h_series, copy_all);
 }
 
@@ -1968,8 +1798,6 @@ static int format_streams(int format) {
   }
 }
 
-// enqueue every stage of one block on ctx->stream (no host sync); results land in
-// ctx->h_res[res_base .. res_base + streams) once the stream reaches the final D2H copy
 // unpack fused into the first FFT sweep: possible when the samples are 8-bit, the window is the rectangle and every
 // complex point of a stream is one fixed-size byte group (simple, "1 1 2 2", "1 2 1 2"); fills raw[stream]
 static bool raw_sources_for(const srtb_b200_block_config* cfg, const void* d_baseband, size_t baseband_bytes, int streams,
@@ -1977,6 +1805,7 @@ static bool raw_sources_for(const srtb_b200_block_config* cfg, const void* d_bas
   const int bits = cfg->baseband_input_bits;
   const int fmt = cfg->baseband_format;
   const size_t N = cfg->baseband_input_count;
+  // SRTB_B200_NO_FUSED_UNPACK forces the unpack kernel: the test of the fused first sweep compares both routes with it
   if (cfg->window != SRTB_B200_WINDOW_RECTANGLE || N < ((size_t)1 << 14) || !get_encode_tiled() ||
       std::getenv("SRTB_B200_NO_FUSED_UNPACK"))
     return false;
@@ -2030,21 +1859,12 @@ static int ensure_stream_bufs(srtb_b200_ctx* ctx, float* (&bufs)[4], size_t* ele
   return 0;
 }
 
-// bufs[s]: working buffer of stream s (N + 2 floats, 16-byte aligned for the fused routes) — holds the dynamic
-// spectrum [C][L] when the block is done. host_series (optional): pinned host memory that receives positive series.
-// K12 phase table for the whole-row waterfall kernel (block path; SRTB_B200_CHIRP_TABLE=0 evaluates every phase on the
-// fly like the DM sweep does). Rebuilt when the geometry or the DM changes; built synchronously, so both lanes and any
-// later launch may read it.
-static bool use_chirp_table() {
-  static const bool on = [] {
-    const char* e = std::getenv("SRTB_B200_CHIRP_TABLE");
-    return !(e && e[0] == '0');
-  }();
-  return on;
-}
+// K12 phase table for the whole-row waterfall kernel (block path; the DM sweep, and tables above 4 GiB, evaluate every
+// phase on the fly). Rebuilt when the geometry or the DM changes; built synchronously, so both lanes and any later
+// launch may read it.
 static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params& cp, const float** out) {
   *out = nullptr;
-  if (!use_chirp_table() || n * sizeof(float) > ((size_t)4 << 30)) return 0;
+  if (n * sizeof(float) > ((size_t)4 << 30)) return 0;
   const double key[6] = {(double)n, cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm};
   if (ctx->chirp_tab && std::memcmp(key, ctx->chirp_tab_key, sizeof(key)) == 0) {
     *out = ctx->chirp_tab;
@@ -2052,52 +1872,189 @@ static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params&
   }
   if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->chirp_tab), &ctx->chirp_tab_bytes, n * sizeof(float))) return rc;
   if (int rc = sync_lanes(ctx)) return rc;  // a block still in flight may be reading the previous table
-  chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->stream>>>(ctx->chirp_tab, n, cp.f_min, cp.df, cp.inv_fc,
+  chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(ctx->chirp_tab, n, cp.f_min, cp.df, cp.inv_fc,
                                                                            cp.f_c, cp.ddm);
   CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(ctx->stream));
+  CK(cudaStreamSynchronize(ctx->lane.stream));
   std::memcpy(ctx->chirp_tab_key, key, sizeof(key));
   *out = ctx->chirp_tab;
   return 0;
 }
 
-// second lane of a context (see srtb_b200_ctx::lane_state): created on first use
+// second lane of a context (see lane_state): created on first use
 static int ensure_alt_lane(srtb_b200_ctx* ctx) {
   if (ctx->alt_ready) return 0;
-  auto& a = ctx->alt;
-  {
-    // SRTB_B200_LANE_PRIORITY=1: the second lane at the lowest stream priority, so that its CTAs only fill what the
-    // first lane leaves free instead of being co-scheduled with it (experiment; default: equal priorities)
-    const char* e = std::getenv("SRTB_B200_LANE_PRIORITY");
-    if (e && e[0] == '1') {
-      int lo = 0, hi = 0;
-      CK(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-      CK(cudaStreamCreateWithPriority(&a.stream, cudaStreamNonBlocking, lo));
-    } else {
-      CK(cudaStreamCreateWithFlags(&a.stream, cudaStreamNonBlocking));
-    }
-  }
-  CK(cudaMalloc(&a.partial, sizeof(double) * 4096));
-  CK(cudaMalloc(&a.ticket, sizeof(unsigned)));
-  CK(cudaMemset(a.ticket, 0, sizeof(unsigned)));
-  CK(cudaMalloc(&a.detect_ticket, sizeof(unsigned)));
-  CK(cudaMemset(a.detect_ticket, 0, sizeof(unsigned)));
-  CK(cudaMalloc(&a.mean, sizeof(float)));
+  CK(cudaStreamCreateWithFlags(&ctx->alt.stream, cudaStreamNonBlocking));
+  CK(lane_alloc(&ctx->alt));
   CK(cudaEventCreateWithFlags(&ctx->lane_fork, cudaEventDisableTiming));
   CK(cudaEventCreateWithFlags(&ctx->lane_join, cudaEventDisableTiming));
   ctx->alt_ready = true;
   return 0;
 }
 
-// join_lanes: the first lane waits for the second at the end (process_block); the ring leaves the lanes free-running
-// (each copies its own result headers back, *alt_used tells the caller to record a completion event on both).
-static int block_enqueue(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* d_baseband,
-                         size_t baseband_bytes, int res_base, int* streams_out, size_t* L_out, float* const* bufs,
-                         float* host_series, bool join_lanes = true, bool* alt_used = nullptr) {
-  const int streams = format_streams(cfg->baseband_format);
-  if (!streams) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "process_block: unknown format");
-  const size_t N = cfg->baseband_input_count;
-  if (N < 2 || !is_pow2(N)) return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(N));
+// called on the first lane: the second lane continues from this point of it
+static int fork_lanes(srtb_b200_ctx* ctx) {
+  CK(cudaEventRecord(ctx->lane_fork, ctx->lane.stream));
+  CK(cudaStreamWaitEvent(ctx->alt.stream, ctx->lane_fork, 0));
+  return 0;
+}
+
+// what a block's configuration fixes for every one of its data streams
+struct block_params {
+  const srtb_b200_block_config* cfg = nullptr;
+  int streams = 0;
+  size_t N = 0, Nc = 0, batch = 0, L = 0;  // samples per stream, spectrum bins, channel rows, time samples per row
+  std::vector<size_t> bins;                // manual zap ranges as (lo, hi) bin pairs
+  float coef = 0, f_min = 0, f_c = 0, df = 0;
+  // time samples at the end of each row the detector leaves out at this DM
+  size_t reserved(float dm) const {
+    return srtb_b200_nsamps_reserved(N, cfg->spectrum_channel_count, cfg->baseband_freq_low, cfg->baseband_bandwidth,
+                                     cfg->baseband_sample_rate, dm, cfg->baseband_reserve_sample) /
+           batch;
+  }
+  // s1 + chirp at this DM, applied as a waterfall kernel loads the spectrum
+  row_chirp_params chirp(float dm, const float* mean) const {
+    constexpr double D = 4.148808e3;  // coherent_dedispersion.hpp:67
+    return {(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)dm,
+            mean, cfg->mitigate_rfi_average_method_threshold, coef, 0};
+  }
+};
+
+static int block_params_for(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const char* who, block_params* p) {
+  p->cfg = cfg;
+  p->streams = format_streams(cfg->baseband_format);
+  if (!p->streams) return fail(ctx, SRTB_B200_E_UNSUPPORTED, std::string(who) + ": unknown format");
+  p->N = cfg->baseband_input_count;
+  if (p->N < 2 || !is_pow2(p->N))
+    return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(p->N));
+  p->Nc = p->N / 2;
+  p->batch = std::min<size_t>(cfg->spectrum_channel_count, p->Nc);  // fft_pipe.hpp:318-320
+  if (p->batch == 0 || !is_pow2(p->batch))
+    return fail(ctx, SRTB_B200_E_SIZE, "spectrum_channel_count must be a power of 2");
+  p->L = p->Nc / p->batch;
+  // manual zap ranges -> bins (host, rfi_mitigation.hpp:102-143)
+  for (uint64_t r = 0; r < cfg->n_rfi_freq_pairs; r++) {
+    size_t lo, hi;
+    if (srtb_b200_rfi_range_to_bins(cfg->rfi_freq_pairs[2 * r], cfg->rfi_freq_pairs[2 * r + 1],
+                                    cfg->baseband_freq_low, cfg->baseband_bandwidth, p->Nc, &lo, &hi)) {
+      p->bins.push_back(lo);
+      p->bins.push_back(hi);
+    }
+  }
+  p->coef = srtb_b200_norm_coefficient(p->Nc, cfg->spectrum_channel_count);
+  p->df = cfg->baseband_bandwidth / static_cast<float>(p->Nc);  // dedisperse_pipe.hpp:34
+  p->f_min = cfg->baseband_freq_low;
+  p->f_c = p->f_min + cfg->baseband_bandwidth;
+  return 0;
+}
+
+// the block's baseband on the device and the per-stream buffers its R2C writes; raw[] describes the bytes for the
+// route with the unpack fused into the first sweep
+struct block_input {
+  const void* d_baseband;
+  size_t bytes;
+  float* const* bufs;
+  raw_source raw[4];
+  bool fuse_unpack = false, unpacked = false;
+};
+
+static int unpack_block(srtb_b200_ctx* ctx, const block_params& p, block_input* in) {
+  if (in->unpacked) return 0;
+  in->unpacked = true;
+  return srtb_b200_unpack(ctx, in->d_baseband, in->bytes, p.cfg->baseband_input_bits, p.cfg->baseband_format,
+                          p.cfg->window, in->bufs, p.N);
+}
+
+// the fused route when the format allows it, else the unpack kernel for every stream now
+static int block_input_init(srtb_b200_ctx* ctx, const block_params& p, block_input* in) {
+  in->fuse_unpack = raw_sources_for(p.cfg, in->d_baseband, in->bytes, p.streams, in->raw);
+  return in->fuse_unpack ? 0 : unpack_block(ctx, p, in);
+}
+
+// R2C of stream s in its buffer, leaving mean(|X|^2) in the lane's `mean`. When the fused route refuses this size or
+// alignment, all streams are unpacked once and take the plain R2C. The route is a property of the block (same size and
+// base pointer for every stream), so it can only change on stream 0; later it would overwrite finished streams with
+// their unpacked input. fork: the second lane must see the unpacked samples, so it is forked again after that unpack.
+static int r2c_stream(srtb_b200_ctx* ctx, const block_params& p, block_input* in, int s, bool fork) {
+  float* buf = in->bufs[s];
+  if (in->fuse_unpack && !in->unpacked) {
+    const int rc = fft_r2c_with_power_mean(ctx, buf, p.N, &in->raw[s], nullptr);
+    if (rc != SRTB_B200_E_UNSUPPORTED) return rc;
+    if (s > 0)
+      return fail(ctx, SRTB_B200_E_UNSUPPORTED,
+                  "fused unpack refused stream " + std::to_string(s) + " after accepting stream 0");
+    if (int rc2 = unpack_block(ctx, p, in)) return rc2;
+    if (fork)
+      if (int rc2 = fork_lanes(ctx)) return rc2;
+  }
+  return fft_r2c_with_power_mean(ctx, buf, p.N);
+}
+
+static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
+// routes that apply s1 + the chirp as a waterfall kernel loads the spectrum: the caller zaps the manual ranges on the
+// spectrum beforehand (0 stays 0 through s1 and the chirp)
+static bool chirp_on_load(size_t L, const void* dst, const void* src) {
+  return aligned16(dst) && aligned16(src) && (chirp_fusable(L) || long_fusable(L));
+}
+
+// one stream's chain after its R2C, at one DM: s1 + chirp, waterfall FFT, SK and detector, result header in
+// d_res[slot]. src holds the spectrum, dst receives the dynamic spectrum: the same buffer on the block path, while the
+// DM sweep keeps src for the next trial. phase_table: the whole-row kernel may read a tabulated chirp (built for the
+// block's DM; the DM sweep changes DM every trial).
+static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, float2* dst, const float2* src, float dm,
+                       bool phase_table) {
+  const srtb_b200_block_config* cfg = p.cfg;
+  const size_t reserved = p.reserved(dm);
+  const bool aligned = aligned16(dst) && aligned16(src);
+  if (aligned && chirp_fusable(p.L)) {
+    // ONE kernel: s1 + chirp on load, waterfall FFT, SK, partial column sums
+    row_chirp_params cp = p.chirp(dm, ctx->lane.mean);
+    if (phase_table)
+      if (int rc = get_chirp_table(ctx, p.Nc, cp, &cp.phase)) return rc;
+    return watfft_sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
+                                  cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
+                                  cfg->signal_detect_max_boxcar_length, &cp, src);
+  }
+  if (aligned && long_fusable(p.L)) {
+    // long rows: chirp-on-load column sweep, last sweep with SK statistics, decision, column sums (20 bytes per
+    // sample). No phase table here: the long-row column sweep is DRAM-bound, and the 4 extra bytes per bin a table
+    // costs outweigh the fp64 evaluation it would replace.
+    const int rc = watfft_long_fused(ctx, slot, dst, src, p.L, p.batch, reserved,
+                                     cfg->mitigate_rfi_spectral_kurtosis_threshold,
+                                     cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
+                                     cfg->signal_detect_max_boxcar_length, p.chirp(dm, ctx->lane.mean));
+    if (rc != SRTB_B200_E_UNSUPPORTED) return rc;
+  }
+  if (int rc = rfi_s1_dedisperse_fused(ctx, dst, src, p.Nc, cfg->mitigate_rfi_average_method_threshold, p.coef, p.bins,
+                                       p.f_min, p.f_c, p.df, dm))
+    return rc;
+  if (watfft_sk_fusable(p.L) && aligned16(dst)) {
+    // waterfall FFT + SK + partial column sums in one kernel, then the small detector tail
+    return watfft_sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
+                                  cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
+                                  cfg->signal_detect_max_boxcar_length);
+  }
+  if (int rc = srtb_b200_watfft_c2c_backward(ctx, dst, p.L, p.batch)) return rc;
+  if (sk_detect_fusable(p.L))
+    return sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
+                           cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
+                           cfg->signal_detect_max_boxcar_length);
+  if (int rc = srtb_b200_rfi_s2_sk(ctx, dst, p.L, p.batch, cfg->mitigate_rfi_spectral_kurtosis_threshold, nullptr))
+    return rc;
+  return detect_enqueue(ctx, slot, dst, p.L, p.batch, reserved, cfg->signal_detect_signal_noise_threshold,
+                        cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length);
+}
+
+// enqueue every stage of one block (no host sync); results land in ctx->h_res[res_base .. res_base + streams) once the
+// lanes reach their D2H copies. bufs[s]: working buffer of stream s (N + 2 floats, 16-byte aligned for the fused
+// routes), which holds the dynamic spectrum [C][L] when the block is done. host_series (optional): pinned host memory
+// that receives positive series. join_lanes: the first lane waits for the second at the end (process_block); the ring
+// leaves the lanes free-running (each copies its own result headers back, *alt_used tells the caller to record a
+// completion event on both).
+static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* d_baseband, size_t baseband_bytes,
+                         int res_base, float* const* bufs, float* host_series, bool join_lanes = true,
+                         bool* alt_used = nullptr) {
   struct series_dst_scope {  // detect_tail reads ctx->host_series_dst; it is only meaningful inside this call
     srtb_b200_ctx* c;
     ~series_dst_scope() {
@@ -2107,153 +2064,43 @@ static int block_enqueue(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, 
     }
   } series_scope_{ctx};
   ctx->host_series_dst = host_series;
-  ctx->pdl_auto = N <= ((size_t)1 << 25);
+  ctx->pdl_auto = p.N <= ((size_t)1 << 25);
   // the data streams of a block are independent: odd ones go to the context's second lane (per-stage timing wants the
   // kernels alone, so it keeps one lane)
-  const bool two_lanes = ctx->lanes >= 2 && streams >= 2 && !ctx->stats_on;
+  const bool two_lanes = ctx->lanes >= 2 && p.streams >= 2 && !ctx->stats_on;
   if (alt_used) *alt_used = two_lanes;
   if (two_lanes) {
     if (int rc = ensure_alt_lane(ctx)) return rc;
   } else {
     // result headers zeroed before the first kernel (a memset between kernels would break the dependent-launch chain);
     // with two lanes every stream zeroes its own header at the head of its chain, on its lane
-    CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result) * streams, ctx->stream));
+    CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result) * p.streams, ctx->lane.stream));
   }
   ctx->res_zeroed = true;
-  // unpack: fused into the first FFT pass when the samples are 8-bit and every complex point of a
-  // stream is one fixed-size byte group (simple, "1 1 2 2", "1 2 1 2"); otherwise the unpack kernel
-  raw_source raw[4];
-  const bool fuse_unpack = raw_sources_for(cfg, d_baseband, baseband_bytes, streams, raw);
-  bool unpacked = false;
-  auto ensure_unpacked = [&]() -> int {
-    if (unpacked) return 0;
-    unpacked = true;
-    return srtb_b200_unpack(ctx, d_baseband, baseband_bytes, cfg->baseband_input_bits, cfg->baseband_format,
-                            cfg->window, bufs, N);
-  };
-  if (!fuse_unpack)
-    if (int rc = ensure_unpacked()) return rc;
-  const size_t Nc = N / 2;
-  const size_t batch = std::min<size_t>(cfg->spectrum_channel_count, Nc);  // fft_pipe.hpp:318-320
-  if (batch == 0 || !is_pow2(batch)) return fail(ctx, SRTB_B200_E_SIZE, "spectrum_channel_count must be a power of 2");
-  const size_t L = Nc / batch;
-  // manual zap ranges -> bins (host, rfi_mitigation.hpp:102-143)
-  std::vector<size_t> bins;
-  for (uint64_t r = 0; r < cfg->n_rfi_freq_pairs; r++) {
-    size_t lo, hi;
-    if (srtb_b200_rfi_range_to_bins(cfg->rfi_freq_pairs[2 * r], cfg->rfi_freq_pairs[2 * r + 1],
-                                    cfg->baseband_freq_low, cfg->baseband_bandwidth, Nc, &lo, &hi)) {
-      bins.push_back(lo);
-      bins.push_back(hi);
-    }
-  }
-  const float coef = srtb_b200_norm_coefficient(Nc, cfg->spectrum_channel_count);
-  const float df = cfg->baseband_bandwidth / static_cast<float>(Nc);  // dedisperse_pipe.hpp:34
-  const float f_min = cfg->baseband_freq_low, f_c = f_min + cfg->baseband_bandwidth;
-  const size_t reserved = srtb_b200_nsamps_reserved(N, cfg->spectrum_channel_count, cfg->baseband_freq_low,
-                                                    cfg->baseband_bandwidth, cfg->baseband_sample_rate, cfg->dm,
-                                                    cfg->baseband_reserve_sample) /
-                          batch;
-  auto fork_lanes = [&]() -> int {  // called on the first lane: the second lane continues from this point of it
-    CK(cudaEventRecord(ctx->lane_fork, ctx->stream));
-    CK(cudaStreamWaitEvent(ctx->alt.stream, ctx->lane_fork, 0));
-    return 0;
-  };
+  block_input in{d_baseband, baseband_bytes, bufs};
+  if (int rc = block_input_init(ctx, p, &in)) return rc;
   if (two_lanes)
-    if (int rc = fork_lanes()) return rc;
+    if (int rc = fork_lanes(ctx)) return rc;
   auto enqueue_stream = [&](int s) -> int {
-    float* buf = bufs[s];
-    if (two_lanes) CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->stream));
+    float2* buf = reinterpret_cast<float2*>(bufs[s]);
+    if (two_lanes) CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
     {
       stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
-                         (double)N * (fuse_unpack ? (double)std::abs(cfg->baseband_input_bits) / 8.0 : 4.0) + 4.0 * (double)N);
-      int rc = SRTB_B200_E_UNSUPPORTED;
-      if (fuse_unpack && !unpacked) rc = fft_r2c_with_power_mean(ctx, buf, N, &raw[s], nullptr);
-      if (rc == SRTB_B200_E_UNSUPPORTED) {
-        // this size/alignment cannot take the fused route: unpack all streams once, then the plain R2C. The route is a
-        // property of the block (same size and base pointer for every stream), so it can only change on stream 0;
-        // later it would overwrite finished streams with their unpacked input
-        if (fuse_unpack && !unpacked && s > 0)
-          return fail(ctx, SRTB_B200_E_UNSUPPORTED, "process_block: fused unpack refused stream " + std::to_string(s) + " after accepting stream 0");
-        const bool was_unpacked = unpacked;
-        if (int rc2 = ensure_unpacked()) return rc2;
-        if (two_lanes && !was_unpacked)
-          if (int rc2 = fork_lanes()) return rc2;  // s == 0 here: the second lane must see the unpacked samples
-        rc = fft_r2c_with_power_mean(ctx, buf, N);
-      }
-      if (rc) return rc;
+                         (double)p.N * (in.fuse_unpack ? (double)std::abs(p.cfg->baseband_input_bits) / 8.0 : 4.0) +
+                             4.0 * (double)p.N);
+      if (int rc = r2c_stream(ctx, p, &in, s, /*fork=*/two_lanes)) return rc;
     }
-    const bool aligned = (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
-    if (chirp_fusable(L) && aligned) {
-      // manual zap on the raw spectrum (0 stays 0 through s1 and the chirp), then ONE kernel: s1 + chirp on load,
-      // waterfall FFT, SK, partial column sums
-      if (int rc = zero_bin_ranges(ctx, reinterpret_cast<float2*>(buf), bins)) return rc;
-      constexpr double D = 4.148808e3;  // coherent_dedispersion.hpp:67
-      row_chirp_params cp{(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)cfg->dm,
-                          ctx->mean, cfg->mitigate_rfi_average_method_threshold, coef};
-      if (int rc = get_chirp_table(ctx, Nc, cp, &cp.phase)) return rc;
-      if (int rc = watfft_sk_detect_fused(ctx, s, reinterpret_cast<float2*>(buf), L, batch, reserved,
-                                          cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                          cfg->signal_detect_signal_noise_threshold,
-                                          cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length,
-                                          &cp))
-        return rc;
-      return 0;
-    }
-    if (long_fusable(L, reinterpret_cast<float2*>(buf))) {
-      // long rows: manual zap on the raw spectrum, then chirp-on-load column sweep, last sweep with SK statistics,
-      // decision, column sums (20 bytes per sample)
-      if (int rc = zero_bin_ranges(ctx, reinterpret_cast<float2*>(buf), bins)) return rc;
-      constexpr double D = 4.148808e3;
-      row_chirp_params cp{(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)cfg->dm,
-                          ctx->mean, cfg->mitigate_rfi_average_method_threshold, coef, 0};
-      // (no phase table here: the long-row column sweep is DRAM-bound, and the 4 extra bytes per bin a table costs
-      // outweigh the fp64 evaluation it would replace)
-      const int rc = watfft_long_fused(ctx, s, reinterpret_cast<float2*>(buf), reinterpret_cast<const float2*>(buf), L, batch,
-                                       reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                       cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                                       cfg->signal_detect_max_boxcar_length, cp);
-      if (rc != SRTB_B200_E_UNSUPPORTED) {
-        if (rc) return rc;
-        return 0;
-      }
-    }
-    if (int rc = rfi_s1_dedisperse_fused(ctx, reinterpret_cast<float2*>(buf), Nc,
-                                         cfg->mitigate_rfi_average_method_threshold, coef, bins, f_min, f_c, df, cfg->dm,
-                                         /*mean_ready=*/true))
-      return rc;
-    if (watfft_sk_fusable(L) && aligned) {
-      // waterfall FFT + SK + partial column sums in one kernel, then the small detector tail
-      if (int rc = watfft_sk_detect_fused(ctx, s, reinterpret_cast<float2*>(buf), L, batch, reserved,
-                                          cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                          cfg->signal_detect_signal_noise_threshold,
-                                          cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length))
-        return rc;
-      return 0;
-    }
-    if (int rc = srtb_b200_watfft_c2c_backward(ctx, buf, L, batch)) return rc;
-    if (sk_detect_fusable(L)) {
-      if (int rc = sk_detect_fused(ctx, s, reinterpret_cast<float2*>(buf), L, batch, reserved,
-                                   cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                                   cfg->signal_detect_max_boxcar_length))
-        return rc;
-    } else {
-      if (int rc = srtb_b200_rfi_s2_sk(ctx, buf, L, batch, cfg->mitigate_rfi_spectral_kurtosis_threshold, nullptr)) return rc;
-      if (int rc = detect_enqueue(ctx, s, reinterpret_cast<const float2*>(buf), L, batch, reserved,
-                                  cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                                  cfg->signal_detect_max_boxcar_length))
-        return rc;
-    }
-    return 0;
+    if (chirp_on_load(p.L, buf, buf))
+      if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
+    return stream_tail(ctx, p, s, buf, buf, p.cfg->dm, /*phase_table=*/true);
   };
-  for (int s = 0; s < streams; s++) {
+  for (int s = 0; s < p.streams; s++) {
     const bool alt = two_lanes && (s & 1);
     if (alt) lane_swap(ctx);
     int rc = enqueue_stream(s);
     if (!rc && two_lanes) {
       const cudaError_t e = cudaMemcpyAsync(ctx->h_res + res_base + s, ctx->d_res + s, sizeof(detect_dev_result),
-                                            cudaMemcpyDeviceToHost, ctx->stream);
+                                            cudaMemcpyDeviceToHost, ctx->lane.stream);
       if (e != cudaSuccess) rc = fail(ctx, SRTB_B200_E_CUDA, std::string("result header copy: ") + cudaGetErrorString(e));
     }
     if (alt) lane_swap(ctx);
@@ -2262,14 +2109,12 @@ static int block_enqueue(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, 
   if (two_lanes) {
     if (join_lanes) {
       CK(cudaEventRecord(ctx->lane_join, ctx->alt.stream));
-      CK(cudaStreamWaitEvent(ctx->stream, ctx->lane_join, 0));
+      CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->lane_join, 0));
     }
   } else {
-    CK(cudaMemcpyAsync(ctx->h_res + res_base, ctx->d_res, sizeof(detect_dev_result) * streams, cudaMemcpyDeviceToHost,
-                       ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_res + res_base, ctx->d_res, sizeof(detect_dev_result) * p.streams, cudaMemcpyDeviceToHost,
+                       ctx->lane.stream));
   }
-  *streams_out = streams;
-  *L_out = L;
   return 0;
 }
 
@@ -2280,18 +2125,16 @@ extern "C" int srtb_b200_process_block_device(srtb_b200_ctx* ctx, const srtb_b20
   API_LOCK(ctx);
   if (!ctx || !cfg || !d_baseband || !h_results) return fail(ctx, SRTB_B200_E_INVALID, "process_block: null argument");
   CK(cudaSetDevice(ctx->device));
-  int streams = 0;
-  size_t L = 0;
-  if (format_streams(cfg->baseband_format) && cfg->baseband_input_count >= 2)
-    if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, cfg->baseband_input_count,
-                                    format_streams(cfg->baseband_format)))
+  block_params p;
+  if (int rc = block_params_for(ctx, cfg, "process_block", &p)) return rc;
+  if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, p.N, p.streams)) return rc;
+  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, 0, ctx->stream_buf, nullptr)) return rc;
+  CK(cudaStreamSynchronize(ctx->lane.stream));
+  for (int s = 0; s < p.streams; s++)
+    if (int rc = detect_collect(ctx, s, h_results + s, h_series ? h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
+                                copy_all))
       return rc;
-  if (int rc = block_enqueue(ctx, cfg, d_baseband, baseband_bytes, 0, &streams, &L, ctx->stream_buf, nullptr)) return rc;
-  CK(cudaStreamSynchronize(ctx->stream));
-  for (int s = 0; s < streams; s++)
-    if (int rc = detect_collect(ctx, s, h_results + s, h_series ? h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * L : nullptr, copy_all))
-      return rc;
-  return streams;
+  return p.streams;
 }
 
 extern "C" int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
@@ -2301,7 +2144,7 @@ extern "C" int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block
   if (!ctx || !cfg || !h_baseband) return fail(ctx, SRTB_B200_E_INVALID, "process_block: null argument");
   CK(cudaSetDevice(ctx->device));
   if (int rc = ensure(ctx, &ctx->d_baseband, &ctx->d_baseband_bytes, baseband_bytes)) return rc;
-  CK(cudaMemcpyAsync(ctx->d_baseband, h_baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->d_baseband, h_baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
   return srtb_b200_process_block_device(ctx, cfg, ctx->d_baseband, baseband_bytes, h_results, h_series, copy_all);
 }
 
@@ -2316,114 +2159,38 @@ extern "C" int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b
   if (!ctx || !cfg || !baseband || !h_dms || !h_results || n_dm == 0)
     return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: bad argument");
   CK(cudaSetDevice(ctx->device));
-  const int streams = format_streams(cfg->baseband_format);
-  if (!streams) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "dm_sweep: unknown format");
-  const size_t N = cfg->baseband_input_count;
-  if (N < 2 || !is_pow2(N)) return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(N));
+  block_params p;
+  if (int rc = block_params_for(ctx, cfg, "dm_sweep", &p)) return rc;
   const void* d_baseband = baseband;
   if (!on_device) {
     if (int rc = ensure(ctx, &ctx->d_baseband, &ctx->d_baseband_bytes, baseband_bytes)) return rc;
-    CK(cudaMemcpyAsync(ctx->d_baseband, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_baseband, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
     d_baseband = ctx->d_baseband;
   }
-  if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, N, streams)) return rc;
-  const size_t Nc = N / 2;
-  const size_t batch = std::min<size_t>(cfg->spectrum_channel_count, Nc);
-  if (batch == 0 || !is_pow2(batch)) return fail(ctx, SRTB_B200_E_SIZE, "spectrum_channel_count must be a power of 2");
-  const size_t L = Nc / batch;
-  if (int rc = ensure(ctx, &ctx->sweep_buf, &ctx->sweep_buf_bytes, (Nc + 1) * sizeof(float2))) return rc;
+  if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, p.N, p.streams)) return rc;
+  if (int rc = ensure(ctx, &ctx->sweep_buf, &ctx->sweep_buf_bytes, (p.Nc + 1) * sizeof(float2))) return rc;
   float2* W = static_cast<float2*>(ctx->sweep_buf);
-  // unpack: fused into the first R2C sweep when the format allows (as in process_block), else the unpack kernel
-  raw_source raw[4];
-  bool fuse_unpack = raw_sources_for(cfg, d_baseband, baseband_bytes, streams, raw);
-  bool unpacked = false;
-  auto ensure_unpacked = [&]() -> int {
-    if (unpacked) return 0;
-    unpacked = true;
-    return srtb_b200_unpack(ctx, d_baseband, baseband_bytes, cfg->baseband_input_bits, cfg->baseband_format,
-                            cfg->window, ctx->stream_buf, N);
-  };
-  if (!fuse_unpack)
-    if (int rc = ensure_unpacked()) return rc;
-  std::vector<size_t> bins;
-  for (uint64_t r = 0; r < cfg->n_rfi_freq_pairs; r++) {
-    size_t lo, hi;
-    if (srtb_b200_rfi_range_to_bins(cfg->rfi_freq_pairs[2 * r], cfg->rfi_freq_pairs[2 * r + 1],
-                                    cfg->baseband_freq_low, cfg->baseband_bandwidth, Nc, &lo, &hi)) {
-      bins.push_back(lo);
-      bins.push_back(hi);
-    }
-  }
-  const float coef = srtb_b200_norm_coefficient(Nc, cfg->spectrum_channel_count);
-  const float df = cfg->baseband_bandwidth / static_cast<float>(Nc);
-  const float f_min = cfg->baseband_freq_low, f_c = f_min + cfg->baseband_bandwidth;
+  block_input in{d_baseband, baseband_bytes, ctx->stream_buf};
+  if (int rc = block_input_init(ctx, p, &in)) return rc;
   // every trial's result header is parked on the device and fetched once at the end: no host sync per trial
-  if (int rc = ensure(ctx, &ctx->sweep_res, &ctx->sweep_res_bytes, n_dm * streams * sizeof(detect_dev_result))) return rc;
+  if (int rc = ensure(ctx, &ctx->sweep_res, &ctx->sweep_res_bytes, n_dm * p.streams * sizeof(detect_dev_result))) return rc;
   detect_dev_result* d_sweep = static_cast<detect_dev_result*>(ctx->sweep_res);
-  const bool fuse_chirp = chirp_fusable(L);
-  for (int s = 0; s < streams; s++) {
-    float* buf = ctx->stream_buf[s];
-    {
-      int rc = SRTB_B200_E_UNSUPPORTED;
-      if (fuse_unpack && !unpacked) rc = fft_r2c_with_power_mean(ctx, buf, N, &raw[s], nullptr);
-      if (rc == SRTB_B200_E_UNSUPPORTED) {
-        if (fuse_unpack && !unpacked && s > 0) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "dm_sweep: fused unpack refused a later stream");
-        if (int rc2 = ensure_unpacked()) return rc2;
-        rc = fft_r2c_with_power_mean(ctx, buf, N);  // leaves mean(|X|^2) in ctx->mean
-      }
-      if (rc) return rc;
-    }
-    const bool longf = long_fusable(L, W) && (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
-    const bool fused = (fuse_chirp || longf) && (reinterpret_cast<uintptr_t>(buf) & 15u) == 0;
-    if (fused)  // the manual zap does not depend on the DM: once, on the kept spectrum
-      if (int rc = zero_bin_ranges(ctx, reinterpret_cast<float2*>(buf), bins)) return rc;
+  for (int s = 0; s < p.streams; s++) {
+    if (int rc = r2c_stream(ctx, p, &in, s, /*fork=*/false)) return rc;
+    float2* buf = reinterpret_cast<float2*>(ctx->stream_buf[s]);
+    if (chirp_on_load(p.L, W, buf))  // the manual zap does not depend on the DM: once, on the kept spectrum
+      if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
     for (size_t j = 0; j < n_dm; j++) {
-      const size_t reserved = srtb_b200_nsamps_reserved(N, cfg->spectrum_channel_count, cfg->baseband_freq_low,
-                                                        cfg->baseband_bandwidth, cfg->baseband_sample_rate, h_dms[j],
-                                                        cfg->baseband_reserve_sample) / batch;
-      if (longf) {
-        constexpr double D = 4.148808e3;
-        row_chirp_params cp{(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)h_dms[j],
-                            ctx->mean, cfg->mitigate_rfi_average_method_threshold, coef, 0};
-        if (int rc = watfft_long_fused(ctx, 0, W, reinterpret_cast<const float2*>(buf), L, batch, reserved,
-                                       cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                       cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                                       cfg->signal_detect_max_boxcar_length, cp))
-          return rc;
-      } else if (fused) {
-        constexpr double D = 4.148808e3;
-        row_chirp_params cp{(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)h_dms[j],
-                            ctx->mean, cfg->mitigate_rfi_average_method_threshold, coef};
-        if (int rc = watfft_sk_detect_fused(ctx, 0, W, L, batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                            cfg->signal_detect_signal_noise_threshold,
-                                            cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length,
-                                            &cp, reinterpret_cast<const float2*>(buf)))
-          return rc;
-      } else {
-        if (int rc = rfi_s1_dedisperse_fused(ctx, W, Nc, cfg->mitigate_rfi_average_method_threshold, coef, bins, f_min,
-                                             f_c, df, h_dms[j], /*mean_ready=*/true, reinterpret_cast<const float2*>(buf)))
-          return rc;
-        if (watfft_sk_fusable(L)) {
-          if (int rc = watfft_sk_detect_fused(ctx, 0, W, L, batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                                              cfg->signal_detect_signal_noise_threshold,
-                                              cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length))
-            return rc;
-        } else {
-          if (int rc = srtb_b200_watfft_c2c_backward(ctx, W, L, batch)) return rc;
-          if (int rc = srtb_b200_rfi_s2_sk(ctx, W, L, batch, cfg->mitigate_rfi_spectral_kurtosis_threshold, nullptr)) return rc;
-          if (int rc = detect_enqueue(ctx, 0, W, L, batch, reserved, cfg->signal_detect_signal_noise_threshold,
-                                      cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length))
-            return rc;
-        }
-      }
-      CK(cudaMemcpyAsync(d_sweep + j * streams + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToDevice,
-                         ctx->stream));
+      if (int rc = stream_tail(ctx, p, 0, W, buf, h_dms[j], /*phase_table=*/false)) return rc;
+      CK(cudaMemcpyAsync(d_sweep + j * p.streams + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToDevice,
+                         ctx->lane.stream));
     }
   }
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
-  CK(cudaMemcpyAsync(h_results, d_sweep, n_dm * streams * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return streams;
+  CK(cudaMemcpyAsync(h_results, d_sweep, n_dm * p.streams * sizeof(detect_dev_result), cudaMemcpyDeviceToHost,
+                     ctx->lane.stream));
+  CK(cudaStreamSynchronize(ctx->lane.stream));
+  return p.streams;
 }
 
 // tickets wrap at a multiple of the slot count, so ticket % SRTB_B200_RING_SLOTS is always the slot that was used
@@ -2449,10 +2216,8 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
   CK(cudaSetDevice(ctx->device));
   const int slot = (int)(ctx->submit_count % SRTB_B200_RING_SLOTS);
   if (ctx->slot_busy[slot]) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: ring full, collect a block first");
-  const int streams = format_streams(cfg->baseband_format);
-  if (!streams) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "process_block: unknown format");
-  const size_t N = cfg->baseband_input_count;
-  if (N < 2 || !is_pow2(N)) return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(N));
+  block_params p;
+  if (int rc = block_params_for(ctx, cfg, "process_block", &p)) return rc;
   if (!ctx->slot_done[slot])
     for (int i = 0; i < SRTB_B200_RING_SLOTS; i++)
       if (!ctx->slot_done[i]) CK(cudaEventCreateWithFlags(&ctx->slot_done[i], cudaEventDisableTiming));
@@ -2460,20 +2225,18 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
   float* bufs[4] = {nullptr, nullptr, nullptr, nullptr};
   bool user_spec = outputs && outputs->d_spectrum[0];
   if (user_spec) {
-    for (int s = 0; s < streams; s++) {
+    for (int s = 0; s < p.streams; s++) {
       if (!outputs->d_spectrum[s]) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: d_spectrum given for some streams only");
       bufs[s] = outputs->d_spectrum[s];
     }
   } else {
-    if (int rc = ensure_stream_bufs(ctx, ctx->slot_stream_buf[slot], &ctx->slot_stream_elems[slot], N, streams)) return rc;
-    for (int s = 0; s < streams; s++) bufs[s] = ctx->slot_stream_buf[slot][s];
+    if (int rc = ensure_stream_bufs(ctx, ctx->slot_stream_buf[slot], &ctx->slot_stream_elems[slot], p.N, p.streams))
+      return rc;
+    for (int s = 0; s < p.streams; s++) bufs[s] = ctx->slot_stream_buf[slot][s];
   }
-  const size_t Nc = N / 2;
-  const size_t batch = std::min<size_t>(cfg->spectrum_channel_count ? cfg->spectrum_channel_count : 1, Nc);
-  const size_t L = Nc / batch;
   float* h_series = outputs ? outputs->h_series : nullptr;
   if (!h_series) {
-    const size_t need = (size_t)streams * SRTB_B200_MAX_BOXCARS * L;
+    const size_t need = (size_t)p.streams * SRTB_B200_MAX_BOXCARS * p.L;
     if (ctx->slot_h_series_elems[slot] < need) {
       if (int rc = sync_lanes(ctx)) return rc;
       if (ctx->slot_h_series[slot]) CK(cudaFreeHost(ctx->slot_h_series[slot]));
@@ -2494,14 +2257,15 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
     if (int rc = ensure(ctx, &ctx->slot_baseband[slot], &ctx->slot_baseband_bytes[slot], baseband_bytes)) return rc;
     CK(cudaMemcpyAsync(ctx->slot_baseband[slot], baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
     CK(cudaEventRecord(ctx->slot_h2d[slot], ctx->copy_stream));
-    CK(cudaStreamWaitEvent(ctx->stream, ctx->slot_h2d[slot], 0));
+    CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->slot_h2d[slot], 0));
     d_baseband = ctx->slot_baseband[slot];
   }
   bool alt_used = false;
-  if (int rc = block_enqueue(ctx, cfg, d_baseband, baseband_bytes, 4 * (1 + slot), &ctx->slot_streams[slot],
-                             &ctx->slot_L[slot], bufs, h_series, /*join_lanes=*/false, &alt_used))
+  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, 4 * (1 + slot), bufs, h_series, /*join_lanes=*/false,
+                             &alt_used))
     return rc;
-  CK(cudaEventRecord(ctx->slot_done[slot], ctx->stream));
+  ctx->slot_streams[slot] = p.streams;
+  CK(cudaEventRecord(ctx->slot_done[slot], ctx->lane.stream));
   ctx->slot_alt_used[slot] = alt_used;
   if (alt_used) {
     if (!ctx->slot_done_alt[slot]) CK(cudaEventCreateWithFlags(&ctx->slot_done_alt[slot], cudaEventDisableTiming));
