@@ -253,6 +253,9 @@ int srtb_b200_collect_block_ex(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_
 int srtb_b200_debug_set_submit_count(srtb_b200_ctx* ctx, uint64_t value);
 /* device pointer of stream s's dynamic spectrum after process_block (valid until next call) */
 const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int stream);
+/* test hook: device pointer of the [C][L] dynamic spectrum of the last trial of the last stream of the most recent
+   process_block_dm_sweep (valid until the next call) */
+const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx);
 
 #ifdef __cplusplus
 }

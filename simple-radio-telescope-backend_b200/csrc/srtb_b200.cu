@@ -2323,3 +2323,9 @@ extern "C" const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int st
   if (!ctx || stream < 0 || stream >= 4) return nullptr;
   return ctx->stream_buf[stream];
 }
+
+// every trial of a DM sweep writes its dynamic spectrum into sweep_buf; the last one written stays there
+extern "C" const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx) {
+  if (!ctx) return nullptr;
+  return ctx->sweep_buf;
+}

@@ -115,6 +115,7 @@ SYMBOLS = {
     "srtb_b200_collect_block_ex": (_I, [_P, _I, C.POINTER(DetectResult), C.POINTER(_P), C.POINTER(_P)]),
     "srtb_b200_debug_set_submit_count": (_I, [_P, C.c_uint64]),
     "srtb_b200_block_spectrum": (_P, [_P, _I]),
+    "srtb_b200_sweep_spectrum": (_P, [_P]),
 }
 
 _lib = None
@@ -301,6 +302,10 @@ class Context:
 
     def block_spectrum_ptr(self, stream: int) -> int:
         return self.lib.srtb_b200_block_spectrum(self.h, stream)
+
+    def sweep_spectrum_ptr(self) -> int:
+        """test hook: device pointer of the last trial's dynamic spectrum (last stream) of the latest DM sweep"""
+        return self.lib.srtb_b200_sweep_spectrum(self.h)
 
 
 # host helpers (pure host arithmetic of the reference's pipes)
