@@ -21,6 +21,14 @@ inline constexpr bool fft_operate_in_place = true;    // config.hpp:47
 inline constexpr size_t MEMORY_ALIGNMENT = 64ul;      // config.hpp:56
 inline constexpr size_t BITS_PER_BYTE = 8ul;          // config.hpp:58
 
+// waterfall thumbnail colours, ARGB32 (config.hpp:60-68): intensity 0 -> color_0, 1 -> color_1, else color_overflow
+namespace gui {
+inline constexpr uint32_t opaque = 0xff000000;
+inline constexpr uint32_t color_0 = 0x1f1e33 | opaque;
+inline constexpr uint32_t color_1 = 0x33e1f1 | opaque;
+inline constexpr uint32_t color_overflow = 0xe0e1cc | opaque;
+}  // namespace gui
+
 struct configs {
   std::string config_file_name = "srtb_config.cfg";
   size_t baseband_input_count = size_t{1} << 28;

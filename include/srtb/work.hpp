@@ -72,6 +72,37 @@ class mpmc_queue {
   bool empty() const { return read_available() == 0; }
 };
 
+/** multi-producer multi-consumer queue holding at most `capacity` works: push fails (returns false) when it is full,
+ *  so a loose out-functor drops the work instead of queueing it */
+template <typename T>
+class bounded_mpmc_queue {
+  mutable std::mutex m_;
+  std::deque<T> q_;
+  size_t capacity_;
+
+ public:
+  using work_type = T;
+  explicit bounded_mpmc_queue(size_t capacity = srtb::work_queue_capacity) : capacity_{capacity} {}
+  bool push(const T& v) {
+    std::lock_guard<std::mutex> g{m_};
+    if (q_.size() >= capacity_) return false;
+    q_.push_back(v);
+    return true;
+  }
+  bool pop(T& out) {
+    std::lock_guard<std::mutex> g{m_};
+    if (q_.empty()) return false;
+    out = std::move(q_.front());
+    q_.pop_front();
+    return true;
+  }
+  size_t read_available() const {
+    std::lock_guard<std::mutex> g{m_};
+    return q_.size();
+  }
+  bool empty() const { return read_available() == 0; }
+};
+
 // work_queue<T, spsc, fixed_size, capacity> as in the reference; spsc = false -> MPMC
 template <typename T, bool spsc = true, bool fixed_size = srtb::work_queue_fixed_size,
           size_t capacity = srtb::work_queue_capacity>
@@ -152,6 +183,18 @@ struct time_series_holder {
 struct write_signal_work : public write_file_work {
   std::vector<time_series_holder> time_series;  // non-empty <=> has_signal
   size_t zero_count = 0;
+};
+
+/** a [batch_size][count] complex dynamic spectrum on the device, to be turned into a waterfall thumbnail
+ *  (work.hpp:267-271); a write_signal_work converts to it */
+using simplify_spectrum_work = work<complex_ptr>;
+
+/** ARGB32 thumbnail of width * height pixels in host memory, row 0 = channel 0 (work.hpp:276-284) */
+struct draw_spectrum_work_2 {
+  std::shared_ptr<uint32_t> ptr;
+  uint32_t data_stream_id = 0;
+  size_t width = 0;
+  size_t height = 0;
 };
 
 }  // namespace work

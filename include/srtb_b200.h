@@ -257,6 +257,14 @@ const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int stream);
    process_block_dm_sweep (valid until the next call) */
 const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx);
 
+/* simplify_spectrum_pipe_2 (pipeline/spectrum_pipe.hpp:82-143): resample_spectrum_3 with norm(),
+ * normalize_with_average_value, generate_pixmap. d_spectrum is [in_height][in_width] complex64
+ * (time contiguous, as a block leaves it); d_intensity [out_height][out_width] floats receives the
+ * normalised intensity, d_pixmap the ARGB32 image; d_average (optional, 1 float) the average before scaling. */
+int srtb_b200_simplify_spectrum(srtb_b200_ctx* ctx, const void* d_spectrum, size_t in_width, size_t in_height,
+                                size_t out_width, size_t out_height, uint32_t argb_0, uint32_t argb_1,
+                                uint32_t argb_overflow, float* d_intensity, uint32_t* d_pixmap, float* d_average);
+
 #ifdef __cplusplus
 }
 #endif

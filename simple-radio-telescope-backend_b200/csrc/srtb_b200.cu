@@ -21,6 +21,7 @@
 #include "fft_engine.cuh"
 #include "fft_bigrow.cuh"
 #include "ops_kernels.cuh"
+#include "thumbnail.cuh"
 
 using namespace srtb_b200;
 
@@ -118,6 +119,11 @@ struct srtb_b200_ctx {
   float* chirp_tab = nullptr;
   size_t chirp_tab_bytes = 0;
   double chirp_tab_key[6] = {0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm
+  // simplify_spectrum: row-resampled intensities R[C][W] and the column stage's per-CTA partial sums
+  float* thumb_rows = nullptr;
+  size_t thumb_rows_bytes = 0;
+  float* thumb_partial = nullptr;
+  size_t thumb_partial_bytes = 0;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -292,6 +298,8 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   cudaFree(ctx->sweep_buf);
   cudaFree(ctx->sweep_res);
   cudaFree(ctx->chirp_tab);
+  cudaFree(ctx->thumb_rows);
+  cudaFree(ctx->thumb_partial);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
     cudaFree(ctx->slot_baseband[i]);
     for (auto& p : ctx->slot_stream_buf[i]) cudaFree(p);
@@ -2328,4 +2336,55 @@ extern "C" const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int st
 extern "C" const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx) {
   if (!ctx) return nullptr;
   return ctx->sweep_buf;
+}
+
+// ------------------------------------------------------------------------------------
+// waterfall thumbnail (simplify_spectrum_pipe_2): see thumbnail.cuh
+// ------------------------------------------------------------------------------------
+extern "C" int srtb_b200_simplify_spectrum(srtb_b200_ctx* ctx, const void* d_spectrum, size_t in_width,
+                                           size_t in_height, size_t out_width, size_t out_height, uint32_t argb_0,
+                                           uint32_t argb_1, uint32_t argb_overflow, float* d_intensity,
+                                           uint32_t* d_pixmap, float* d_average) {
+  API_LOCK(ctx);
+  if (!ctx || !d_spectrum || !d_intensity || !d_pixmap)
+    return fail(ctx, SRTB_B200_E_INVALID, "simplify_spectrum: null argument");
+  if (in_width == 0 || in_height == 0 || out_width == 0 || out_height == 0)
+    return fail(ctx, SRTB_B200_E_INVALID, "simplify_spectrum: zero size");
+  if (in_height > 0x7fffffffu || out_width > ((size_t)1 << 31))
+    return fail(ctx, SRTB_B200_E_INVALID, "simplify_spectrum: size exceeds the launch grid");
+  CK(cudaSetDevice(ctx->device));
+  // G threads per output pixel, about four input cells per thread; the CTA covers 256 / G pixels of one input row
+  const double ratio = (double)in_width / (double)out_width;
+  int G = 1;
+  while (G < 32 && 4.0 * (2 * G) <= ratio) G *= 2;
+  const size_t tiles = (out_width + THUMB_THREADS / G - 1) / (THUMB_THREADS / G);
+  if (tiles > 65535) return fail(ctx, SRTB_B200_E_INVALID, "simplify_spectrum: out_width too large for this in_width");
+  const size_t n = out_width * out_height;
+  const unsigned col_grid = (unsigned)std::min<size_t>(1024, (n + THUMB_THREADS - 1) / THUMB_THREADS);
+  void* rows = ctx->thumb_rows;
+  if (int rc = ensure(ctx, &rows, &ctx->thumb_rows_bytes, sizeof(float) * in_height * out_width)) return rc;
+  ctx->thumb_rows = static_cast<float*>(rows);
+  void* part = ctx->thumb_partial;
+  if (int rc = ensure(ctx, &part, &ctx->thumb_partial_bytes, sizeof(float) * col_grid)) return rc;
+  ctx->thumb_partial = static_cast<float*>(part);
+
+  const float2* spec = static_cast<const float2*>(d_spectrum);
+  const dim3 row_grid((unsigned)in_height, (unsigned)tiles);
+  if (in_width % 2 == 0 && (reinterpret_cast<uintptr_t>(d_spectrum) & 15u) == 0)
+    thumb_row_kernel<true><<<row_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(spec, in_width, out_width, G,
+                                                                           ctx->thumb_rows);
+  else
+    thumb_row_kernel<false><<<row_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(spec, in_width, out_width, G,
+                                                                            ctx->thumb_rows);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  thumb_col_kernel<<<col_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(ctx->thumb_rows, in_height, out_width, out_height,
+                                                                     d_intensity, ctx->thumb_partial);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  thumb_norm_kernel<<<grid_for(ctx, n, THUMB_THREADS, 4), THUMB_THREADS, 0, ctx->lane.stream>>>(
+      d_intensity, n, ctx->thumb_partial, (int)col_grid, argb_0, argb_1, argb_overflow, d_pixmap, d_average);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
 }

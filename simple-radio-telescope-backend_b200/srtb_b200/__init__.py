@@ -78,6 +78,12 @@ class SrtbError(RuntimeError):
         self.message = message
 
 
+# waterfall thumbnail colours (srtb::gui, include/srtb/config.hpp)
+GUI_OPAQUE = 0xFF000000
+GUI_COLOR_0 = 0xFF1F1E33
+GUI_COLOR_1 = 0xFF33E1F1
+GUI_COLOR_OVERFLOW = 0xFFE0E1CC
+
 # every symbol include/srtb_b200.h declares: (name, restype, argtypes)
 _P, _SZ, _F, _I = C.c_void_p, C.c_size_t, C.c_float, C.c_int
 SYMBOLS = {
@@ -116,6 +122,7 @@ SYMBOLS = {
     "srtb_b200_debug_set_submit_count": (_I, [_P, C.c_uint64]),
     "srtb_b200_block_spectrum": (_P, [_P, _I]),
     "srtb_b200_sweep_spectrum": (_P, [_P]),
+    "srtb_b200_simplify_spectrum": (_I, [_P, _P, _SZ, _SZ, _SZ, _SZ, C.c_uint32, C.c_uint32, C.c_uint32, _P, _P, _P]),
 }
 
 _lib = None
@@ -306,6 +313,16 @@ class Context:
     def sweep_spectrum_ptr(self) -> int:
         """test hook: device pointer of the last trial's dynamic spectrum (last stream) of the latest DM sweep"""
         return self.lib.srtb_b200_sweep_spectrum(self.h)
+
+    def simplify_spectrum(self, d_spectrum, in_width: int, in_height: int, out_width: int, out_height: int,
+                          d_intensity, d_pixmap, d_average=None, argb_0: int = GUI_COLOR_0,
+                          argb_1: int = GUI_COLOR_1, argb_overflow: int = GUI_COLOR_OVERFLOW):
+        """waterfall thumbnail of a [in_height][in_width] complex64 dynamic spectrum (simplify_spectrum_pipe_2):
+        d_intensity receives [out_height][out_width] normalised floats, d_pixmap the ARGB32 image, d_average (optional)
+        the average intensity before scaling"""
+        self._ck(self.lib.srtb_b200_simplify_spectrum(self.h, _ptr(d_spectrum), in_width, in_height, out_width,
+                                                      out_height, argb_0, argb_1, argb_overflow, _ptr(d_intensity),
+                                                      _ptr(d_pixmap), _ptr(d_average)))
 
 
 # host helpers (pure host arithmetic of the reference's pipes)

@@ -6,7 +6,10 @@
 // sink the seven device pipes run as the fused chain pipe (baseband_chain_pipe = srtb_b200_submit_block_ex /
 // collect_block_ex), several per GPU, and — new with respect to the reference, which drives one device
 // (main.cpp:99) — blocks are dealt round-robin over every visible GPU (block k -> GPU k mod G, SURVEY §8e; no
-// collective on the data path). GUI, spectrum thumbnails and the termination handler are out of scope.
+// collective on the data path). With gui_enable, the chain's spectra also feed a loose side branch per GPU
+// (main.cpp:197-201,220-228): simplify_spectrum_pipe_2 on that GPU makes the waterfall thumbnail and one sink writes it
+// to <baseband_output_file_prefix>waterfall.<data_stream_id>.ppm, replaced on every block (the headless counterpart of
+// the reference's refreshed window). The Qt window itself and the termination handler are out of scope.
 //
 // Extra options (not part of srtb::configs; consumed here before the reference-style parser sees argv):
 //   --gpu_devices 0,1,...   GPUs to use (default: all visible)      --chains_per_gpu N   chain pipes per GPU (default 2)
@@ -33,6 +36,7 @@
 #include "srtb/pipeline/framework/pipe.hpp"
 #include "srtb/pipeline/framework/pipe_io.hpp"
 #include "srtb/pipeline/read_file_pipe.hpp"
+#include "srtb/pipeline/spectrum_pipe.hpp"
 #include "srtb/pipeline/udp_receiver_pipe.hpp"
 #include "srtb/pipeline/write_file_pipe.hpp"
 #include "srtb/pipeline/write_signal_pipe.hpp"
@@ -46,6 +50,17 @@ void on_signal(int) { g_interrupted = true; }
 
 using copy_queue = srtb::work_queue<srtb::work::copy_to_device_work, false>;
 using output_queue = srtb::work_queue<srtb::work::write_signal_work, false>;
+using draw_queue = srtb::bounded_mpmc_queue<srtb::work::draw_spectrum_work_2>;
+
+/** writes each thumbnail as the stream's PPM; `written` counts them */
+struct waterfall_sink {
+  std::shared_ptr<std::atomic<uint64_t>> written;
+  std::optional<srtb::work::dummy_work> operator()(std::stop_token, srtb::work::draw_spectrum_work_2 w) {
+    srtb::pipeline::write_waterfall_ppm(w);
+    (*written)++;
+    return srtb::work::dummy_work{};
+  }
+};
 
 /** source -> per-GPU queues: block k goes to GPU k mod G (all streams of a block stay together) */
 struct round_robin_out_functor {
@@ -175,6 +190,11 @@ int main(int argc, char** argv) {
     std::fprintf(stderr, "srtb_b200: %s\n", e.what());
     return 2;
   }
+  if (cfg.gui_enable && (cfg.gui_pixmap_width == 0 || cfg.gui_pixmap_height == 0)) {
+    std::fprintf(stderr, "srtb_b200: gui_enable needs a non-zero gui_pixmap_width and gui_pixmap_height (got %zu x %zu)\n",
+                 (size_t)cfg.gui_pixmap_width, (size_t)cfg.gui_pixmap_height);
+    return 2;
+  }
 
   std::vector<int> devices;
   if (devices_opt.empty()) {
@@ -196,14 +216,38 @@ int main(int argc, char** argv) {
   std::vector<std::shared_ptr<copy_queue>> gpu_queues;
   std::vector<std::jthread> threads;
 
+  auto thumbnails_open = std::make_shared<std::atomic<bool>>(false);
+  auto thumbnails_accepted = std::make_shared<std::atomic<uint64_t>>(0);
+  auto thumbnails_written = std::make_shared<std::atomic<uint64_t>>(0);
+  auto thumbnails_dropped = std::make_shared<std::atomic<uint64_t>>(0);
+  // the sink's queue is bounded too: a thumbnail pipe waits for room, its own input queue fills, and then the side
+  // branch drops blocks, so a slow disk never holds more than a few images and spectra per GPU
+  auto draw_q = std::make_shared<draw_queue>(srtb::work_queue_capacity * devices.size());
+
   // device side: the fused chain, `chains_per_gpu` pipes per GPU on their own CUDA stream / context each
   for (int dev : devices) {
     gpu_queues.push_back(std::make_shared<copy_queue>());
-    for (int c = 0; c < chains_per_gpu; c++)
-      threads.push_back(start_pipe<baseband_chain_pipe>(idle_queue_in_functor{gpu_queues.back()},
-                                                        multiple_works_out_functor{queue_out_functor{out_q}},
-                                                        srtb::cuda_queue{dev}, false, ring_depth));
+    if (cfg.gui_enable) {
+      // the thumbnail side branch is offered each work before the sink's queue, so once the sink has seen a block
+      // that block's side-branch decision has been made
+      auto thumb_q = std::make_shared<thumbnail_out_functor::queue>(srtb::work_queue_capacity);
+      for (int c = 0; c < chains_per_gpu; c++)
+        threads.push_back(start_pipe<baseband_chain_pipe>(
+            idle_queue_in_functor{gpu_queues.back()},
+            multiple_works_out_functor{multiple_out_functors_functor{
+                thumbnail_out_functor{thumb_q, thumbnails_open, thumbnails_accepted, thumbnails_dropped}, queue_out_functor{out_q}}},
+            srtb::cuda_queue{dev}, false, ring_depth));
+      threads.push_back(start_pipe<simplify_spectrum_pipe_2>(queue_in_functor{thumb_q}, queue_out_functor{draw_q},
+                                                             srtb::cuda_queue{dev}));
+    } else {
+      for (int c = 0; c < chains_per_gpu; c++)
+        threads.push_back(start_pipe<baseband_chain_pipe>(idle_queue_in_functor{gpu_queues.back()},
+                                                          multiple_works_out_functor{queue_out_functor{out_q}},
+                                                          srtb::cuda_queue{dev}, false, ring_depth));
+    }
   }
+  if (cfg.gui_enable)
+    threads.push_back(start_pipe<waterfall_sink>(queue_in_functor{draw_q}, dummy_out_functor<>{}, thumbnails_written));
   // sink (main.cpp:206-216)
   srtb::cuda_queue q0{devices.front()};
   auto positives = std::make_shared<std::atomic<uint64_t>>(0);
@@ -248,6 +292,7 @@ int main(int argc, char** argv) {
     positives->store(0);
     SRTB_LOGI << " [main] " << "warmed up with " << pushed << " silent block(s)";
   }
+  thumbnails_open->store(true);
   const auto t0 = std::chrono::steady_clock::now();
   if (!synth_rate_opt.empty()) {
     // synthetic live stream (BASELINE config #5): one paced receiver, blocks dealt over the GPUs; ends after
@@ -278,6 +323,9 @@ int main(int argc, char** argv) {
     std::jthread source = start_pipe<read_file_pipe>(dummy_in_functor<>{}, rr);
     source.join();  // the pipe thread ends when the file has been read
     while (done->load() < submitted->load() * streams && !g_interrupted) std::this_thread::yield();
+    // every block has reached the sink, so the side branch has taken all it will: let its thumbnails be written
+    while (thumbnails_written->load() < thumbnails_accepted->load() && !g_interrupted)
+      std::this_thread::sleep_for(std::chrono::milliseconds(1));
   } else {
     std::vector<std::jthread> sources;
     for (size_t i = 0; i < cfg.udp_receiver_address.size(); i++) {
@@ -297,6 +345,10 @@ int main(int argc, char** argv) {
   std::fprintf(stderr, "[srtb_b200] %llu block(s) x %zu stream(s) of %zu samples in %.3f s = %.2f Gsamples/s\n",
                (unsigned long long)submitted->load(), streams, (size_t)cfg.baseband_input_count, dt,
                (double)submitted->load() * (double)streams * (double)cfg.baseband_input_count / dt / 1e9);
+  if (cfg.gui_enable)
+    std::fprintf(stderr, "[srtb_b200] waterfall: %llu thumbnail(s) written, %llu block(s) skipped while the thumbnail "
+                 "pipe was busy\n", (unsigned long long)thumbnails_written->load(),
+                 (unsigned long long)thumbnails_dropped->load());
   for (auto& t : threads) t.request_stop();
   threads.clear();
   srtb::device_allocator.deallocate_all_free_ptrs();
