@@ -15,6 +15,9 @@
  *     re-sized when a call's size differs (mirrors fft_wrapper::set_size re-planning,
  *     fft/fft_wrapper.hpp:106-113);
  *   - return value 0 = ok, negative = srtb_b200_status; text via srtb_b200_last_error.
+ *   - alignment: a complex64 (float2) pointer must be 8-byte aligned, so any element of a cudaMalloc'd array
+ *     (x + 1 included) is accepted; a misaligned one returns SRTB_B200_E_INVALID before any launch. 16-byte
+ *     alignment only selects the faster 16-byte-load / TMA routes. Stricter rules are stated per entry below.
  *   - there is NO CPU fallback: without a CUDA device ctx_create fails;
  *   - a ctx may be shared by several host threads (the reference copies one sycl::queue into every pipe): each entry
  *     locks the ctx while it plans and enqueues, waits (synchronize, collect_block) run unlocked;
@@ -114,25 +117,31 @@ const char* srtb_b200_version(void);
  * (unpack.hpp:171-197,221-244,255-283,293-403; bits dispatch pipeline/unpack_pipe.hpp:72-127)
  * bits: 1,2,4,8 unsigned; -8 int8; 16/-16; 32 float; 64 double.
  * out_count: samples PER OUTPUT STREAM; d_out[s] must hold out_count (+2 for in-place R2C) floats.
+ * Alignment (else SRTB_B200_E_INVALID before any launch): SIMPLE: d_in aligned to the sample width (any byte for
+ * 1/2/4/8-bit samples, 2 bytes for 16-bit, 4 for 32-bit, 8 for 64-bit), d_out[0] 4-byte aligned; the multi-stream
+ * formats: d_in and every d_out[s] 16-byte aligned.
  * streams written: 1 (SIMPLE), 2 (INTERLEAVED_2, SNAP1, GZNUPSR_A1_2), 4 (GZNUPSR_A1_4). */
 int srtb_b200_unpack(srtb_b200_ctx* ctx, const void* d_in, size_t in_bytes, int bits, int format,
                      int window, float* const d_out[4], size_t out_count);
 
 /* ---- fft_1d_dispatcher<R2C_1D>::process (fft/fft.hpp:146-149; naive_fft.hpp:221-261) ----
- * in place on n_real + 2 floats: X[k], k = 0..n_real/2, unnormalised, forward sign. */
+ * in place on n_real + 2 floats: X[k], k = 0..n_real/2, unnormalised, forward sign.
+ * n_real: power of two, 2 .. 2^31. d_inout is read as complex64: it must be 8-byte aligned (a float
+ * pointer at +4 bytes returns SRTB_B200_E_INVALID). */
 int srtb_b200_fft_r2c_inplace(srtb_b200_ctx* ctx, float* d_inout, size_t n_real);
 
 /* ---- batched C2C, unnormalised, in place (fft_1d_dispatcher<C2C_1D_*>; naive_fft.hpp:155-176) ----
- * direction +1 forward (e^-i), -1 backward (e^+i). d_x is [batch][length] complex64. */
+ * direction +1 forward (e^-i), -1 backward (e^+i). d_x is [batch][length] complex64, 8-byte aligned.
+ * length: power of two up to 2^30; batch * length up to 2^34 (else SRTB_B200_E_SIZE). */
 int srtb_b200_fft_c2c(srtb_b200_ctx* ctx, void* d_x, size_t length, size_t batch, int direction);
 
-/* watfft_1d_c2c_pipe (pipeline/fft_pipe.hpp:313-371): batch backward C2C of `length` */
+/* watfft_1d_c2c_pipe (pipeline/fft_pipe.hpp:313-371): batch backward C2C of `length` (rules of srtb_b200_fft_c2c) */
 int srtb_b200_watfft_c2c_backward(srtb_b200_ctx* ctx, void* d_x, size_t length, size_t batch);
 
 /* ---- rfi_mitigation_s1_pipe (pipeline/rfi_mitigation_pipe.hpp:43-101) ---------------
  * mean m of |X|^2; X = (|X|^2 > avg_threshold*m) ? 0 : X*norm_coef; then zero the
  * inclusive bin ranges h_bin_ranges[n_ranges][2] (spectrum/rfi_mitigation.hpp:137-143).
- * d_mean_out (optional device float) receives m. */
+ * d_mean_out (optional device float) receives m. d_x: 8-byte aligned complex64. */
 int srtb_b200_rfi_s1(srtb_b200_ctx* ctx, void* d_x, size_t count, float avg_threshold,
                      float norm_coef, const size_t* h_bin_ranges, size_t n_ranges,
                      float* d_mean_out);
@@ -143,7 +152,8 @@ size_t srtb_b200_eval_rfi_ranges(const char* freq_list, float* pairs, size_t max
 int srtb_b200_rfi_range_to_bins(float f1, float f2, float freq_low, float bandwidth, size_t in_count,
                                 size_t* lo, size_t* hi); /* rfi_mitigation.hpp:102-143; 1 = applied */
 
-/* ---- coherent_dedispertion (coherent_dedispersion.hpp:133-150,223-237) --------------- */
+/* ---- coherent_dedispertion (coherent_dedispersion.hpp:133-150,223-237) ---------------
+ * d_x: 8-byte aligned complex64. */
 int srtb_b200_dedisperse(srtb_b200_ctx* ctx, void* d_x, size_t count, float f_min, float f_c,
                          float df, float dm);
 /* nsamps_reserved (coherent_dedispersion.hpp:76-128) */
@@ -152,14 +162,14 @@ size_t srtb_b200_nsamps_reserved(size_t baseband_input_count, size_t spectrum_ch
                                  int reserve_sample);
 
 /* ---- mitigate_rfi_spectral_kurtosis_method_2 (spectrum/rfi_mitigation.hpp:292-341) ----
- * d_x is [chan_count][time_count]. d_sk_out (optional, chan_count floats) receives sk. */
+ * d_x is [chan_count][time_count], 8-byte aligned complex64. d_sk_out (optional, chan_count floats) receives sk. */
 int srtb_b200_rfi_s2_sk(srtb_b200_ctx* ctx, void* d_x, size_t time_count, size_t chan_count,
                         float sk_threshold, float* d_sk_out);
 
 /* ---- signal_detect_pipe_2 (pipeline/signal_detect_pipe.hpp:252-442) -------------------
  * h_series: NULL, or host buffer of SRTB_B200_MAX_BOXCARS * time_count floats; row i receives
  * the series of entry i when signal_count[i] > 0 (all entries if copy_all != 0).
- * Synchronises the stream. */
+ * d_x: [chan_count][time_count], 8-byte aligned complex64. Synchronises the stream. */
 int srtb_b200_signal_detect(srtb_b200_ctx* ctx, const void* d_x, size_t time_count,
                             size_t chan_count, size_t time_reserved_count, float snr_threshold,
                             float channel_threshold, size_t max_boxcar_length,
@@ -169,13 +179,13 @@ int srtb_b200_signal_detect(srtb_b200_ctx* ctx, const void* d_x, size_t time_cou
  * [time][frequency], as refft_1d_c2c_pipe leaves them (pipeline/fft_pipe.hpp:197-278) ------------------------------
  * mitigate_rfi_spectral_kurtosis_method (v1, spectrum/rfi_mitigation.hpp:181-275, normalization = false):
  * d_x is [time_counts][fft_bins]; every frequency column whose sk = M s4 / s2^2 over the time_counts spectra leaves
- * the thresholds is zeroed. d_sk_out (optional, fft_bins floats) receives sk. */
+ * the thresholds is zeroed. d_sk_out (optional, fft_bins floats) receives sk. d_x: 8-byte aligned complex64. */
 int srtb_b200_rfi_sk_v1(srtb_b200_ctx* ctx, void* d_x, size_t fft_bins, size_t time_counts, float sk_threshold,
                         float* d_sk_out);
 /* signal_detect_pipe (v1, pipeline/signal_detect_pipe.hpp:51-230): SK v1 in place, masked channels counted over the
  * first spectrum, one time-series value per spectrum (sum over its count_per_batch bins of |x|^2), mean removal,
  * count_signal, boxcars 2..max (series lengths batch_size - boxcar; nothing is trimmed). h_series rows are
- * batch_size floats apart. Synchronises the stream. */
+ * batch_size floats apart. d_x: 8-byte aligned complex64. Synchronises the stream. */
 int srtb_b200_signal_detect_v1(srtb_b200_ctx* ctx, void* d_x, size_t count_per_batch, size_t batch_size,
                                float sk_threshold, float snr_threshold, float channel_threshold,
                                size_t max_boxcar_length, srtb_b200_detect_result* h_result, float* h_series,
@@ -204,7 +214,11 @@ typedef struct {
  * format says; the call copies them to the device, runs every stage for every stream and
  * fills h_results[stream]. d_spectrum_out (optional): per-stream device pointers that
  * receive the dynamic spectrum [C][L] (else it stays in ctx scratch).
- * Returns the number of streams processed (>0) or a negative status. */
+ * Returns the number of streams processed (>0) or a negative status.
+ * Baseband alignment (the rules of srtb_b200_unpack): a SIMPLE baseband must be aligned to its sample width (any
+ * byte address for 1/2/4/8-bit samples, 2/4/8 bytes for 16/32/64-bit ones). The two- and four-stream formats
+ * (INTERLEAVED_2, NAOCPSR_SNAP1, GZNUPSR_A1_2, GZNUPSR_A1_4) need a 16-byte aligned baseband pointer. A pointer that
+ * breaks the rule returns SRTB_B200_E_INVALID. The same holds for submit_block_device / submit_block_ex. */
 int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
                             const void* h_baseband, size_t baseband_bytes,
                             srtb_b200_detect_result* h_results, float* h_series, int copy_all);
@@ -235,7 +249,8 @@ int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_c
  * (SRTB_B200_RING_SLOTS - 1 further submissions). */
 #define SRTB_B200_RING_SLOTS 3
 typedef struct {
-  float* d_spectrum[4]; /* per stream: device buffer of baseband_input_count + 2 floats, 16-byte aligned        */
+  float* d_spectrum[4]; /* per stream: device buffer of baseband_input_count + 2 floats, 16-byte aligned
+                           (else submit_block_ex returns SRTB_B200_E_INVALID before it enqueues anything)        */
   float* h_series;      /* pinned (cudaMallocHost / cudaHostRegister) host buffer,
                            [streams][SRTB_B200_MAX_BOXCARS][L] floats; only positive series are written          */
 } srtb_b200_block_outputs;

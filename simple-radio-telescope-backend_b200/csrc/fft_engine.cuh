@@ -1068,8 +1068,8 @@ struct col16_smem {
 // L x T box at (row a*L, column b0) of the 2-D tensor [A*L][B]; ONE TMA box load (per 256 rows) brings
 // it into shared memory in exactly the column-mode layout [idx][t], double buffered across tiles.
 // Stores go straight from registers with the inter-pass twiddle W_{L*B}^{k b} applied.
-// RAW != 0 (process_block only) fuses the unpack pipe into this first pass of the packed real
-// transform: the tensor map then describes the 8-bit baseband bytes, a tile is L x (T*G) bytes
+// The raw first pass (unpack fused in) exists on the sixteen-point kernel only (fft_col16_tma_kernel, RAW != 0):
+// the tensor map then describes the 8-bit baseband bytes, a tile is L x (T*G) bytes
 // (G = bytes per complex point: 2 for one stream, 4 when two streams share the block) and stage 0
 // converts the two samples at byte offsets o0/o1 of each group to float (K1's integer -> f32 cast,
 // exact) instead of reading complex64 that a separate kernel would have written and this one re-read.
@@ -1083,11 +1083,10 @@ struct raw_params {
   int bits;       // RAW 3: bits per sample
 };
 
-template <int LOGL, int T, bool FWD, int RAW = 0 /* 0 = complex64, 1 = int8 pairs, 2 = uint8 pairs */>
+template <int LOGL, int T, bool FWD>
 __global__ void __launch_bounds__(pass_threads<LOGL, T>::value, pass_threads<LOGL, T>::min_blocks)
     fft_col_tma_kernel(const __grid_constant__ tensor_map_blob tmap, float2* __restrict__ out, size_t B,
-                       uint32_t btiles, uint32_t ntiles, big_twiddle btw, const float2* __restrict__ tw,
-                       raw_params rp) {
+                       uint32_t btiles, uint32_t ntiles, big_twiddle btw, const float2* __restrict__ tw) {
   using SC = sched<LOGL>;
   constexpr int L = 1 << LOGL, U = L / 8, S = SC::S, BUF = tile_tma_smem<LOGL, T>::BUF;
   constexpr int ROWS_PER_BOX = (L < 256) ? L : 256;
@@ -1095,9 +1094,6 @@ __global__ void __launch_bounds__(pass_threads<LOGL, T>::value, pass_threads<LOG
   float2* const buf0 = reinterpret_cast<float2*>(smraw);
   float2* const buf1 = buf0 + BUF;
   uint64_t* const mbar = reinterpret_cast<uint64_t*>(buf1 + BUF);
-  // RAW: buf0 is the exchange buffer, buf1 is carved into two raw-byte tiles of T*L*4 bytes each
-  unsigned char* const raw0 = reinterpret_cast<unsigned char*>(buf1);
-  unsigned char* const raw1 = raw0 + (size_t)BUF * 4;
   float2* const ltw = reinterpret_cast<float2*>(smraw + tile_tma_smem<LOGL, T>::data_bytes + 128);
   float2* const stw = ltw + L;
   const int tid = threadIdx.x;
@@ -1113,42 +1109,24 @@ __global__ void __launch_bounds__(pass_threads<LOGL, T>::value, pass_threads<LOG
   auto issue = [&](uint32_t tl, int b) {
     const uint32_t a = tl / btiles, b0 = (tl % btiles) * T;
     fence_proxy_async();
-    if constexpr (RAW == 0) {
-      float2* dst = b ? buf1 : buf0;
-      mbar_expect_tx(&mbar[b], (uint32_t)(BUF * sizeof(float2)));
+    float2* dst = b ? buf1 : buf0;
+    mbar_expect_tx(&mbar[b], (uint32_t)(BUF * sizeof(float2)));
 #pragma unroll
-      for (int r = 0; r < L; r += ROWS_PER_BOX)
-        tma_load_2d(dst + r * T, &tmap, (int)b0, (int)(a * L + r), &mbar[b]);
-    } else {
-      unsigned char* dst = b ? raw1 : raw0;
-      mbar_expect_tx(&mbar[b], (uint32_t)(BUF * rp.G));
-#pragma unroll
-      for (int r = 0; r < L; r += ROWS_PER_BOX)
-        tma_load_2d(dst + (size_t)r * T * rp.G, &tmap, (int)(b0 * rp.G), (int)(a * L + r), &mbar[b]);
-    }
+    for (int r = 0; r < L; r += ROWS_PER_BOX)
+      tma_load_2d(dst + r * T, &tmap, (int)b0, (int)(a * L + r), &mbar[b]);
   };
   uint32_t tile = blockIdx.x;
   if (tile < ntiles && tid == 0) issue(tile, 0);
   for (uint32_t it = 0; tile < ntiles; tile += gridDim.x, it++) {
     const int b = it & 1;
-    float2* const sm = (RAW == 0) ? (b ? buf1 : buf0) : buf0;
+    float2* const sm = b ? buf1 : buf0;
     const uint32_t nxt = tile + gridDim.x;
     if (nxt < ntiles && tid == 0) issue(nxt, b ^ 1);
     mbar_wait(&mbar[b], (it >> 1) & 1);
     float2 v[8];
     int oidx[8];
-    if constexpr (RAW == 0) {
 #pragma unroll
-      for (int e = 0; e < 8; e++) v[e] = sm[(u + e * U) * T + t];
-    } else {
-      const unsigned char* rawb = (b ? raw1 : raw0) + (size_t)t * rp.G;
-#pragma unroll
-      for (int e = 0; e < 8; e++) {
-        const unsigned char* g = rawb + (size_t)(u + e * U) * T * rp.G;
-        if (RAW == 1) v[e] = make_float2((float)(int)(signed char)g[rp.o0], (float)(int)(signed char)g[rp.o1]);
-        else v[e] = make_float2((float)g[rp.o0], (float)g[rp.o1]);
-      }
-    }
+    for (int e = 0; e < 8; e++) v[e] = sm[(u + e * U) * T + t];
     stage_compute<LOGL, SC::logr(0), 0, FWD>(v, u, tw, oidx);
     if constexpr (S > 1) {
       __syncthreads();

@@ -367,6 +367,8 @@ __device__ __forceinline__ float2 r2c_twiddle(size_t k, size_t M) {
 // ------------------------------------------------------------------------------
 // reductions
 // ------------------------------------------------------------------------------
+__host__ __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
@@ -454,6 +456,7 @@ __global__ void __launch_bounds__(256) r2c_post_kernel(float2* __restrict__ H, s
 // K9 mean of |X|^2 (S/algorithm/map_reduce.hpp:84-91 over rfi_mitigation_pipe.hpp:53-60).
 // fp32 per-thread partials, fp64 combine, deterministic: per-CTA partials are summed in
 // index order by the last CTA to finish. mean = float(sum) / float(count).
+// A spectrum that is only 8-byte aligned (a complex64 view starting at an odd element) is read one element at a time.
 __global__ void __launch_bounds__(256) power_sum_kernel(const float2* __restrict__ x, size_t count,
                                                         double* __restrict__ partial,
                                                         unsigned* __restrict__ ticket,
@@ -465,6 +468,13 @@ __global__ void __launch_bounds__(256) power_sum_kernel(const float2* __restrict
   float acc0 = 0.f, acc1 = 0.f;
   const float4* x4 = reinterpret_cast<const float4*>(x);
   size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (!aligned16(x)) {
+    for (size_t j = i; j < count; j += stride) {
+      const float2 v = x[j];
+      acc0 += v.x * v.x + v.y * v.y;
+    }
+    i = pairs;  // skip the vector loops and the odd tail below
+  }
   for (; i + 3 * stride < pairs; i += 4 * stride) {   // four loads in flight per thread
     const float4 a = x4[i], b = x4[i + stride], c = x4[i + 2 * stride], d = x4[i + 3 * stride];
     acc0 += (a.x * a.x + a.y * a.y) + (b.x * b.x + b.y * b.y);
@@ -477,7 +487,7 @@ __global__ void __launch_bounds__(256) power_sum_kernel(const float2* __restrict
     acc0 += v.x * v.x + v.y * v.y;
     acc1 += v.z * v.z + v.w * v.w;
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0 && (count & 1)) {
+  if (blockIdx.x == 0 && threadIdx.x == 0 && (count & 1) && aligned16(x)) {
     const float2 v = x[count - 1];
     acc0 += v.x * v.x + v.y * v.y;
   }
@@ -507,6 +517,15 @@ __global__ void __launch_bounds__(256) rfi_s1_apply_kernel(float2* __restrict__ 
                                                            float threshold, float coef) {
   const float limit = threshold * (*mean);
   const size_t stride = (size_t)gridDim.x * blockDim.x;
+  if (!aligned16(x)) {  // 8-byte aligned spectrum: one element per load
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) {
+      float2 v = x[i];
+      if (v.x * v.x + v.y * v.y > limit) v = make_float2(0.f, 0.f);
+      else { v.x *= coef; v.y *= coef; }
+      x[i] = v;
+    }
+    return;
+  }
   const size_t pairs = count / 2;
   float4* x4 = reinterpret_cast<float4*>(x);
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < pairs; i += stride) {
@@ -556,6 +575,18 @@ __global__ void __launch_bounds__(256) dedisperse_kernel(const float2* in, float
   const size_t pairs = count / 2;
   const double inv_fc = 1.0 / f_c;
   const float limit = S1 ? threshold * (*mean) : 0.f;
+  if (!aligned16(in) || !aligned16(x)) {  // 8-byte aligned spectra: one element per load
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += stride) {
+      float2 v = in[i];
+      if (S1) {
+        if (v.x * v.x + v.y * v.y > limit) v = make_float2(0.f, 0.f);
+        else { v.x *= coef; v.y *= coef; }
+      }
+      const float2 w = chirp_factor(f_min, df, inv_fc, f_c, ddm, (unsigned)i);
+      x[i] = make_float2(v.x * w.x - v.y * w.y, v.x * w.y + v.y * w.x);
+    }
+    return;
+  }
   float4* x4 = reinterpret_cast<float4*>(x);
   const float4* in4 = reinterpret_cast<const float4*>(in);
   auto one = [&](float4 v, size_t i) {
@@ -600,7 +631,7 @@ __global__ void __launch_bounds__(256) sk_kernel(float2* __restrict__ x, size_t 
   float s2 = 0.f, s4 = 0.f;
   const size_t pairs = time_count / 2;
   const float4* r4 = reinterpret_cast<const float4*>(row);
-  const bool vec = ((((size_t)blockIdx.x * time_count) & 1) == 0);
+  const bool vec = aligned16(row);
   if (vec) {
     size_t i = threadIdx.x;
     const size_t bd = blockDim.x;
@@ -683,6 +714,7 @@ __global__ void __launch_bounds__(256) sk_decide_kernel(const float2* __restrict
 // K17 stage 1: partial column sums over a chunk of channels. Thread = 2 adjacent time
 // samples (one float4 load), lanes along time (coalesced); blockIdx.y = channel chunk.
 // zap (optional): rows flagged by sk_decide_kernel are zeroed here (K15) instead of being added.
+// Rows that are not 16-byte aligned (odd time_count, or an 8-byte aligned spectrum) take two float2 loads.
 __global__ void __launch_bounds__(256) colsum_partial_kernel(float2* __restrict__ x,
                                                              size_t time_count, size_t chan_count,
                                                              size_t ts_count, size_t rows_per_chunk,
@@ -696,7 +728,7 @@ __global__ void __launch_bounds__(256) colsum_partial_kernel(float2* __restrict_
   const size_t c1 = min(c0 + rows_per_chunk, chan_count);
   float a0 = 0.f, a1 = 0.f;
   const bool two = (j2 + 1 < time_count);
-  const bool vec = ((time_count & 1) == 0);
+  const bool vec = ((time_count & 1) == 0) && aligned16(x);  // then every row, and j2, is 16-byte aligned
   if (vec && two) {
 #pragma unroll 8
     for (size_t c = c0; c < c1; c++) {
@@ -728,74 +760,6 @@ __global__ void __launch_bounds__(256) colsum_partial_kernel(float2* __restrict_
     float* p = partial + (size_t)blockIdx.y * ts_count + j2;
     p[0] = a0;
     if (j2 + 1 < ts_count) p[1] = a1;
-  }
-}
-
-// K14 + K15 + K17 stage 1 fused (process_block only): one sweep over the dynamic spectrum computes
-// every row's spectral kurtosis, zeroes the flagged rows AND accumulates the partial column sums
-// of the surviving rows, so the detector does not read the spectrum again.
-// CTA = rows_per_chunk consecutive channel rows; thread owns NJ float4 (2*NJ time samples) per row.
-template <int NJ>
-__global__ void __launch_bounds__(256) sk_colsum_kernel(float2* __restrict__ x, size_t time_count,
-                                                        size_t chan_count, size_t ts_count,
-                                                        size_t rows_per_chunk, float thr_lo, float thr_hi,
-                                                        float* __restrict__ partial) {
-  __shared__ float sm2[8], sm4[8];
-  __shared__ int s_zap;
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  const size_t c0 = (size_t)blockIdx.x * rows_per_chunk;
-  const size_t c1 = min(c0 + rows_per_chunk, chan_count);
-  float acc[2 * NJ];
-#pragma unroll
-  for (int j = 0; j < 2 * NJ; j++) acc[j] = 0.f;
-  for (size_t c = c0; c < c1; c++) {
-    float4* row4 = reinterpret_cast<float4*>(x + c * time_count);
-    float4 v[NJ];
-#pragma unroll
-    for (int j = 0; j < NJ; j++) v[j] = row4[tid + 256 * j];
-    float p[2 * NJ];
-    float s2 = 0.f, s4 = 0.f;
-#pragma unroll
-    for (int j = 0; j < NJ; j++) {
-      p[2 * j] = v[j].x * v[j].x + v[j].y * v[j].y;
-      p[2 * j + 1] = v[j].z * v[j].z + v[j].w * v[j].w;
-      s2 += p[2 * j] + p[2 * j + 1];
-      s4 += p[2 * j] * p[2 * j] + p[2 * j + 1] * p[2 * j + 1];
-    }
-    s2 = warp_sum(s2);
-    s4 = warp_sum(s4);
-    if (lane == 0) {
-      sm2[wid] = s2;
-      sm4[wid] = s4;
-    }
-    __syncthreads();
-    if (wid == 0) {
-      float a = (lane < 8) ? sm2[lane] : 0.f, b = (lane < 8) ? sm4[lane] : 0.f;
-      a = warp_sum(a);
-      b = warp_sum(b);
-      if (lane == 0) {
-        const float sk = (float)time_count * (b / (a * a));
-        s_zap = (sk > thr_hi || sk < thr_lo) ? 1 : 0;
-      }
-    }
-    __syncthreads();
-    if (s_zap) {
-#pragma unroll
-      for (int j = 0; j < NJ; j++) row4[tid + 256 * j] = make_float4(0.f, 0.f, 0.f, 0.f);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 2 * NJ; j++) acc[j] += p[j];
-    }
-  }
-  float* out = partial + (size_t)blockIdx.x * ts_count;
-#pragma unroll
-  for (int j = 0; j < NJ; j++) {
-    const size_t col = 2 * ((size_t)tid + 256 * j);
-    if (col + 1 < ts_count) {
-      *reinterpret_cast<float2*>(out + col) = make_float2(acc[2 * j], acc[2 * j + 1]);
-    } else if (col < ts_count) {
-      out[col] = acc[2 * j];
-    }
   }
 }
 

@@ -206,6 +206,7 @@ static int ensure_colsum_partial(srtb_b200_ctx* ctx, size_t elems) {
 }
 
 static inline bool is_pow2(size_t n) { return n && !(n & (n - 1)); }
+static inline bool aligned8(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7u) == 0; }
 static inline int ilog2(size_t n) {
   int k = 0;
   while (((size_t)1 << k) < n) k++;
@@ -413,6 +414,13 @@ extern "C" int srtb_b200_unpack(srtb_b200_ctx* ctx, const void* d_in, size_t in_
     return fail(ctx, SRTB_B200_E_INVALID, "unpack: in_bytes too small for out_count");
   for (int s = 0; s < streams; s++)
     if (!d_out[s]) return fail(ctx, SRTB_B200_E_INVALID, "unpack: null output stream");
+  if (streams == 1) {
+    // the scalar fall-back loads one sample at a time: 16/32/64-bit samples need their natural alignment
+    const uintptr_t width = abits >= 16 ? (uintptr_t)(abits / 8) : 1u;
+    if (reinterpret_cast<uintptr_t>(d_in) % width)
+      return fail(ctx, SRTB_B200_E_INVALID, "unpack: d_in is not aligned to the " + std::to_string(width) + "-byte sample width");
+    if (reinterpret_cast<uintptr_t>(d_out[0]) & 3u) return fail(ctx, SRTB_B200_E_INVALID, "unpack: d_out[0] is not 4-byte aligned");
+  }
   if (streams > 1) {
     // the multi-stream kernels move 8/16-byte words: the board formats are int8 only, whole 4-sample words, and
     // every buffer 16-byte aligned (the single-stream path has a scalar fall-back, these do not)
@@ -722,8 +730,8 @@ static int launch_col_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, siz
     constexpr int threads = col16_threads<LOGL, T>::value;
     const size_t smem16 = col16_smem<LOGL, T, false>::bytes(btw.q);
     if (int rc = persistent_grid(ctx, kern16, threads, smem16, col16_smem<LOGL, T, false>::bytes(10), ntiles, &grid)) return rc;
-    if constexpr (!FWD) {
-      if (chirp) {  // s1 + chirp applied as the tile is read (long waterfall rows)
+    if constexpr (!FWD && LOGL >= 8) {
+      if (chirp) {  // s1 + chirp applied as the tile is read (long waterfall rows: a 2^8 or 2^9 first sweep)
         auto kernc = fft_col16_tma_kernel<LOGL, T, FWD, 0, true>;
         if (int rc = persistent_grid(ctx, kernc, threads, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
         CK(launch_pdl(ctx, kernc, dim3(grid), dim3(threads), smem, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
@@ -733,6 +741,8 @@ static int launch_col_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, siz
         *done = true;
         return 0;
       }
+    } else {
+      if (chirp) return 0;  // no chirp-on-load kernel for a 2^7 column sweep (nor for a forward one)
     }
     CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
                   raw_params{}, row_chirp_params{}));
@@ -740,7 +750,7 @@ static int launch_col_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, siz
     if (chirp) return 0;  // the chirp-on-load sweep exists for the sixteen-point kernel only
     auto kern = fft_col_tma_kernel<LOGL, T, FWD>;
     if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, raw_params{});
+    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw);
   }
   ctx->launches++;
   CK(cudaGetLastError());
@@ -757,8 +767,12 @@ struct raw_source {
   bool is_signed = true;
 };
 
+// the first sweep of the packed R2C plans that take the raw route is 2^7 .. 2^9 points long (plan3 / plan4 on a
+// 16-byte aligned buffer; the two-sweep plans with a first sweep of 2^10 end on a 2^9 or 2^10 last sweep, which has no
+// fused R2C split)
 template <int LOGL, int RAW, int TT = col_t<LOGL>::value>
 static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2* out, size_t B, bool* done) {
+  static_assert(LOGL >= 7 && LOGL <= 9, "raw first sweep: sixteen-point column kernel only");
   constexpr int T = TT, L = 1 << LOGL;
   if constexpr (LOGL == 7 && TT == col_t<LOGL>::value) {
     if (wide_col(1, L, B)) return launch_col_tma_raw<LOGL, RAW, 32>(ctx, src, out, B, done);
@@ -782,21 +796,12 @@ static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2*
   const size_t ntiles = B / T;
   unsigned grid = 1;
   const raw_params rp{src.G, src.o0, src.o1, src.delta, (int)row_bytes, src.bits};
-  if constexpr (LOGL >= 7 && LOGL <= 9) {
-    auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
-    constexpr int threads = col16_threads<LOGL, T>::value;
-    constexpr size_t smem16 = raw16_smem<LOGL, T>::bytes;  // inter-sweep tables stay in global memory here
-    if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
-    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
-                  row_chirp_params{}));
-  } else if constexpr (RAW == 3) {
-    return 0;  // packed samples: sixteen-point kernel only
-  } else {
-    if (src.delta) return 0;
-    auto kern = fft_col_tma_kernel<LOGL, T, true, RAW>;
-    if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp);
-  }
+  auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
+  constexpr int threads = col16_threads<LOGL, T>::value;
+  constexpr size_t smem16 = raw16_smem<LOGL, T>::bytes;  // inter-sweep tables stay in global memory here
+  if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
+  CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
+                row_chirp_params{}));
   ctx->launches++;
   CK(cudaGetLastError());
   *done = true;
@@ -816,7 +821,6 @@ static int dispatch_col_raw(srtb_b200_ctx* ctx, int logl, const raw_source& src,
     case 7: return src.is_signed ? launch_col_tma_raw<7, 1>(ctx, src, out, B, done) : launch_col_tma_raw<7, 2>(ctx, src, out, B, done);
     case 8: return src.is_signed ? launch_col_tma_raw<8, 1>(ctx, src, out, B, done) : launch_col_tma_raw<8, 2>(ctx, src, out, B, done);
     case 9: return src.is_signed ? launch_col_tma_raw<9, 1>(ctx, src, out, B, done) : launch_col_tma_raw<9, 2>(ctx, src, out, B, done);
-    case 10: return src.is_signed ? launch_col_tma_raw<10, 1>(ctx, src, out, B, done) : launch_col_tma_raw<10, 2>(ctx, src, out, B, done);
     default: return 0;
   }
 }
@@ -990,9 +994,8 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
     if (sk && chirp && chirp->newton == 3) return go(fft_bigrow_kernel<LOGL, false, true, 3>, true);
     if (sk && chirp && chirp->newton == 4) return go(fft_bigrow_kernel<LOGL, false, true, 4>, true);
     if (sk && chirp) return go(fft_bigrow_kernel<LOGL, false, true, 2>, true);
-    if (sk) return go(fft_bigrow_kernel<LOGL, false, true, 0>, true);
   }
-  if (sk || chirp) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "fft: fused epilogue exists for the backward transform only");
+  if (sk || chirp) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "fft: fused epilogue exists for the backward transform with the chirp only");
   return go(fft_bigrow_kernel<LOGL, FWD, false, 0>, false);
 }
 
@@ -1033,8 +1036,6 @@ static int fft_c2c_impl(srtb_b200_ctx* ctx, float2* x, size_t n, size_t batch) {
                    : launch_bigrow<14, FWD>(ctx, x, x, batch, nullptr, nullptr, nullptr);
   }
   if (q > 30) return fail(ctx, SRTB_B200_E_SIZE, "fft: length above 2^30 not supported");
-  if (batch * n > ((size_t)1 << 32) * 4)
-    return fail(ctx, SRTB_B200_E_SIZE, "fft: batch * length too large");
   if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, batch * n * sizeof(float2))) return rc;
   float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
   if (q <= 20) {
@@ -1069,9 +1070,12 @@ static int fft_c2c_impl(srtb_b200_ctx* ctx, float2* x, size_t n, size_t batch) {
 extern "C" int srtb_b200_fft_c2c(srtb_b200_ctx* ctx, void* d_x, size_t length, size_t batch, int direction) {
   API_LOCK(ctx);
   if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "fft_c2c: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "fft_c2c: d_x is not 8-byte aligned");
   if (length == 0 || batch == 0) return fail(ctx, SRTB_B200_E_INVALID, "fft_c2c: zero size");
   if (!is_pow2(length))
     return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(length));
+  if (length > ((size_t)1 << 30)) return fail(ctx, SRTB_B200_E_SIZE, "fft: length above 2^30 not supported");
+  if (batch > ((size_t)1 << 34) / length) return fail(ctx, SRTB_B200_E_SIZE, "fft: batch * length above 2^34");
   if (direction != 1 && direction != -1) return fail(ctx, SRTB_B200_E_INVALID, "fft_c2c: direction must be +1 / -1");
   CK(cudaSetDevice(ctx->device));
   if (direction == 1) return fft_c2c_impl<true>(ctx, static_cast<float2*>(d_x), length, batch);
@@ -1081,6 +1085,7 @@ extern "C" int srtb_b200_fft_c2c(srtb_b200_ctx* ctx, void* d_x, size_t length, s
 extern "C" int srtb_b200_watfft_c2c_backward(srtb_b200_ctx* ctx, void* d_x, size_t length, size_t batch) {
   API_LOCK(ctx);
   if (!ctx) return fail(nullptr, SRTB_B200_E_INVALID, "watfft: ctx is null");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "watfft: d_x is not 8-byte aligned");
   stage_scope stats_(ctx, SRTB_B200_STAGE_WATFFT, 16.0 * (double)length * (double)batch);
   return srtb_b200_fft_c2c(ctx, d_x, length, batch, -1);
 }
@@ -1091,6 +1096,7 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
 extern "C" int srtb_b200_fft_r2c_inplace(srtb_b200_ctx* ctx, float* d_inout, size_t n_real) {
   API_LOCK(ctx);
   if (!ctx || !d_inout) return fail(ctx, SRTB_B200_E_INVALID, "fft_r2c: null argument");
+  if (!aligned8(d_inout)) return fail(ctx, SRTB_B200_E_INVALID, "fft_r2c: d_inout is not 8-byte aligned");
   if (n_real < 2 || !is_pow2(n_real))
     return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(n_real));
   CK(cudaSetDevice(ctx->device));
@@ -1328,6 +1334,7 @@ extern "C" int srtb_b200_rfi_s1(srtb_b200_ctx* ctx, void* d_x, size_t count, flo
                                 float* d_mean_out) {
   API_LOCK(ctx);
   if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: d_x is not 8-byte aligned");
   if (count == 0) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: zero count");
   if (n_ranges && !h_bin_ranges) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s1: null ranges");
   const std::vector<size_t> bins(h_bin_ranges, h_bin_ranges + 2 * n_ranges);
@@ -1355,6 +1362,7 @@ extern "C" int srtb_b200_dedisperse(srtb_b200_ctx* ctx, void* d_x, size_t count,
                                     float df, float dm) {
   API_LOCK(ctx);
   if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "dedisperse: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "dedisperse: d_x is not 8-byte aligned");
   if (count == 0) return 0;
   CK(cudaSetDevice(ctx->device));
   stage_scope stats_(ctx, SRTB_B200_STAGE_DEDISPERSE, 16.0 * (double)count);
@@ -1414,6 +1422,7 @@ extern "C" int srtb_b200_rfi_s2_sk(srtb_b200_ctx* ctx, void* d_x, size_t time_co
                                    float sk_threshold, float* d_sk_out) {
   API_LOCK(ctx);
   if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s2: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s2: d_x is not 8-byte aligned");
   if (time_count == 0 || chan_count == 0) return fail(ctx, SRTB_B200_E_INVALID, "rfi_s2: zero size");
   CK(cudaSetDevice(ctx->device));
   stage_scope stats_(ctx, SRTB_B200_STAGE_RFI_S2, 8.0 * (double)time_count * (double)chan_count);
@@ -1519,7 +1528,9 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
   const float2* tw = nullptr;
   if constexpr (LOGL >= 10) {  // sixteen-point row kernel; L = 512 has the eight-point one only
     constexpr int T16 = row16_t<LOGL>::value, threads = ((1 << LOGL) / 16) * T16;
-    auto kern = chirp ? fft_row16_tma_kernel<LOGL, T16, false, true, true> : fft_row16_tma_kernel<LOGL, T16, false, true, false>;
+    // block buffers are 16-byte aligned, so rows of these lengths always take the chirp-on-load route
+    if (!chirp) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: the sixteen-point SK row kernel needs the fused chirp");
+    auto kern = fft_row16_tma_kernel<LOGL, T16, false, true, true>;
     constexpr size_t smem = row16_smem<LOGL, T16>::bytes;
     const size_t ntiles = (chan_count + T16 - 1) / T16;
     if (int rc = persistent_grid(ctx, kern, threads, smem, smem, ntiles, &grid)) return rc;
@@ -1672,35 +1683,6 @@ static int watfft_long_fused(srtb_b200_ctx* ctx, int slot, float2* x, const floa
   return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr, max_boxcar);
 }
 
-// s2 (spectral kurtosis) + the detector's first column-sum stage in one sweep; used by process_block
-// when a row fits the per-thread register tile (L = 512 .. 4096)
-static bool sk_detect_fusable(size_t time_count) {
-  return time_count == 512 || time_count == 1024 || time_count == 2048 || time_count == 4096;
-}
-// waterfall FFT + SK + column sums in one kernel (no chirp): the row kernels above plus the whole-row kernel
-static bool watfft_sk_fusable(size_t time_count) {
-  return sk_detect_fusable(time_count) || time_count == 8192 || time_count == 16384;
-}
-static int sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_t time_count, size_t chan_count,
-                           size_t time_reserved_count, float sk_threshold, float snr, float chan_thr,
-                           size_t max_boxcar) {
-  const size_t ts_count = (time_count <= time_reserved_count) ? time_count : time_count - time_reserved_count;
-  const size_t rows_per_chunk = std::max<size_t>(1, chan_count / ((size_t)ctx->sm_count * 4));
-  const size_t chunks = (chan_count + rows_per_chunk - 1) / rows_per_chunk;
-  if (int rc = detect_prepare(ctx, slot, time_count, chunks * ts_count)) return rc;
-  CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
-  const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
-  switch (time_count / 512) {
-    case 1: sk_colsum_kernel<1><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
-    case 2: sk_colsum_kernel<2><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
-    case 4: sk_colsum_kernel<4><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
-    default: sk_colsum_kernel<8><<<(unsigned)chunks, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, rows_per_chunk, lo_, hi_, ctx->lane.colsum_partial); break;
-  }
-  ctx->launches++;
-  CK(cudaGetLastError());
-  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, chunks, snr, chan_thr, max_boxcar);
-}
-
 static int detect_collect(srtb_b200_ctx* ctx, int slot, srtb_b200_detect_result* h_result, float* h_series,
                           int copy_all) {
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
@@ -1731,6 +1713,7 @@ extern "C" int srtb_b200_signal_detect(srtb_b200_ctx* ctx, const void* d_x, size
                                        srtb_b200_detect_result* h_result, float* h_series, int copy_all) {
   API_LOCK(ctx);
   if (!ctx || !d_x || !h_result) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect: d_x is not 8-byte aligned");
   if (time_count == 0 || chan_count == 0) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect: zero size");
   CK(cudaSetDevice(ctx->device));
   stage_scope stats_(ctx, SRTB_B200_STAGE_SIGNAL_DETECT, 8.0 * (double)time_count * (double)chan_count);
@@ -1762,6 +1745,7 @@ extern "C" int srtb_b200_rfi_sk_v1(srtb_b200_ctx* ctx, void* d_x, size_t fft_bin
                                    float sk_threshold, float* d_sk_out) {
   API_LOCK(ctx);
   if (!ctx || !d_x) return fail(ctx, SRTB_B200_E_INVALID, "rfi_sk_v1: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "rfi_sk_v1: d_x is not 8-byte aligned");
   if (fft_bins == 0 || time_counts == 0) return fail(ctx, SRTB_B200_E_INVALID, "rfi_sk_v1: zero size");
   CK(cudaSetDevice(ctx->device));
   return sk_v1_enqueue(ctx, static_cast<float2*>(d_x), fft_bins, time_counts, sk_threshold, d_sk_out);
@@ -1773,6 +1757,7 @@ extern "C" int srtb_b200_signal_detect_v1(srtb_b200_ctx* ctx, void* d_x, size_t 
                                           int copy_all) {
   API_LOCK(ctx);
   if (!ctx || !d_x || !h_result) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect_v1: null argument");
+  if (!aligned8(d_x)) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect_v1: d_x is not 8-byte aligned");
   if (count_per_batch == 0 || batch_size == 0) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect_v1: zero size");
   CK(cudaSetDevice(ctx->device));
   float2* x = static_cast<float2*>(d_x);
@@ -1998,24 +1983,20 @@ static int r2c_stream(srtb_b200_ctx* ctx, const block_params& p, block_input* in
   return fft_r2c_with_power_mean(ctx, buf, p.N);
 }
 
-static inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 // routes that apply s1 + the chirp as a waterfall kernel loads the spectrum: the caller zaps the manual ranges on the
 // spectrum beforehand (0 stays 0 through s1 and the chirp)
-static bool chirp_on_load(size_t L, const void* dst, const void* src) {
-  return aligned16(dst) && aligned16(src) && (chirp_fusable(L) || long_fusable(L));
-}
+static bool chirp_on_load(size_t L) { return chirp_fusable(L) || long_fusable(L); }
 
 // one stream's chain after its R2C, at one DM: s1 + chirp, waterfall FFT, SK and detector, result header in
 // d_res[slot]. src holds the spectrum, dst receives the dynamic spectrum: the same buffer on the block path, while the
 // DM sweep keeps src for the next trial. phase_table: the whole-row kernel may read a tabulated chirp (built for the
-// block's DM; the DM sweep changes DM every trial).
+// block's DM; the DM sweep changes DM every trial). Both buffers are 16-byte aligned: the ctx allocates them, or
+// submit_block_ex checked the caller's.
 static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, float2* dst, const float2* src, float dm,
                        bool phase_table) {
   const srtb_b200_block_config* cfg = p.cfg;
   const size_t reserved = p.reserved(dm);
-  const bool aligned = aligned16(dst) && aligned16(src);
-  if (aligned && chirp_fusable(p.L)) {
+  if (chirp_fusable(p.L)) {
     // ONE kernel: s1 + chirp on load, waterfall FFT, SK, partial column sums
     row_chirp_params cp = p.chirp(dm, ctx->lane.mean);
     if (phase_table)
@@ -2024,7 +2005,7 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
                                   cfg->signal_detect_max_boxcar_length, &cp, src);
   }
-  if (aligned && long_fusable(p.L)) {
+  if (long_fusable(p.L)) {
     // long rows: chirp-on-load column sweep, last sweep with SK statistics, decision, column sums (20 bytes per
     // sample). No phase table here: the long-row column sweep is DRAM-bound, and the 4 extra bytes per bin a table
     // costs outweigh the fp64 evaluation it would replace.
@@ -2037,17 +2018,14 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
   if (int rc = rfi_s1_dedisperse_fused(ctx, dst, src, p.Nc, cfg->mitigate_rfi_average_method_threshold, p.coef, p.bins,
                                        p.f_min, p.f_c, p.df, dm))
     return rc;
-  if (watfft_sk_fusable(p.L) && aligned16(dst)) {
-    // waterfall FFT + SK + partial column sums in one kernel, then the small detector tail
+  if (p.L == 512) {
+    // waterfall FFT + SK + partial column sums in one kernel (the eight-point row kernel has no chirp on load), then
+    // the small detector tail
     return watfft_sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
                                   cfg->signal_detect_max_boxcar_length);
   }
   if (int rc = srtb_b200_watfft_c2c_backward(ctx, dst, p.L, p.batch)) return rc;
-  if (sk_detect_fusable(p.L))
-    return sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
-                           cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                           cfg->signal_detect_max_boxcar_length);
   if (int rc = srtb_b200_rfi_s2_sk(ctx, dst, p.L, p.batch, cfg->mitigate_rfi_spectral_kurtosis_threshold, nullptr))
     return rc;
   return detect_enqueue(ctx, slot, dst, p.L, p.batch, reserved, cfg->signal_detect_signal_noise_threshold,
@@ -2098,7 +2076,7 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
                              4.0 * (double)p.N);
       if (int rc = r2c_stream(ctx, p, &in, s, /*fork=*/two_lanes)) return rc;
     }
-    if (chirp_on_load(p.L, buf, buf))
+    if (chirp_on_load(p.L))
       if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
     return stream_tail(ctx, p, s, buf, buf, p.cfg->dm, /*phase_table=*/true);
   };
@@ -2186,7 +2164,7 @@ extern "C" int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b
   for (int s = 0; s < p.streams; s++) {
     if (int rc = r2c_stream(ctx, p, &in, s, /*fork=*/false)) return rc;
     float2* buf = reinterpret_cast<float2*>(ctx->stream_buf[s]);
-    if (chirp_on_load(p.L, W, buf))  // the manual zap does not depend on the DM: once, on the kept spectrum
+    if (chirp_on_load(p.L))  // the manual zap does not depend on the DM: once, on the kept spectrum
       if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
     for (size_t j = 0; j < n_dm; j++) {
       if (int rc = stream_tail(ctx, p, 0, W, buf, h_dms[j], /*phase_table=*/false)) return rc;
@@ -2235,6 +2213,8 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
   if (user_spec) {
     for (int s = 0; s < p.streams; s++) {
       if (!outputs->d_spectrum[s]) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: d_spectrum given for some streams only");
+      if (!aligned16(outputs->d_spectrum[s]))
+        return fail(ctx, SRTB_B200_E_INVALID, "submit_block: d_spectrum[" + std::to_string(s) + "] is not 16-byte aligned");
       bufs[s] = outputs->d_spectrum[s];
     }
   } else {
