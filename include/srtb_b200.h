@@ -280,6 +280,22 @@ int srtb_b200_simplify_spectrum(srtb_b200_ctx* ctx, const void* d_spectrum, size
                                 size_t out_width, size_t out_height, uint32_t argb_0, uint32_t argb_1,
                                 uint32_t argb_overflow, float* d_intensity, uint32_t* d_pixmap, float* d_average);
 
+/* ---- the baseband correlator (the reference's userspace/src/correlator.cpp:53-149) ----------------------------------
+ * cross spectrum, its step (1): d_out[i] = (norm * d_a[i]) * conj(d_b[i]) for i < count, complex64, in SyclCPLX's float
+ * arithmetic without contraction. d_out may be d_a or d_b (in place); any other overlap with them, a null pointer, a
+ * zero count or a pointer that is not 8-byte aligned returns SRTB_B200_E_INVALID before any launch. */
+int srtb_b200_cross_spectrum(srtb_b200_ctx* ctx, const void* d_a, const void* d_b, size_t count, float norm,
+                             void* d_out);
+/* the whole program on device bytes: d_in_1 and d_in_2 hold input_size unsigned 8-bit samples each (the smaller of the
+ * two file sizes), of which real_count = 2 (input_size / 2) are read. Each is unpacked and R2C-transformed (the unpack
+ * fused into the first sweep where the block path would fuse it), the cross spectrum of the first M = real_count / 2
+ * bins is scaled by norm = float(pow(double(input_size), -1.5)), transformed by an unnormalised backward C2C of M
+ * points, and d_out (4-byte aligned) receives its M magnitudes |y[i]| as floats.
+ * Before any launch: input_size < 2, a null pointer or a misaligned d_out returns SRTB_B200_E_INVALID; real_count not
+ * a power of two ("[fft] n must be a power of 2", fft/naive_fft_wrapper.hpp:52-56) or above 2^31 returns
+ * SRTB_B200_E_SIZE. Working buffers (2 x (real_count + 2) floats) live in the ctx and grow on demand. Stream-ordered. */
+int srtb_b200_correlate(srtb_b200_ctx* ctx, const void* d_in_1, const void* d_in_2, size_t input_size, float* d_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,6 +22,7 @@
 #include "fft_bigrow.cuh"
 #include "ops_kernels.cuh"
 #include "thumbnail.cuh"
+#include "correlator.cuh"
 
 using namespace srtb_b200;
 
@@ -124,6 +125,9 @@ struct srtb_b200_ctx {
   size_t thumb_rows_bytes = 0;
   float* thumb_partial = nullptr;
   size_t thumb_partial_bytes = 0;
+  // correlate: the two inputs' in-place R2C buffers of real_count + 2 floats (entries 2 and 3 stay null)
+  float* corr_buf[4] = {};
+  size_t corr_buf_elems = 0;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -301,6 +305,7 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   cudaFree(ctx->chirp_tab);
   cudaFree(ctx->thumb_rows);
   cudaFree(ctx->thumb_partial);
+  for (auto& p : ctx->corr_buf) cudaFree(p);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
     cudaFree(ctx->slot_baseband[i]);
     for (auto& p : ctx->slot_stream_buf[i]) cudaFree(p);
@@ -2364,6 +2369,91 @@ extern "C" int srtb_b200_simplify_spectrum(srtb_b200_ctx* ctx, const void* d_spe
   CK(cudaGetLastError());
   thumb_norm_kernel<<<grid_for(ctx, n, THUMB_THREADS, 4), THUMB_THREADS, 0, ctx->lane.stream>>>(
       d_intensity, n, ctx->thumb_partial, (int)col_grid, argb_0, argb_1, argb_overflow, d_pixmap, d_average);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------
+// baseband correlator (the reference's correlator.cpp): see correlator.cuh
+// ------------------------------------------------------------------------------------
+static int launch_cross_spectrum(srtb_b200_ctx* ctx, const float2* a, const float2* b, size_t M, float norm,
+                                 float2* out) {
+  const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) |
+                     reinterpret_cast<uintptr_t>(out)) & 15u) == 0;
+  if (vec)
+    cross_spectrum_kernel<true><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(a, b, M, norm, out);
+  else
+    cross_spectrum_kernel<false><<<grid_for(ctx, M, 256), 256, 0, ctx->lane.stream>>>(a, b, M, norm, out);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
+}
+
+static bool byte_ranges_overlap(const void* p, const void* q, size_t bytes) {
+  const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
+  return a < b + bytes && b < a + bytes;
+}
+
+extern "C" int srtb_b200_cross_spectrum(srtb_b200_ctx* ctx, const void* d_a, const void* d_b, size_t count, float norm,
+                                        void* d_out) {
+  API_LOCK(ctx);
+  if (!ctx || !d_a || !d_b || !d_out) return fail(ctx, SRTB_B200_E_INVALID, "cross_spectrum: null argument");
+  if (count == 0) return fail(ctx, SRTB_B200_E_INVALID, "cross_spectrum: zero count");
+  if (!aligned8(d_a) || !aligned8(d_b) || !aligned8(d_out))
+    return fail(ctx, SRTB_B200_E_INVALID, "cross_spectrum: a pointer is not 8-byte aligned");
+  if (count > (SIZE_MAX >> 4)) return fail(ctx, SRTB_B200_E_INVALID, "cross_spectrum: count too large");
+  const size_t bytes = count * sizeof(float2);
+  if ((d_out != d_a && byte_ranges_overlap(d_out, d_a, bytes)) || (d_out != d_b && byte_ranges_overlap(d_out, d_b, bytes)))
+    return fail(ctx, SRTB_B200_E_INVALID, "cross_spectrum: d_out overlaps an input without being it");
+  CK(cudaSetDevice(ctx->device));
+  return launch_cross_spectrum(ctx, static_cast<const float2*>(d_a), static_cast<const float2*>(d_b), count, norm,
+                               static_cast<float2*>(d_out));
+}
+
+extern "C" int srtb_b200_correlate(srtb_b200_ctx* ctx, const void* d_in_1, const void* d_in_2, size_t input_size,
+                                   float* d_out) {
+  API_LOCK(ctx);
+  if (!ctx || !d_in_1 || !d_in_2 || !d_out) return fail(ctx, SRTB_B200_E_INVALID, "correlate: null argument");
+  if (reinterpret_cast<uintptr_t>(d_out) & 3u)
+    return fail(ctx, SRTB_B200_E_INVALID, "correlate: d_out is not 4-byte aligned");
+  if (input_size < 2)
+    return fail(ctx, SRTB_B200_E_INVALID, "correlate: input_size must be at least 2 bytes, got " +
+                                              std::to_string(input_size));
+  const size_t M = input_size / 2, N = 2 * M;  // complex_count, real_count (correlator.cpp:56-57)
+  if (!is_pow2(N)) return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(N));
+  if (N > ((size_t)1 << 31))
+    return fail(ctx, SRTB_B200_E_SIZE, "correlate: real_count " + std::to_string(N) + " above 2^31 samples not supported");
+  CK(cudaSetDevice(ctx->device));
+  if (int rc = ensure_stream_bufs(ctx, ctx->corr_buf, &ctx->corr_buf_elems, N, 2)) return rc;
+  // std::pow(input_size, -1.5) in double, stored as float (correlator.cpp:59): an odd input_size counts (q13)
+  const float norm = static_cast<float>(std::pow(static_cast<double>(input_size), -1.5));
+  // each input is one SIMPLE stream of unsigned 8-bit samples without a window: the block path's R2C, with the unpack
+  // fused into the first sweep where raw_sources_for allows it
+  srtb_b200_block_config cfg{};
+  cfg.baseband_input_count = N;
+  cfg.baseband_input_bits = 8;
+  cfg.baseband_format = SRTB_B200_FORMAT_SIMPLE;
+  cfg.window = SRTB_B200_WINDOW_RECTANGLE;
+  block_params p;
+  p.cfg = &cfg;
+  p.streams = 1;
+  p.N = N;
+  const void* inputs[2] = {d_in_1, d_in_2};
+  for (int s = 0; s < 2; s++) {
+    float* const bufs[4] = {ctx->corr_buf[s], nullptr, nullptr, nullptr};
+    block_input in{inputs[s], N, bufs};
+    if (int rc = block_input_init(ctx, p, &in)) return rc;
+    if (int rc = r2c_stream(ctx, p, &in, 0, /*fork=*/false)) return rc;
+  }
+  // (1) cross spectrum over X1 (the Nyquist bin is dropped), (2) unnormalised backward C2C of M points, (3) |y|
+  float2* x1 = reinterpret_cast<float2*>(ctx->corr_buf[0]);
+  if (int rc = launch_cross_spectrum(ctx, x1, reinterpret_cast<const float2*>(ctx->corr_buf[1]), M, norm, x1)) return rc;
+  if (int rc = fft_c2c_impl<false>(ctx, x1, M, 1)) return rc;
+  if ((reinterpret_cast<uintptr_t>(d_out) & 7u) == 0)
+    magnitude_kernel<true><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(x1, M, d_out);
+  else
+    magnitude_kernel<false><<<grid_for(ctx, M, 256), 256, 0, ctx->lane.stream>>>(x1, M, d_out);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;

@@ -123,6 +123,8 @@ SYMBOLS = {
     "srtb_b200_block_spectrum": (_P, [_P, _I]),
     "srtb_b200_sweep_spectrum": (_P, [_P]),
     "srtb_b200_simplify_spectrum": (_I, [_P, _P, _SZ, _SZ, _SZ, _SZ, C.c_uint32, C.c_uint32, C.c_uint32, _P, _P, _P]),
+    "srtb_b200_cross_spectrum": (_I, [_P, _P, _P, _SZ, _F, _P]),
+    "srtb_b200_correlate": (_I, [_P, _P, _P, _SZ, _P]),
 }
 
 _lib = None
@@ -323,6 +325,15 @@ class Context:
         self._ck(self.lib.srtb_b200_simplify_spectrum(self.h, _ptr(d_spectrum), in_width, in_height, out_width,
                                                       out_height, argb_0, argb_1, argb_overflow, _ptr(d_intensity),
                                                       _ptr(d_pixmap), _ptr(d_average)))
+
+    def cross_spectrum(self, d_a, d_b, count: int, norm: float, d_out):
+        """the correlator's cross spectrum: d_out[i] = (norm d_a[i]) conj(d_b[i]), complex64; d_out may be d_a or d_b"""
+        self._ck(self.lib.srtb_b200_cross_spectrum(self.h, _ptr(d_a), _ptr(d_b), count, norm, _ptr(d_out)))
+
+    def correlate(self, d_in_1, d_in_2, input_size: int, d_out):
+        """the reference's baseband correlator on device bytes: d_out receives input_size // 2 floats, the magnitude of
+        the cross-correlation of the two unsigned 8-bit inputs"""
+        self._ck(self.lib.srtb_b200_correlate(self.h, _ptr(d_in_1), _ptr(d_in_2), input_size, _ptr(d_out)))
 
 
 # host helpers (pure host arithmetic of the reference's pipes)
