@@ -296,6 +296,32 @@ int srtb_b200_cross_spectrum(srtb_b200_ctx* ctx, const void* d_a, const void* d_
  * SRTB_B200_E_SIZE. Working buffers (2 x (real_count + 2) floats) live in the ctx and grow on demand. Stream-ordered. */
 int srtb_b200_correlate(srtb_b200_ctx* ctx, const void* d_in_1, const void* d_in_2, size_t input_size, float* d_out);
 
+/* ---- the integrating, segment-averaged correlator (an FX correlator: the noise falls as 1/sqrt(K)) -----------------
+ * Inputs: samples of width bits = 1, 2, 4, 8 (unsigned) or -8 (int8), in srtb_b200_unpack's SIMPLE order (sub-byte
+ * samples MSB first within a byte). Segment size Ls: a power of two from 16 to 2^30 real samples; Ms = Ls / 2.
+ * Segment s of each input is its samples [s Ls, (s + 1) Ls), with no overlap and no window; A_s and B_s are the first Ms
+ * bins of each segment's real FFT (the Nyquist bin is dropped). Over K segments in all,
+ *   out[j] = | sum_k ((norm / K) sum_s A_s[k] conj(B_s[k])) e^{+2 pi i j k / Ms} |, j < Ms, float32,
+ *   norm = float(pow(double(Ls), -1.5)).
+ * With K = 1 and Ls = input_size this is what srtb_b200_correlate computes. Lags: if input 2 is input 1 delayed by d
+ * samples (|d| << Ls), the peak is at (-d / 2) mod Ms.
+ *
+ * accumulate: reads n_segments Ls |bits| / 8 bytes of each input (any byte address) and adds sum_s A_s conj(B_s) into
+ * d_acc, Ms complex float64 values (16-byte aligned, owned by the caller); reset != 0 overwrites d_acc instead. The sum
+ * within a call has a fixed grouping, so the result is deterministic. Kernels: a pack of two segments of one input per
+ * complex row, one batched forward C2C of Ls points over the rows of both inputs, a split / cross-multiply /
+ * accumulate; their number does not depend on n_segments. Working buffers (2 ceil(n_segments / 2) Ls complex64, plus
+ * the C2C's scratch above 2^14 points) live in the ctx and grow on demand.
+ * finish: scales d_acc by norm / total_segments, rounds it to complex64, runs an unnormalised backward C2C of Ms points
+ * on a ctx buffer and writes the Ms magnitudes (hypotf) into d_out (4-byte aligned).
+ * Both are stream-ordered and do not synchronise. Before any launch they return SRTB_B200_E_INVALID for a null
+ * pointer, n_segments == 0, total_segments == 0, a d_acc not 16-byte aligned, a d_out not 4-byte aligned or bits
+ * outside the set, and SRTB_B200_E_SIZE for an Ls that is not a power of two in [16, 2^30] or n_segments Ls > 2^34. */
+int srtb_b200_correlate_accumulate(srtb_b200_ctx* ctx, const void* d_in_1, const void* d_in_2, int bits,
+                                   size_t segment_size, size_t n_segments, void* d_acc, int reset);
+int srtb_b200_correlate_finish(srtb_b200_ctx* ctx, const void* d_acc, size_t segment_size, uint64_t total_segments,
+                               float* d_out);
+
 #ifdef __cplusplus
 }
 #endif

@@ -128,6 +128,13 @@ struct srtb_b200_ctx {
   // correlate: the two inputs' in-place R2C buffers of real_count + 2 floats (entries 2 and 3 stay null)
   float* corr_buf[4] = {};
   size_t corr_buf_elems = 0;
+  // correlate_accumulate / _finish: the packed segment rows of both inputs (also finish's Ms-point C2C buffer), the
+  // split's per-row-group partial sums and its per-bin-tile tickets (sm_count * 8, zero between launches)
+  void* corr_rows = nullptr;
+  size_t corr_rows_bytes = 0;
+  void* corr_partial = nullptr;
+  size_t corr_partial_bytes = 0;
+  unsigned* corr_tickets = nullptr;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -306,6 +313,9 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   cudaFree(ctx->thumb_rows);
   cudaFree(ctx->thumb_partial);
   for (auto& p : ctx->corr_buf) cudaFree(p);
+  cudaFree(ctx->corr_rows);
+  cudaFree(ctx->corr_partial);
+  cudaFree(ctx->corr_tickets);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
     cudaFree(ctx->slot_baseband[i]);
     for (auto& p : ctx->slot_stream_buf[i]) cudaFree(p);
@@ -2390,6 +2400,17 @@ static int launch_cross_spectrum(srtb_b200_ctx* ctx, const float2* a, const floa
   return 0;
 }
 
+// out[i] = |y[i]| for i < M; two bins per access when out is 8-byte aligned (y is a ctx buffer, 16-byte aligned)
+static int launch_magnitude(srtb_b200_ctx* ctx, const float2* y, size_t M, float* out) {
+  if ((reinterpret_cast<uintptr_t>(out) & 7u) == 0)
+    magnitude_kernel<true><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(y, M, out);
+  else
+    magnitude_kernel<false><<<grid_for(ctx, M, 256), 256, 0, ctx->lane.stream>>>(y, M, out);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
+}
+
 static bool byte_ranges_overlap(const void* p, const void* q, size_t bytes) {
   const uintptr_t a = reinterpret_cast<uintptr_t>(p), b = reinterpret_cast<uintptr_t>(q);
   return a < b + bytes && b < a + bytes;
@@ -2450,11 +2471,110 @@ extern "C" int srtb_b200_correlate(srtb_b200_ctx* ctx, const void* d_in_1, const
   float2* x1 = reinterpret_cast<float2*>(ctx->corr_buf[0]);
   if (int rc = launch_cross_spectrum(ctx, x1, reinterpret_cast<const float2*>(ctx->corr_buf[1]), M, norm, x1)) return rc;
   if (int rc = fft_c2c_impl<false>(ctx, x1, M, 1)) return rc;
-  if ((reinterpret_cast<uintptr_t>(d_out) & 7u) == 0)
-    magnitude_kernel<true><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(x1, M, d_out);
+  return launch_magnitude(ctx, x1, M, d_out);
+}
+
+// ---- the integrating, segment-averaged correlator (see include/srtb_b200.h and correlator.cuh)
+
+static int check_segment_size(srtb_b200_ctx* ctx, const char* who, size_t Ls) {
+  if (!is_pow2(Ls) || Ls < 16 || Ls > ((size_t)1 << 30))
+    return fail(ctx, SRTB_B200_E_SIZE, std::string(who) + ": segment_size must be a power of two from 16 to 2^30, got " +
+                                           std::to_string(Ls));
+  return 0;
+}
+
+template <int BITS>
+static int launch_corr_pack(srtb_b200_ctx* ctx, const void* in_1, const void* in_2, int log_ls, size_t n_segments,
+                            size_t rows, float2* out) {
+  const uintptr_t group = BITS < 0 ? -BITS : BITS;  // bytes of 8 samples: unpack_src<BITS>'s load width
+  const bool vec = reinterpret_cast<uintptr_t>(in_1) % group == 0 && reinterpret_cast<uintptr_t>(in_2) % group == 0;
+  const size_t pairs = (2 * rows) << log_ls;
+  if (vec)
+    corr_pack_kernel<BITS, true><<<grid_for(ctx, pairs / 8, 256), 256, 0, ctx->lane.stream>>>(in_1, in_2, log_ls,
+                                                                                               n_segments, rows, out);
   else
-    magnitude_kernel<false><<<grid_for(ctx, M, 256), 256, 0, ctx->lane.stream>>>(x1, M, d_out);
+    corr_pack_kernel<BITS, false><<<grid_for(ctx, pairs, 256), 256, 0, ctx->lane.stream>>>(in_1, in_2, log_ls,
+                                                                                           n_segments, rows, out);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
+}
+
+extern "C" int srtb_b200_correlate_accumulate(srtb_b200_ctx* ctx, const void* d_in_1, const void* d_in_2, int bits,
+                                              size_t segment_size, size_t n_segments, void* d_acc, int reset) {
+  API_LOCK(ctx);
+  if (!ctx || !d_in_1 || !d_in_2 || !d_acc) return fail(ctx, SRTB_B200_E_INVALID, "correlate_accumulate: null argument");
+  if (bits != 1 && bits != 2 && bits != 4 && bits != 8 && bits != -8)
+    return fail(ctx, SRTB_B200_E_INVALID, "correlate_accumulate: bits must be 1, 2, 4, 8 or -8, got " +
+                                              std::to_string(bits));
+  if (n_segments == 0) return fail(ctx, SRTB_B200_E_INVALID, "correlate_accumulate: n_segments is zero");
+  if (reinterpret_cast<uintptr_t>(d_acc) & 15u)
+    return fail(ctx, SRTB_B200_E_INVALID, "correlate_accumulate: d_acc is not 16-byte aligned");
+  if (int rc = check_segment_size(ctx, "correlate_accumulate", segment_size)) return rc;
+  if (n_segments > ((size_t)1 << 34) / segment_size)
+    return fail(ctx, SRTB_B200_E_SIZE, "correlate_accumulate: n_segments * segment_size above 2^34");
+  CK(cudaSetDevice(ctx->device));
+  const size_t Ls = segment_size, Ms = Ls / 2, rows = (n_segments + 1) / 2;  // rows per input
+  const int log_ls = ilog2(Ls);
+  if (int rc = ensure(ctx, &ctx->corr_rows, &ctx->corr_rows_bytes, 2 * rows * Ls * sizeof(float2))) return rc;
+  const unsigned target = (unsigned)ctx->sm_count * 8;  // resident 256-thread CTAs of the whole GPU
+  if (!ctx->corr_tickets) {
+    CK(cudaMalloc(&ctx->corr_tickets, target * sizeof(unsigned)));
+    CK(cudaMemsetAsync(ctx->corr_tickets, 0, target * sizeof(unsigned), ctx->lane.stream));
+  }
+  float2* z = static_cast<float2*>(ctx->corr_rows);
+  int rc = 0;
+  switch (bits) {
+    case 1: rc = launch_corr_pack<1>(ctx, d_in_1, d_in_2, log_ls, n_segments, rows, z); break;
+    case 2: rc = launch_corr_pack<2>(ctx, d_in_1, d_in_2, log_ls, n_segments, rows, z); break;
+    case 4: rc = launch_corr_pack<4>(ctx, d_in_1, d_in_2, log_ls, n_segments, rows, z); break;
+    case 8: rc = launch_corr_pack<8>(ctx, d_in_1, d_in_2, log_ls, n_segments, rows, z); break;
+    default: rc = launch_corr_pack<-8>(ctx, d_in_1, d_in_2, log_ls, n_segments, rows, z); break;
+  }
+  if (rc) return rc;
+  if (int rc2 = fft_c2c_impl<true>(ctx, z, Ls, 2 * rows)) return rc2;
+  // split grid: bin tiles of BT bins x row groups. More than one group only when the tiles alone cannot fill the GPU;
+  // then tiles < target, so the target tickets suffice.
+  const int log_bt = std::min(log_ls - 1, 8);
+  const size_t BT = (size_t)1 << log_bt, tiles = Ms / BT, lanes = 256 / BT;
+  size_t groups = 1;
+  if (tiles < target) groups = std::min((target + tiles - 1) / tiles, (rows + lanes - 1) / lanes);
+  const size_t rows_per_group = (rows + groups - 1) / groups;
+  groups = (rows + rows_per_group - 1) / rows_per_group;
+  double2* partial = nullptr;
+  if (groups > 1) {
+    if (int rc2 = ensure(ctx, &ctx->corr_partial, &ctx->corr_partial_bytes, groups * Ms * sizeof(double2))) return rc2;
+    partial = static_cast<double2*>(ctx->corr_partial);
+  }
+  corr_split_accumulate_kernel<<<dim3((unsigned)tiles, (unsigned)groups), 256, 0, ctx->lane.stream>>>(
+      z, log_ls, log_bt, rows, n_segments, rows_per_group, partial, ctx->corr_tickets, static_cast<double2*>(d_acc),
+      reset);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int srtb_b200_correlate_finish(srtb_b200_ctx* ctx, const void* d_acc, size_t segment_size,
+                                          uint64_t total_segments, float* d_out) {
+  API_LOCK(ctx);
+  if (!ctx || !d_acc || !d_out) return fail(ctx, SRTB_B200_E_INVALID, "correlate_finish: null argument");
+  if (total_segments == 0) return fail(ctx, SRTB_B200_E_INVALID, "correlate_finish: total_segments is zero");
+  if (reinterpret_cast<uintptr_t>(d_acc) & 15u)
+    return fail(ctx, SRTB_B200_E_INVALID, "correlate_finish: d_acc is not 16-byte aligned");
+  if (reinterpret_cast<uintptr_t>(d_out) & 3u)
+    return fail(ctx, SRTB_B200_E_INVALID, "correlate_finish: d_out is not 4-byte aligned");
+  if (int rc = check_segment_size(ctx, "correlate_finish", segment_size)) return rc;
+  CK(cudaSetDevice(ctx->device));
+  const size_t Ms = segment_size / 2;
+  if (int rc = ensure(ctx, &ctx->corr_rows, &ctx->corr_rows_bytes, Ms * sizeof(float2))) return rc;
+  // the reference's norm with Ls in place of input_size, rounded to float, then over the segment count in float64
+  const float norm = static_cast<float>(std::pow(static_cast<double>(segment_size), -1.5));
+  const double scale = static_cast<double>(norm) / static_cast<double>(total_segments);
+  float2* y = static_cast<float2*>(ctx->corr_rows);
+  corr_scale_kernel<<<grid_for(ctx, Ms, 256), 256, 0, ctx->lane.stream>>>(static_cast<const double2*>(d_acc), Ms,
+                                                                           scale, y);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  if (int rc = fft_c2c_impl<false>(ctx, y, Ms, 1)) return rc;
+  return launch_magnitude(ctx, y, Ms, d_out);
 }

@@ -125,6 +125,8 @@ SYMBOLS = {
     "srtb_b200_simplify_spectrum": (_I, [_P, _P, _SZ, _SZ, _SZ, _SZ, C.c_uint32, C.c_uint32, C.c_uint32, _P, _P, _P]),
     "srtb_b200_cross_spectrum": (_I, [_P, _P, _P, _SZ, _F, _P]),
     "srtb_b200_correlate": (_I, [_P, _P, _P, _SZ, _P]),
+    "srtb_b200_correlate_accumulate": (_I, [_P, _P, _P, _I, _SZ, _SZ, _P, _I]),
+    "srtb_b200_correlate_finish": (_I, [_P, _P, _SZ, C.c_uint64, _P]),
 }
 
 _lib = None
@@ -334,6 +336,19 @@ class Context:
         """the reference's baseband correlator on device bytes: d_out receives input_size // 2 floats, the magnitude of
         the cross-correlation of the two unsigned 8-bit inputs"""
         self._ck(self.lib.srtb_b200_correlate(self.h, _ptr(d_in_1), _ptr(d_in_2), input_size, _ptr(d_out)))
+
+    def correlate_accumulate(self, d_in_1, d_in_2, bits: int, segment_size: int, n_segments: int, d_acc,
+                             reset: bool = False):
+        """the integrating correlator's accumulation: adds sum_s A_s conj(B_s) over n_segments segments of
+        segment_size samples of width bits (1, 2, 4, 8 or -8) of each input into d_acc, segment_size // 2 complex128
+        values (16-byte aligned); reset overwrites d_acc instead"""
+        self._ck(self.lib.srtb_b200_correlate_accumulate(self.h, _ptr(d_in_1), _ptr(d_in_2), bits, segment_size,
+                                                         n_segments, _ptr(d_acc), int(bool(reset))))
+
+    def correlate_finish(self, d_acc, segment_size: int, total_segments: int, d_out):
+        """the integrating correlator's result: d_out receives segment_size // 2 floats, the magnitude of the backward
+        transform of d_acc scaled by norm / total_segments"""
+        self._ck(self.lib.srtb_b200_correlate_finish(self.h, _ptr(d_acc), segment_size, total_segments, _ptr(d_out)))
 
 
 # host helpers (pure host arithmetic of the reference's pipes)
