@@ -68,6 +68,37 @@ __device__ __forceinline__ void st_l2_keep(float* a, float v, uint64_t pol) {
   asm volatile("st.global.L2::cache_hint.f32 [%0], %1, %2;" ::"l"(a), "f"(v), "l"(pol) : "memory");
 }
 
+// ---- distributed shared memory of a two-CTA cluster (the R2C row sweep reads its partner row's spectrum)
+__device__ __forceinline__ void cluster_sync_all() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+__device__ __forceinline__ uint32_t dsmem_addr(const void* p, unsigned rank) {
+  uint32_t a;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(a) : "r"(smem_u32(p)), "r"(rank));
+  return a;
+}
+__device__ __forceinline__ float4 ld_dsmem_f4(uint32_t a) {
+  float4 v;
+  asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
+  return v;
+}
+
+// R2C split of bin k = k1 + P k2 from Z[k] and Z[M - k] (w = e^{-i pi k / M}):
+//   X[k] = (Z[k] + conj Z[M-k]) / 2 - i w (Z[k] - conj Z[M-k]) / 2, the expression of fft_trans_r2c16_tma_kernel
+__device__ __forceinline__ float2 r2c_split_point(float2 hk, float2 hm, float2 w) {
+  const float2 F = make_float2(0.5f * (hk.x + hm.x), 0.5f * (hk.y - hm.y));
+  const float2 G = make_float2(0.5f * (hk.y + hm.y), -0.5f * (hk.x - hm.x));
+  const float2 gw = make_float2(G.x * w.x - G.y * w.y, G.x * w.y + G.y * w.x);
+  return make_float2(F.x + gw.x, F.y + gw.y);
+}
+
+// the R2C row sweep (SRC = 2): rows of the [P][L] scratch, Σ|X|^2 partials per CTA, mean over M = P L bins
+struct r2c_rows_params {
+  double* partial;
+  unsigned* ticket;
+  float* mean;
+};
+
 // a[i] *= w^i, i = 1..15 (powers at most four multiplications deep)
 __device__ __forceinline__ void bigrow_twiddle_powers(float2 (&a)[16], const float2 w1) {
   const float2 w2 = c_sqr(w1), w3 = c_mul(w2, w1), w4 = c_sqr(w2);
@@ -114,10 +145,25 @@ __device__ __forceinline__ void bigrow_stage_table(float2* __restrict__ p, const
 // CHIRP: 0 = plain transform; otherwise s1 + chirp on load, 1/f of successive bins by Newton steps from the neighbour:
 //   1 = one step along a butterfly's inputs (B1 bins apart) and one to the adjacent bin, 3 = two and one,
 //   4 = two and two, 2 = a correctly rounded reciprocal for every bin (widely spaced bins of short test blocks)
-template <int LOGL, bool FWD, bool SK, int CHIRP>
-__global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
-    fft_bigrow_kernel(const float2* __restrict__ in, float2* __restrict__ out, unsigned nrows,
-                      const float2* __restrict__ tabs, row_sk_params skp, row_chirp_params cp) {
+// SRC: where the rows come from and what is stored.
+//   0 = rows of `in` (natural order), natural-order rows to `out`;
+//   1 = channel `row` of a spectrum left in sweep order by SRC = 2 (bin k = k1 + P k2 at k1 L + k2, P = L / 8): the
+//       box of all P rows k1 by the 8 columns k2 = 8 row .. 8 row + 7, fetched through `tmap` as 8 boxes of 256 rows x
+//       8 elements (dense 64-byte rows, one mbarrier each). Chunk d0 of the channel is column d0 >> 1, rows from
+//       (P / 2) (d0 & 1): buffer A holds rows k1 < P / 2, buffer B the rest, and stage 0 gathers butterfly j from rows
+//       j and j + P / 2 before it stores the standard layout (tools/proto_r2c_sweep_order.py);
+//   2 = the R2C row sweep, run as clusters of two CTAs: nrows = P rows of the in-place scratch, the cluster's CTAs
+//       take rows i and P - i (cluster 0: rows 0 and P / 2, each its own mirror), transform them forward and store
+//       the split spectrum X[k1 + P k2] in place, reading the mirror row's Z through distributed shared memory.
+// The body is shared by three entry points: fft_bigrow_kernel (SRC = 0) and the two kernels of the sweep-order R2C
+// route below it.
+template <int LOGL, bool FWD, bool SK, int CHIRP, int SRC>
+__device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float2* __restrict__ out, unsigned nrows,
+                                            const float2* __restrict__ tabs, const row_sk_params& skp,
+                                            const row_chirp_params& cp, const tensor_map_blob* tmap,
+                                            const r2c_rows_params& rr) {
+  static_assert(SRC == 0 || (LOGL == 14 && ((SRC == 1 && !FWD && SK && CHIRP == 5) || (SRC == 2 && FWD && !SK && CHIRP == 0))),
+                "sweep-order routes: rows of 2^14");
   using C = bigrow<LOGL>;
   constexpr int L = C::L, R3 = C::R3, B1 = C::B1, B2 = C::B2, S1 = C::S1, S2 = C::S2, NT = C::NT, NW = C::NW;
   constexpr int HALF = C::HALF;
@@ -147,7 +193,13 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
   // chunk, each signalled on its own mbarrier
   auto issue_half = [&](unsigned row, int which, int hb) {
     fence_proxy_async();
-    if (lane < 8) {
+    if constexpr (SRC == 1) {
+      if (lane < 4) {  // rows (P / 2) which + 256 lane .. + 255, columns 8 row .. 8 row + 7
+        mbar_expect_tx(&mbar[hb * 8 + lane], (uint32_t)(256 * 8 * sizeof(float2)));
+        tma_load_2d(hbuf + hb * HALF + lane * 2048, tmap, (int)(8 * row), which * (L / 16) + 256 * lane,
+                    &mbar[hb * 8 + lane]);
+      }
+    } else if (lane < 8) {
       mbar_expect_tx(&mbar[hb * 8 + lane], (uint32_t)(B1 * sizeof(float2)));
       bulk_g2s(hbuf + hb * HALF + lane * S1, in + (size_t)row * L + (size_t)(which * 8 + lane) * B1,
                (uint32_t)(B1 * sizeof(float2)), &mbar[hb * 8 + lane]);
@@ -159,7 +211,21 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
     if constexpr (CHIRP == 5)
       asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const char*>(cp.phase + (size_t)r * L) + (size_t)tid * 128));
   };
-  if (blockIdx.x < nrows) prefetch_phase(blockIdx.x);  // the table is a constant of the run: no dependency to wait for
+  // the row of iteration it: SRC = 2 walks pairs (i, P - i) cluster by cluster, the others rows blockIdx.x + it gridDim.x
+  const unsigned crank = blockIdx.x & 1;
+  auto row_of = [&](unsigned it) -> unsigned {
+    if constexpr (SRC == 2) {
+      const unsigned i = (blockIdx.x >> 1) + it * (gridDim.x >> 1);
+      return i == 0 ? crank * (nrows / 2) : (crank ? nrows - i : i);
+    } else {
+      return blockIdx.x + it * gridDim.x;
+    }
+  };
+  auto live = [&](unsigned it) -> bool {
+    if constexpr (SRC == 2) return (blockIdx.x >> 1) + it * (gridDim.x >> 1) < nrows / 2;
+    else return row_of(it) < nrows;
+  };
+  if (live(0)) prefetch_phase(row_of(0));  // the table is a constant of the run: no dependency to wait for
   pdl_launch_dependents();
   pdl_wait();  // tables and barriers were set up while the preceding kernel drained
   if constexpr (SK) {
@@ -173,15 +239,25 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
   // Rotation of the three half buffers: row `it` of this CTA has chunks 0..7 in A = (2 it) % 3 and chunks 8..15 in
   // B = (2 it + 1) % 3; the third buffer receives chunks 0..7 of the next row meanwhile. Buffer A has been filled
   // floor(2 it / 3) times before, B floor((2 it + 1) / 3) times: the mbarrier phase parities.
-  unsigned row = blockIdx.x;
-  if (wid == 0) {
-    if (row < nrows) {
-      issue_half(row, 0, 0);
-      issue_half(row, 1, 1);
+  if constexpr (SRC == 2) {
+    // e^{-i pi i2 / 64}, i2 = 0..15: the split twiddle's factor along the output digit d2 (k2 = .. + 256 d2)
+    if (tid < 16) {
+      float sn, cs;
+      sincospif(-(float)tid / 64.f, &sn, &cs);
+      reinterpret_cast<float2*>(red)[tid] = make_float2(cs, sn);
     }
-    if (row + gridDim.x < nrows) issue_half(row + gridDim.x, 0, 2);
+    __syncthreads();
   }
-  for (unsigned it = 0; row < nrows; row += gridDim.x, it++) {
+  double psum = 0.0;  // SRC = 2: this thread's Σ|X|^2
+  if (wid == 0) {
+    if (live(0)) {
+      issue_half(row_of(0), 0, 0);
+      issue_half(row_of(0), 1, 1);
+    }
+    if (live(1)) issue_half(row_of(1), 0, 2);
+  }
+  for (unsigned it = 0; live(it); it++) {
+    const unsigned row = row_of(it);
     const int hA = (2 * it) % 3, hB = (2 * it + 1) % 3;
     const unsigned parA = ((2 * it) / 3) & 1, parB = ((2 * it + 1) / 3) & 1;
     float2* const bufA = hbuf + hA * HALF;
@@ -193,7 +269,51 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
       float2* const pa = bufA + j;
       float2* const pb = bufB + j;
       float2 a[16], b[16];
-      if constexpr (CHIRP == 5) {
+      if constexpr (SRC == 1) {
+        // rows j, j + 1 of each half are 128 contiguous bytes: eight 16-byte pieces (columns 2 (p & 3), 2 (p & 3) + 1
+        // of row j + (p >> 2)), read in the lane-rotated order p = q ^ (tid & 7) so that a quarter warp touches eight
+        // distinct bank groups, s1 + chirp applied in that order (the phases of piece p are the p-th pair of the
+        // row pair's 16 table entries), then put back in order by three conditional swaps
+        const int rot = tid & 7, box = tid >> 7;
+        const float2* const ph = reinterpret_cast<const float2*>(cp.phase + (size_t)row * L + 8 * j);
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          mbar_wait(&mbar[(h ? hB : hA) * 8 + box], h ? parB : parA);
+          const float4* const src = reinterpret_cast<const float4*>((h ? bufB : bufA) + 8 * j);
+          float4 v[8];
+#pragma unroll
+          for (int q = 0; q < 8; q++) {
+            const float2 g = __ldg(ph + (size_t)h * (L / 16) * 4 + (q ^ rot));
+            const float4 x = src[q ^ rot];
+            const float2 y0 = chirp_point_tab(make_float2(x.x, x.y), g.x, limit, cp.coef);
+            const float2 y1 = chirp_point_tab(make_float2(x.z, x.w), g.y, limit, cp.coef);
+            v[q] = make_float4(y0.x, y0.y, y1.x, y1.y);
+          }
+#pragma unroll
+          for (int bit = 1; bit < 8; bit <<= 1) {
+            const bool sw = (rot & bit) != 0;
+#pragma unroll
+            for (int p = 0; p < 8; p++)
+              if (!(p & bit)) {
+                const float4 x0 = v[p], x1 = v[p | bit];
+                v[p] = sw ? x1 : x0;
+                v[p | bit] = sw ? x0 : x1;
+              }
+          }
+#pragma unroll
+          for (int p = 0; p < 8; p++) {
+            const int c = 2 * (p & 3);  // columns c, c + 1 -> d0 = 2 c + h, 2 c + 2 + h
+            const float2 y0 = make_float2(v[p].x, v[p].y), y1 = make_float2(v[p].z, v[p].w);
+            if (p < 4) {
+              a[2 * c + h] = y0;
+              a[2 * c + 2 + h] = y1;
+            } else {
+              b[2 * c + h] = y0;
+              b[2 * c + 2 + h] = y1;
+            }
+          }
+        }
+      } else if constexpr (CHIRP == 5) {
         // tabulated phases (two adjacent bins per 8-byte load, prefetched into L2 while the previous row was stored):
         // s1 + chirp applied as the pairs are taken out of shared memory, no pass of its own and no fp64
         const float2* const ph = reinterpret_cast<const float2*>(cp.phase + (size_t)row * L + j);
@@ -246,7 +366,7 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
           *reinterpret_cast<float4*>(p) = make_float4(ya.x, ya.y, yb.x, yb.y);
         }
       }
-      if constexpr (CHIRP != 5) {
+      if constexpr (CHIRP != 5 && SRC != 1) {
 #pragma unroll
         for (int i = 0; i < 16; i++) {
           if constexpr (CHIRP == 0) mbar_wait(&mbar[(i < 8 ? hA : hB) * 8 + (i & 7)], i < 8 ? parA : parB);
@@ -260,6 +380,7 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
       const float4 w = *reinterpret_cast<const float4*>(T0 + j);
       bigrow_twiddle_powers(a, make_float2(w.x, w.y));
       bigrow_twiddle_powers(b, make_float2(w.z, w.w));
+      if constexpr (SRC == 1) __syncthreads();  // every thread has gathered its rows before the layout is rewritten
 #pragma unroll
       for (int i = 0; i < 16; i++)
         *reinterpret_cast<float4*>((i < 8 ? pa : pb) + (i & 7) * S1) = make_float4(a[i].x, a[i].y, b[i].x, b[i].y);
@@ -329,7 +450,8 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
         slot[32 + wid] = s4;
       }
     }
-    __syncthreads();
+    if constexpr (SRC == 2) cluster_sync_all();  // both rows of the pair are transformed
+    else __syncthreads();
     if constexpr (SK) {
       // every warp folds the NW per-warp partials with the same fixed shuffle tree
       const float* const slot = red + (it & 1) * 64;
@@ -344,9 +466,53 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
       const float sk = (float)L * (b / (a * a));
       zap = (sk > skp.thr_hi || sk < skp.thr_lo);  // NaN (all-zero row): untouched (rfi_mitigation.hpp:333-339)
     }
-    if (row + gridDim.x < nrows) prefetch_phase(row + gridDim.x);
+    if (live(it + 1)) prefetch_phase(row_of(it + 1));
+    if constexpr (SRC == 2) {
+      // ---- R2C split and natural-order store of row k1 = row: X[k1 + P k2] from Z[k1][k2] and the mirror Z[M - k],
+      // which the partner CTA holds (itself for rows 0 and P / 2). Lanes as in pass 2 below.
+      const int pd0 = lane & 15, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
+      const float2* const base = half_of(pd0) + pd1 * S2 + 2 * sel;
+      const unsigned prank = (row == 0 || 2 * row == nrows) ? crank : (crank ^ 1);
+      // for k1 != 0 the mirror of k2 is L - 1 - k2: every digit complemented, (d0, d1, d2, d3) -> (15 - d0, 15 - d1,
+      // 15 - d2, 3 - d3), i.e. the 16-byte pair at sel' = 1 - sel with its halves swapped
+      const uint32_t mbase = dsmem_addr(half_of(15 - pd0) + (15 - pd1) * S2 + 2 * (1 - sel), prank);
+      const int kb = pd0 + 16 * pd1 + 4096 * (2 * sel);  // k2 of d2 = 0, d3 = 2 sel
+      float2 wb;  // e^{-i pi (k1 + P kb) / M}; both fractions are exact in fp32
+      {
+        float sn, cs;
+        sincospif(-((float)row / ((float)nrows * (float)L) + (float)kb / (float)L), &sn, &cs);
+        wb = make_float2(cs, sn);
+      }
+      const float2* const htw = reinterpret_cast<const float2*>(red);
+      auto pos = [&](int k) {  // shared-memory position of natural-order k2 (pass 2's digit map)
+        return half_of(k & 15) + ((k >> 4) & 15) * S2 + ((k >> 8) & 15) * R3 + (k >> 12);
+      };
+      float2* const o = out + (size_t)row * L + kb;
+      float ps = 0.f;
+#pragma unroll 4
+      for (int i2 = 0; i2 < 16; i2++) {
+        const float4 q = *reinterpret_cast<const float4*>(base + i2 * R3);
+        float2 m0, m1;
+        if (row != 0) {
+          const float4 m = ld_dsmem_f4(mbase + (uint32_t)((15 - i2) * R3 * sizeof(float2)));
+          m0 = make_float2(m.z, m.w);
+          m1 = make_float2(m.x, m.y);
+        } else {  // row 0 pairs k2 with (L - k2) mod L, in this CTA
+          const int k0 = kb + 256 * i2;
+          m0 = *pos((L - k0) & (L - 1));
+          m1 = *pos((L - k0 - 4096) & (L - 1));
+        }
+        const float2 w0 = c_mul(wb, htw[i2]);
+        const float2 w1 = c_mul(w0, make_float2(0.70710678118654752440f, -0.70710678118654752440f));  // k2 + L / 4
+        const float2 x0 = r2c_split_point(make_float2(q.x, q.y), m0, w0);
+        const float2 x1 = r2c_split_point(make_float2(q.z, q.w), m1, w1);
+        o[256 * i2] = x0;
+        o[256 * i2 + 4096] = x1;
+        ps += (x0.x * x0.x + x0.y * x0.y) + (x1.x * x1.x + x1.y * x1.y);
+      }
+      psum += (double)ps;
+    } else {
     // ---- pass 2: natural-order store. lane -> (d0, d1 bit 0): 32 consecutive output indices per instruction
-    {
       const int pd0 = lane & 15, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
       const float2* const base = half_of(pd0) + pd1 * S2 + 2 * sel;
       float2* const o = out + (size_t)row * L + (pd0 + 16 * pd1 + 4096 * (2 * sel));
@@ -374,13 +540,66 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
         }
       }
     }
-    __syncthreads();  // the row's buffers are free: second half of the next row, first half of the one after
+    // the row's buffers are free (SRC = 2: once the partner has read them too): second half of the next row, first half
+    // of the one after
+    if constexpr (SRC == 2) cluster_sync_all();
+    else __syncthreads();
     if (wid == 0) {
-      const unsigned nxt = row + gridDim.x, nxt2 = row + 2 * gridDim.x;
-      if (nxt < nrows) issue_half(nxt, 1, hA);     // B of row it + 1 is A of row it
-      if (nxt2 < nrows) issue_half(nxt2, 0, hB);   // A of row it + 2 is B of row it
+      if (live(it + 1)) issue_half(row_of(it + 1), 1, hA);  // B of row it + 1 is A of row it
+      if (live(it + 2)) issue_half(row_of(it + 2), 0, hB);  // A of row it + 2 is B of row it
     }
   }
+  if constexpr (SRC == 2) {
+    // Σ|X|^2: per-CTA partial, then the last CTA folds the partials in index order (as r2c_col0_fixup_kernel does)
+    double* const redd = reinterpret_cast<double*>(red + 64);
+    unsigned* const last = reinterpret_cast<unsigned*>(red + 96);
+    double v = psum;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) redd[wid] = v;
+    __syncthreads();
+    if (tid == 0) {
+      double a = 0.0;
+      for (int w = 0; w < NW; w++) a += redd[w];
+      rr.partial[blockIdx.x] = a;
+      __threadfence();
+      *last = (atomicAdd(rr.ticket, 1u) == gridDim.x - 1) ? 1u : 0u;
+      if (*last) __threadfence();
+    }
+    __syncthreads();
+    if (*last && wid == 0) {
+      double a = 0.0;
+      for (unsigned i = lane; i < gridDim.x; i += 32) a += __ldcg(&rr.partial[i]);
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+      if (lane == 0) {
+        *rr.mean = (float)a / ((float)nrows * (float)L);
+        *rr.ticket = 0;
+      }
+    }
+  }
+}
+
+template <int LOGL, bool FWD, bool SK, int CHIRP>
+__global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
+    fft_bigrow_kernel(const float2* __restrict__ in, float2* __restrict__ out, unsigned nrows,
+                      const float2* __restrict__ tabs, row_sk_params skp, row_chirp_params cp) {
+  bigrow_body<LOGL, FWD, SK, CHIRP, 0>(in, out, nrows, tabs, skp, cp, nullptr, r2c_rows_params{});
+}
+
+// the sweep-order R2C route of 2^25-point blocks with rows of 2^14 (srtb_b200.cu, r2c_sweep_order): the paired row
+// sweep with the split (clusters of two CTAs, in place on the [P][L] scratch) ...
+__global__ void __launch_bounds__(bigrow<14>::NT, 1)
+    r2c_rows_split_kernel(float2* __restrict__ z, unsigned nrows, const float2* __restrict__ tabs, r2c_rows_params rr) {
+  bigrow_body<14, true, false, 0, 2>(z, z, nrows, tabs, row_sk_params{}, row_chirp_params{}, nullptr, rr);
+}
+
+// ... and the whole-row waterfall kernel reading channel `row` of that spectrum through a tensor map
+__global__ void __launch_bounds__(bigrow<14>::NT, 1)
+    waterfall_sweep_order_kernel(const float2* __restrict__ in, float2* __restrict__ out, unsigned nrows,
+                                 const float2* __restrict__ tabs, row_sk_params skp, row_chirp_params cp,
+                                 const __grid_constant__ tensor_map_blob tmap) {
+  bigrow_body<14, false, true, 5, 1>(in, out, nrows, tabs, skp, cp, &tmap, r2c_rows_params{});
 }
 
 }  // namespace srtb_b200

@@ -750,10 +750,16 @@ __device__ __forceinline__ float2 chirp_point_tab(float2 v, float ang, float lim
 // correctly rounded reciprocal), reduced to [-1/2, 1/2] cycles and stored as the fp32 angle -2 pi frac(k) — the very
 // value chirp_point hands to the SFU, so both routes agree to the last bit of the argument. DM and band are constants
 // of a run, so the table is part of the plan like the twiddles.
+// logp != 0: the order in which the whole-row kernel reads a sweep-order spectrum (fft_bigrow_kernel, SRC = 1), channel
+// by channel: entry ch L + 8 k1 + c (L = 2^(logp + 3)) holds bin k1 + 2^logp (8 ch + c), so one channel's phases stay
+// one contiguous range
 __global__ void __launch_bounds__(256) chirp_phase_table_kernel(float* __restrict__ out, size_t n, double f_min,
-                                                                double df, double inv_fc, double f_c, double ddm) {
+                                                                double df, double inv_fc, double f_c, double ddm,
+                                                                unsigned logp) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const double f = fma(df, (double)i, f_min);
+    const size_t ch = i >> (logp + 3), r = i & ((((size_t)8) << logp) - 1);
+    const size_t bin = logp ? (r >> 3) + ((8 * ch + (r & 7)) << logp) : i;
+    const double f = fma(df, (double)bin, f_min);
     const double q = (f - f_c) * inv_fc;
     const double k = (ddm * __drcp_rn(f)) * (q * q);
     const float fr = (float)(k - rint(k));  // the difference is exact, in [-1/2, 1/2]
@@ -1041,13 +1047,16 @@ struct tile_tma_smem {
 // stages run) so that three CTAs fit an SM at L = 512. With T = 8 a row of the exchange tile is 64 bytes — half the
 // banks — and the four rows a warp writes after a radix-16 stage would all have the same parity: one spare row
 // after every sixteen (tile rows r -> r + (r >> 4)) spreads them again.
+// From L = 2048 (a 128 KiB exchange tile) ONE raw tile buffer is kept: stage 0 decodes the tile into registers at the
+// start, so the next tile lands in the same buffer while the stages run (one CTA per SM at 1024 threads).
 template <int LOGL, int T>
 struct raw16_smem {
   static constexpr int L = 1 << LOGL;
   static constexpr int BUF = T * L;
   static constexpr bool PAD = (T == 8) && ((L / 16) % 16 == 0);
   static constexpr int XBUF = PAD ? BUF + BUF / 16 : BUF;
-  static constexpr size_t bytes = (size_t)XBUF * sizeof(float2) + 2 * (size_t)BUF * 4 + 128 + (size_t)L * sizeof(float2);
+  static constexpr int NRAW = (LOGL >= 11) ? 1 : 2;
+  static constexpr size_t bytes = (size_t)XBUF * sizeof(float2) + NRAW * (size_t)BUF * 4 + 128 + (size_t)L * sizeof(float2);
 };
 
 // the same two measures for the plain (complex input) sixteen-point column sweep with 64-byte tile rows: both TMA
@@ -1196,11 +1205,12 @@ struct col16_threads {
 // applied to the spectrum as the tile's points are taken out of shared memory (the bin of point idx of column b0 + t
 // of row a is a L B + idx B + b0 + t); 1/f by Newton steps from the point U B bins below (cp.newton = 1 or 2 steps,
 // else the exact reciprocal), like the whole-row kernel.
-template <int LOGL, int T, bool FWD, int RAW = 0, bool CH = false>
-__global__ void __launch_bounds__(col16_threads<LOGL, T>::value, CH ? 2 : col16_threads<LOGL, T>::min_blocks)
-    fft_col16_tma_kernel(const __grid_constant__ tensor_map_blob tmap, float2* __restrict__ out, size_t B,
-                         uint32_t btiles, uint32_t ntiles, big_twiddle btw, const float2* __restrict__ tw,
-                         raw_params rp, row_chirp_params cp) {
+template <int LOGL, int T, bool FWD, int RAW, bool CH>
+__device__ __forceinline__ void col16_body(const tensor_map_blob* tmap_, float2* __restrict__ out, size_t B,
+                                           uint32_t btiles, uint32_t ntiles, const big_twiddle& btw,
+                                           const float2* __restrict__ tw, const raw_params& rp,
+                                           const row_chirp_params& cp) {
+  const tensor_map_blob& tmap = *tmap_;
   using SC = sched16<LOGL>;
   constexpr int L = 1 << LOGL, U = L / 16, S = SC::S, BUF = tile_tma_smem<LOGL, T>::BUF;
   constexpr int ROWS_PER_BOX = (L < 256) ? L : 256;
@@ -1212,10 +1222,11 @@ __global__ void __launch_bounds__(col16_threads<LOGL, T>::value, CH ? 2 : col16_
   extern __shared__ __align__(128) unsigned char smraw[];
   float2* const buf0 = reinterpret_cast<float2*>(smraw);
   float2* const buf1 = buf0 + XBUF;
+  constexpr bool ONE_RAW = (RAW != 0) && raw16_smem<LOGL, T>::NRAW == 1;
   unsigned char* const raw0 = reinterpret_cast<unsigned char*>(buf1);
-  unsigned char* const raw1 = raw0 + (size_t)BUF * 4;
-  // RAW: right after the two raw tiles (2 * 4 BUF bytes = BUF elements); else after the second tile buffer
-  uint64_t* const mbar = reinterpret_cast<uint64_t*>(buf1 + ((RAW != 0) ? BUF : XBUF));
+  unsigned char* const raw1 = ONE_RAW ? raw0 : raw0 + (size_t)BUF * 4;
+  // RAW: right after the raw tiles (4 BUF bytes = BUF / 2 elements each); else after the second tile buffer
+  uint64_t* const mbar = reinterpret_cast<uint64_t*>(buf1 + ((RAW != 0) ? raw16_smem<LOGL, T>::NRAW * BUF / 2 : XBUF));
   float2* const ltw = reinterpret_cast<float2*>(reinterpret_cast<unsigned char*>(mbar) + 128);
   const float2* const stw = STWG ? btw.tab : ltw + L;
   const int tid = threadIdx.x;
@@ -1251,11 +1262,11 @@ __global__ void __launch_bounds__(col16_threads<LOGL, T>::value, CH ? 2 : col16_
   uint32_t tile = blockIdx.x;
   if (tile < ntiles && tid == 0) issue(tile, 0);
   for (uint32_t it = 0; tile < ntiles; tile += gridDim.x, it++) {
-    const int b = it & 1;
+    const int b = ONE_RAW ? 0 : (it & 1);
     float2* const sm = (RAW == 0) ? (b ? buf1 : buf0) : buf0;
     const uint32_t nxt = tile + gridDim.x;
-    if (nxt < ntiles && tid == 0) issue(nxt, b ^ 1);
-    mbar_wait(&mbar[b], (it >> 1) & 1);
+    if (!ONE_RAW && nxt < ntiles && tid == 0) issue(nxt, b ^ 1);
+    mbar_wait(&mbar[b], ONE_RAW ? (it & 1) : ((it >> 1) & 1));
     float2 v[16];
     int oidx[16];
     const int up = PADX ? u + (u >> 4) : u;  // tile row of slot 0
@@ -1319,6 +1330,10 @@ __global__ void __launch_bounds__(col16_threads<LOGL, T>::value, CH ? 2 : col16_
         else v[e] = make_float2((float)g[rp.o0], (float)g[rp.o1]);
       }
     }
+    if constexpr (ONE_RAW) {
+      __syncthreads();  // the raw tile is decoded: the next one may land in its buffer while the stages run
+      if (nxt < ntiles && tid == 0) issue(nxt, 0);
+    }
     stage_compute16<LOGL, SC::logr(0), 0, FWD, LOGL - SC::logr(0), PADX>(v, u, ltw, oidx);
     if constexpr (RAW == 0) __syncthreads();  // every thread has read the tile before it is overwritten
 #pragma unroll
@@ -1361,6 +1376,24 @@ __global__ void __launch_bounds__(col16_threads<LOGL, T>::value, CH ? 2 : col16_
     }
     __syncthreads();  // buffer b (and the exchange buffer) may be refilled from the next iteration on
   }
+}
+
+template <int LOGL, int T, bool FWD, int RAW = 0, bool CH = false>
+__global__ void __launch_bounds__(col16_threads<LOGL, T>::value, CH ? 2 : col16_threads<LOGL, T>::min_blocks)
+    fft_col16_tma_kernel(const __grid_constant__ tensor_map_blob tmap, float2* __restrict__ out, size_t B,
+                         uint32_t btiles, uint32_t ntiles, big_twiddle btw, const float2* __restrict__ tw,
+                         raw_params rp, row_chirp_params cp) {
+  col16_body<LOGL, T, FWD, RAW, CH>(&tmap, out, B, btiles, ntiles, btw, tw, rp, cp);
+}
+
+// the first sweep of the sweep-order R2C route (srtb_b200.cu, r2c_sweep_order): 2^11-point raw columns, T = 8, one
+// raw tile buffer (raw16_smem), one CTA of 1024 threads per SM
+template <int RAW>
+__global__ void __launch_bounds__(col16_threads<11, 8>::value, 1)
+    r2c_raw_col2048_kernel(const __grid_constant__ tensor_map_blob tmap, float2* __restrict__ out, size_t B,
+                           uint32_t btiles, uint32_t ntiles, big_twiddle btw, const float2* __restrict__ tw,
+                           raw_params rp) {
+  col16_body<11, 8, true, RAW, false>(&tmap, out, B, btiles, ntiles, btw, tw, rp, row_chirp_params{});
 }
 
 // Transposing last pass, persistent: input rows [beta][k1][rest][L] as a 3-D tensor (L, S, L1*batch);

@@ -544,16 +544,19 @@ __global__ void __launch_bounds__(256) rfi_s1_apply_kernel(float2* __restrict__ 
 }
 
 // K11 manual zap (S/spectrum/rfi_mitigation.hpp:137-143): blockIdx.y = range
+// logp != 0: the spectrum is in sweep order, bin k at (k mod 2^logp) 2^logq + k / 2^logp
 struct bin_ranges {
   unsigned long long lo[16], hi[16];
+  unsigned logp, logq;
 };
 __global__ void __launch_bounds__(256) rfi_zero_ranges_kernel(float2* __restrict__ x, bin_ranges r) {
   pdl_launch_dependents();
   pdl_wait();
   const size_t lo = r.lo[blockIdx.y], hi = r.hi[blockIdx.y];
   const size_t stride = (size_t)gridDim.x * blockDim.x;
+  const size_t pmask = ((size_t)1 << r.logp) - 1;
   for (size_t i = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i <= hi; i += stride)
-    x[i] = make_float2(0.f, 0.f);
+    x[((i & pmask) << r.logq) + (i >> r.logp)] = make_float2(0.f, 0.f);
 }
 
 // ------------------------------------------------------------------------------

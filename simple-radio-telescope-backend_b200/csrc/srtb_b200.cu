@@ -119,7 +119,7 @@ struct srtb_b200_ctx {
   // K12 phase table of the current (block geometry, DM): see chirp_phase_table_kernel
   float* chirp_tab = nullptr;
   size_t chirp_tab_bytes = 0;
-  double chirp_tab_key[6] = {0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm
+  double chirp_tab_key[7] = {0, 0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm, layout (logp)
   // simplify_spectrum: row-resampled intensities R[C][W] and the column stage's per-CTA partial sums
   float* thumb_rows = nullptr;
   size_t thumb_rows_bytes = 0;
@@ -784,10 +784,10 @@ struct raw_source {
 
 // the first sweep of the packed R2C plans that take the raw route is 2^7 .. 2^9 points long (plan3 / plan4 on a
 // 16-byte aligned buffer; the two-sweep plans with a first sweep of 2^10 end on a 2^9 or 2^10 last sweep, which has no
-// fused R2C split)
+// fused R2C split), or 2^11 on the sweep-order route of 2^25-point blocks (r2c_sweep_order)
 template <int LOGL, int RAW, int TT = col_t<LOGL>::value>
 static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2* out, size_t B, bool* done) {
-  static_assert(LOGL >= 7 && LOGL <= 9, "raw first sweep: sixteen-point column kernel only");
+  static_assert((LOGL >= 7 && LOGL <= 9) || LOGL == 11, "raw first sweep: sixteen-point column kernel only");
   constexpr int T = TT, L = 1 << LOGL;
   if constexpr (LOGL == 7 && TT == col_t<LOGL>::value) {
     if (wide_col(1, L, B)) return launch_col_tma_raw<LOGL, RAW, 32>(ctx, src, out, B, done);
@@ -811,12 +811,19 @@ static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2*
   const size_t ntiles = B / T;
   unsigned grid = 1;
   const raw_params rp{src.G, src.o0, src.o1, src.delta, (int)row_bytes, src.bits};
-  auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
   constexpr int threads = col16_threads<LOGL, T>::value;
   constexpr size_t smem16 = raw16_smem<LOGL, T>::bytes;  // inter-sweep tables stay in global memory here
-  if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
-  CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
-                row_chirp_params{}));
+  if constexpr (LOGL == 11) {
+    static_assert(T == 8, "the 2^11-point raw sweep has 32-byte raw rows and 64-byte stores");
+    auto kern = r2c_raw_col2048_kernel<RAW>;
+    if (int rc = persistent_grid(ctx, kern, threads, smem16, smem16, ntiles, &grid)) return rc;
+    CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp));
+  } else {
+    auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
+    if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
+    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
+                  row_chirp_params{}));
+  }
   ctx->launches++;
   CK(cudaGetLastError());
   *done = true;
@@ -836,6 +843,7 @@ static int dispatch_col_raw(srtb_b200_ctx* ctx, int logl, const raw_source& src,
     case 7: return src.is_signed ? launch_col_tma_raw<7, 1>(ctx, src, out, B, done) : launch_col_tma_raw<7, 2>(ctx, src, out, B, done);
     case 8: return src.is_signed ? launch_col_tma_raw<8, 1>(ctx, src, out, B, done) : launch_col_tma_raw<8, 2>(ctx, src, out, B, done);
     case 9: return src.is_signed ? launch_col_tma_raw<9, 1>(ctx, src, out, B, done) : launch_col_tma_raw<9, 2>(ctx, src, out, B, done);
+    case 11: return src.is_signed ? launch_col_tma_raw<11, 1>(ctx, src, out, B, done) : launch_col_tma_raw<11, 2>(ctx, src, out, B, done);
     default: return 0;
   }
 }
@@ -979,16 +987,17 @@ static int get_bigrow_tables(srtb_b200_ctx* ctx, bool fwd, const float2** out) {
   return 0;
 }
 
-// sk != nullptr: SK + column sums in the epilogue (sk->partial is filled in here); chirp != nullptr: s1 + chirp on load
+// sk != nullptr: SK + column sums in the epilogue (sk->partial is filled in here); chirp != nullptr: s1 + chirp on load.
+// sweep_order: `in` is the [P][L] spectrum r2c_sweep_order leaves (P = nrows = L / 8), read channel by channel
 template <int LOGL, bool FWD>
 static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size_t nrows, row_sk_params* sk,
-                         const row_chirp_params* chirp, size_t* chunks_out) {
+                         const row_chirp_params* chirp, size_t* chunks_out, bool sweep_order = false) {
   using C = bigrow<LOGL>;
   if (nrows >= ((size_t)1 << 31)) return fail(ctx, SRTB_B200_E_SIZE, "fft: too many rows");
   const float2* tabs = nullptr;
   if (int rc = get_bigrow_tables<LOGL>(ctx, FWD, &tabs)) return rc;
   unsigned grid = 1;
-  auto go = [&](auto kern, bool with_sk) -> int {
+  auto go = [&](auto kern, bool with_sk, auto... extra) -> int {
     const size_t smem = C::bytes;
     if (int rc = persistent_grid(ctx, kern, C::NT, smem, smem, nrows, &grid)) return rc;
     row_sk_params p{};
@@ -997,12 +1006,27 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
       sk->partial = ctx->lane.colsum_partial;
       p = *sk;
     }
-    CK(launch_pdl(ctx, kern, dim3(grid), dim3(C::NT), smem, in, out, (unsigned)nrows, tabs, p, chirp ? *chirp : row_chirp_params{}));
+    CK(launch_pdl(ctx, kern, dim3(grid), dim3(C::NT), smem, in, out, (unsigned)nrows, tabs, p,
+                  chirp ? *chirp : row_chirp_params{}, extra...));
     ctx->launches++;
     CK(cudaGetLastError());
     if (chunks_out) *chunks_out = grid;
     return 0;
   };
+  if constexpr (!FWD && LOGL == 14) {
+    if (sweep_order) {
+      if (!(sk && chirp && chirp->newton == 5) || nrows * 8 != (size_t)C::L)
+        return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: the sweep-order load needs the phase table and P = L / 8");
+      const cuuint64_t dims[2] = {(cuuint64_t)C::L, (cuuint64_t)nrows};
+      const cuuint64_t strides[1] = {(cuuint64_t)C::L * sizeof(float2)};
+      const cuuint32_t box[2] = {8u, 256u};
+      tensor_map_blob tm;
+      if (!make_tensor_map(&tm, in, 2, dims, strides, box))
+        return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: tensor map of the sweep-order spectrum refused");
+      return go(waterfall_sweep_order_kernel, true, tm);
+    }
+  }
+  if (sweep_order) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: sweep-order load exists for rows of 2^14");
   if constexpr (!FWD) {
     if (sk && chirp && chirp->newton == 5) return go(fft_bigrow_kernel<LOGL, false, true, 5>, true);
     if (sk && chirp && chirp->newton == 1) return go(fft_bigrow_kernel<LOGL, false, true, 1>, true);
@@ -1012,6 +1036,46 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
   }
   if (sk || chirp) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "fft: fused epilogue exists for the backward transform with the chirp only");
   return go(fft_bigrow_kernel<LOGL, FWD, false, 0>, false);
+}
+
+// the R2C row sweep of the sweep-order route: P rows of 2^14 points in place on s (clusters of two CTAs),
+// leaving mean(|X_k|^2, k < M) in the lane's `mean`
+static int launch_r2c_rows(srtb_b200_ctx* ctx, float2* s, size_t P) {
+  using C = bigrow<14>;
+  auto kern = r2c_rows_split_kernel;
+  const float2* tabs = nullptr;
+  if (int rc = get_bigrow_tables<14>(ctx, true, &tabs)) return rc;
+  cudaLaunchConfig_t cfg{};
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2;
+  attr[0].val.clusterDim.y = 1;
+  attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.blockDim = dim3(C::NT);
+  cfg.dynamicSmemBytes = C::bytes;
+  cfg.stream = ctx->lane.stream;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  const void* key = reinterpret_cast<const void*>(kern);
+  if (!ctx->configured.count(key)) {
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::bytes));
+    int clusters = 0;
+    cfg.gridDim = dim3(2 * (unsigned)ctx->sm_count);
+    CK(cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg));
+    if (clusters < 1) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "r2c: no two-CTA cluster of the row sweep fits an SM pair");
+    ctx->occupancy[key] = clusters;
+    ctx->configured.insert(key);
+  }
+  const unsigned clusters = (unsigned)std::min<size_t>(P / 2, (size_t)ctx->occupancy[key]);
+  if (2 * clusters > 4096) return fail(ctx, SRTB_B200_E_SIZE, "r2c: partial buffer too small");
+  cfg.gridDim = dim3(2 * clusters);
+  cfg.numAttrs = ctx->pdl_auto ? 2 : 1;
+  CK(cudaLaunchKernelEx(&cfg, kern, s, (unsigned)P, tabs, r2c_rows_params{ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean}));
+  ctx->launches++;
+  CK(cudaGetLastError());
+  return 0;
 }
 
 // L = 2 or 4: one thread per row
@@ -1325,10 +1389,14 @@ extern "C" int srtb_b200_rfi_range_to_bins(float f1, float f2, float freq_low, f
   return 0;
 }
 
-// mitigate_rfi_manual (rfi_mitigation.hpp:97-158): zero the listed bin ranges, 16 ranges per launch
-static int zero_bin_ranges(srtb_b200_ctx* ctx, float2* x, const std::vector<size_t>& bins) {
+// mitigate_rfi_manual (rfi_mitigation.hpp:97-158): zero the listed bin ranges, 16 ranges per launch. logp != 0: x holds
+// the spectrum in sweep order (bin k at (k mod 2^logp) 2^logq + k / 2^logp, r2c_sweep_order)
+static int zero_bin_ranges(srtb_b200_ctx* ctx, float2* x, const std::vector<size_t>& bins, unsigned logp = 0,
+                           unsigned logq = 0) {
   for (size_t r0 = 0; r0 < bins.size() / 2; r0 += 16) {
     bin_ranges br;
+    br.logp = logp;
+    br.logq = logq;
     const size_t nr = std::min<size_t>(16, bins.size() / 2 - r0);
     size_t longest = 1;
     for (size_t r = 0; r < nr; r++) {
@@ -1574,7 +1642,7 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
 static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_t time_count, size_t chan_count,
                                   size_t time_reserved_count, float sk_threshold, float snr, float chan_thr,
                                   size_t max_boxcar, const row_chirp_params* chirp = nullptr,
-                                  const float2* src = nullptr) {
+                                  const float2* src = nullptr, bool sweep_order = false) {
   const size_t ts_count = (time_count <= time_reserved_count) ? time_count : time_count - time_reserved_count;
   if (int rc = detect_prepare(ctx, slot, time_count, 1)) return rc;
   // the result header is zeroed here unless the block path did it for every stream up front (a memset between two
@@ -1609,7 +1677,8 @@ static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_
     }
     const float2* s_ = src ? src : x;
     rc = (time_count == 8192) ? launch_bigrow<13, false>(ctx, s_, x, chan_count, &p, chirp ? &cpv : nullptr, &chunks)
-                              : launch_bigrow<14, false>(ctx, s_, x, chan_count, &p, chirp ? &cpv : nullptr, &chunks);
+                              : launch_bigrow<14, false>(ctx, s_, x, chan_count, &p, chirp ? &cpv : nullptr, &chunks,
+                                                         sweep_order);
     if (rc) return rc;
     stats_.reset();
     return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, chunks, snr, chan_thr, max_boxcar);
@@ -1870,10 +1939,12 @@ static int ensure_stream_bufs(srtb_b200_ctx* ctx, float* (&bufs)[4], size_t* ele
 // K12 phase table for the whole-row waterfall kernel (block path; the DM sweep, and tables above 4 GiB, evaluate every
 // phase on the fly). Rebuilt when the geometry or the DM changes; built synchronously, so both lanes and any later
 // launch may read it.
-static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params& cp, const float** out) {
+// logp != 0: the sweep-order layout of r2c_sweep_order, channel by channel (chirp_phase_table_kernel)
+static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params& cp, const float** out,
+                           unsigned logp = 0) {
   *out = nullptr;
   if (n * sizeof(float) > ((size_t)4 << 30)) return 0;
-  const double key[6] = {(double)n, cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm};
+  const double key[7] = {(double)n, cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm, (double)logp};
   if (ctx->chirp_tab && std::memcmp(key, ctx->chirp_tab_key, sizeof(key)) == 0) {
     *out = ctx->chirp_tab;
     return 0;
@@ -1881,7 +1952,7 @@ static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params&
   if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->chirp_tab), &ctx->chirp_tab_bytes, n * sizeof(float))) return rc;
   if (int rc = sync_lanes(ctx)) return rc;  // a block still in flight may be reading the previous table
   chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(ctx->chirp_tab, n, cp.f_min, cp.df, cp.inv_fc,
-                                                                           cp.f_c, cp.ddm);
+                                                                           cp.f_c, cp.ddm, logp);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(ctx->lane.stream));
   std::memcpy(ctx->chirp_tab_key, key, sizeof(key));
@@ -1979,6 +2050,36 @@ static int block_input_init(srtb_b200_ctx* ctx, const block_params& p, block_inp
   return in->fuse_unpack ? 0 : unpack_block(ctx, p, in);
 }
 
+// The sweep-order route of 2^25-point R2Cs with rows of 2^14 (config #3): M = P Q, P = 2^11, Q = L = 2^14. Sweep 1 is the
+// raw-fused 2^11-point column sweep into the lane's scratch, sweep 2 the R2C row sweep (2^14-point rows, split, Σ|X|^2)
+// in place; bin k = k1 + P k2 then sits at k1 Q + k2, channel c is the box of all P rows by columns 8c .. 8c + 7, and
+// the whole-row waterfall kernel reads it from there (24 bytes per sample per stream instead of 32: no third sweep,
+// no fix-up). Taken when the unpack is fused (8-bit samples), the geometry is this one, every buffer is 16-byte
+// aligned and TMA tensor maps can be encoded; everything else keeps the three-sweep plan.
+constexpr unsigned SWEEP_LOGP = 11, SWEEP_LOGQ = 14;
+static bool r2c_sweep_order(const block_params& p, const block_input& in) {
+  if (!in.fuse_unpack || in.raw[0].bits != 0 || p.L != ((size_t)1 << SWEEP_LOGQ) ||
+      p.Nc != ((size_t)1 << (SWEEP_LOGP + SWEEP_LOGQ)) || !get_encode_tiled())
+    return false;
+  if (reinterpret_cast<uintptr_t>(in.raw[0].base) & 15u) return false;
+  for (int s = 0; s < p.streams; s++)
+    if (reinterpret_cast<uintptr_t>(in.bufs[s]) & 15u) return false;
+  return true;
+}
+
+static int r2c_sweep_order_stream(srtb_b200_ctx* ctx, const block_params& p, const block_input& in, int s,
+                                  float2** spectrum) {
+  const size_t P = (size_t)1 << SWEEP_LOGP, Q = (size_t)1 << SWEEP_LOGQ;
+  if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, P * Q * sizeof(float2))) return rc;
+  float2* const z = static_cast<float2*>(ctx->lane.fft_scratch);
+  bool done = false;
+  if (int rc = dispatch_col_raw(ctx, (int)SWEEP_LOGP, in.raw[s], z, Q, &done)) return rc;
+  if (!done) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "r2c: the raw 2^11-point column sweep refused the block");
+  if (int rc = launch_r2c_rows(ctx, z, P)) return rc;
+  *spectrum = z;
+  return 0;
+}
+
 // R2C of stream s in its buffer, leaving mean(|X|^2) in the lane's `mean`. When the fused route refuses this size or
 // alignment, all streams are unpacked once and take the plain R2C. The route is a property of the block (same size and
 // base pointer for every stream), so it can only change on stream 0; later it would overwrite finished streams with
@@ -2008,17 +2109,17 @@ static bool chirp_on_load(size_t L) { return chirp_fusable(L) || long_fusable(L)
 // block's DM; the DM sweep changes DM every trial). Both buffers are 16-byte aligned: the ctx allocates them, or
 // submit_block_ex checked the caller's.
 static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, float2* dst, const float2* src, float dm,
-                       bool phase_table) {
+                       bool phase_table, unsigned sweep_logp = 0) {
   const srtb_b200_block_config* cfg = p.cfg;
   const size_t reserved = p.reserved(dm);
   if (chirp_fusable(p.L)) {
-    // ONE kernel: s1 + chirp on load, waterfall FFT, SK, partial column sums
+    // ONE kernel: s1 + chirp on load, waterfall FFT, SK, partial column sums. sweep_logp: src is in sweep order
     row_chirp_params cp = p.chirp(dm, ctx->lane.mean);
     if (phase_table)
-      if (int rc = get_chirp_table(ctx, p.Nc, cp, &cp.phase)) return rc;
+      if (int rc = get_chirp_table(ctx, p.Nc, cp, &cp.phase, sweep_logp)) return rc;
     return watfft_sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                                  cfg->signal_detect_max_boxcar_length, &cp, src);
+                                  cfg->signal_detect_max_boxcar_length, &cp, src, sweep_logp != 0);
   }
   if (long_fusable(p.L)) {
     // long rows: chirp-on-load column sweep, last sweep with SK statistics, decision, column sums (20 bytes per
@@ -2082,9 +2183,20 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
   if (int rc = block_input_init(ctx, p, &in)) return rc;
   if (two_lanes)
     if (int rc = fork_lanes(ctx)) return rc;
+  const bool sweep_order = r2c_sweep_order(p, in);
   auto enqueue_stream = [&](int s) -> int {
     float2* buf = reinterpret_cast<float2*>(bufs[s]);
     if (two_lanes) CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
+    if (sweep_order) {
+      float2* z = nullptr;
+      {
+        stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
+                           (double)p.N * (double)std::abs(p.cfg->baseband_input_bits) / 8.0 + 4.0 * (double)p.N);
+        if (int rc = r2c_sweep_order_stream(ctx, p, in, s, &z)) return rc;
+      }
+      if (int rc = zero_bin_ranges(ctx, z, p.bins, SWEEP_LOGP, SWEEP_LOGQ)) return rc;
+      return stream_tail(ctx, p, s, buf, z, p.cfg->dm, /*phase_table=*/true, SWEEP_LOGP);
+    }
     {
       stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
                          (double)p.N * (in.fuse_unpack ? (double)std::abs(p.cfg->baseband_input_bits) / 8.0 : 4.0) +

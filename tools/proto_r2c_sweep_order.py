@@ -1,0 +1,148 @@
+#!/usr/bin/env python
+"""Index-algebra prototype of the two-sweep config-#3 R2C that leaves its spectrum in sweep order, and of the
+whole-row waterfall kernel reading its channels from that order (csrc/fft_bigrow.cuh, SRC = 1 and 2; the first
+sweep is fft_col16_tma_kernel). Run on the CPU; no GPU needed.  usage: proto_r2c_sweep_order.py [logP logQ]
+
+M = P * Q complex points packed from 2M real samples. Sweep 1 (P-point columns, stride Q) leaves
+Y[k1][n2] = W_M^{k1 n2} sum_n1 x[n1 Q + n2] W_P^{n1 k1}; sweep 2 (Q-point rows) gives Z[k1][k2] = H[k1 + P k2] and
+splits rows k1 and P - k1 together, so bin k = k1 + P k2 of the real transform sits at address k1 Q + k2. A channel
+of L = 8 P bins is then the box of all P rows by 8 columns; the whole-row kernel's stage 0 takes chunk
+d0 = 2 c + h (B1 = L / 16 = P / 2 bins) from column c, rows h P/2 ...
+
+Checks (a) sweeps 1 + 2 + split against numpy.fft.rfft, (b) the mirror rules of the split, including the digit
+complement the kernel uses for rows k1 != 0 at Q = 2^14, (c) the channel gather of stage 0 against numpy's transform
+of each channel, (d) that the stage-0 reads of the sweep-order tile (16-byte pieces, lane-rotated) are conflict free
+per quarter warp at P = 2^11, (e) the phase-table and zap addresses."""
+import sys
+
+import numpy as np
+
+
+def sweeps(logp, logq, seed=1):
+    P, Q = 1 << logp, 1 << logq
+    M = P * Q
+    rng = np.random.default_rng(seed)
+    real = rng.standard_normal(2 * M)
+    x = real[0::2] + 1j * real[1::2]
+    # sweep 1: P-point DFT down each column n2, inter-sweep twiddle W_M^{k1 n2}
+    cols = x.reshape(P, Q)                      # [n1][n2]
+    Y = np.fft.fft(cols, axis=0)                # [k1][n2]
+    k1 = np.arange(P)[:, None]
+    n2 = np.arange(Q)[None, :]
+    Y = Y * np.exp(-2j * np.pi * k1 * n2 / M)
+    # sweep 2: Q-point DFT along each row, in place -> Z[k1][k2] = H[k1 + P k2]
+    Z = np.fft.fft(Y, axis=1)
+    H = np.fft.fft(x)
+    kk = (np.arange(P)[:, None] + P * np.arange(Q)[None, :])
+    assert np.allclose(Z, H[kk]), "sweep order"
+
+    # split: row k1 pairs with row P - k1 (rows 0 and P/2 with themselves)
+    def mirror(r, c):
+        if r == 0:
+            return 0, (Q - c) % Q
+        if r == P // 2:
+            return r, Q - 1 - c
+        return P - r, Q - 1 - c
+
+    X = np.zeros((P, Q), complex)
+    for r in range(P):
+        for c in range(Q):
+            mr, mc = mirror(r, c)
+            k = r + P * c
+            assert (mr + P * mc) % M == (M - k) % M, "mirror rule"
+            zk, zm = Z[r, c], np.conj(Z[mr, mc])
+            w = np.exp(-1j * np.pi * k / M)
+            X[r, c] = 0.5 * (zk + zm) - 0.5j * w * (zk - zm)
+    ref = np.fft.rfft(real)[:M]
+    err = np.abs(X.T.reshape(-1) - ref).max() / np.abs(ref).max()   # natural order: k = k1 + P k2
+    assert err < 1e-12, err
+    mean = np.mean(np.abs(X) ** 2)
+    assert abs(mean - np.mean(np.abs(ref) ** 2)) < 1e-9 * mean
+    return P, Q, M, X, ref, err
+
+
+def digit_complement_ok():
+    # the kernel's natural-order position of k2 (k2 = d0 + 16 d1 + 256 d2 + 4096 d3, Q = 2^14) is digit-wise, and
+    # Q - 1 - k2 complements every digit: the float4 of (d3 = 2 sel, 2 sel + 1) mirrors onto (d3 = 3 - 2 sel, 2 - 2 sel),
+    # the float4 at sel' = 1 - sel with its halves swapped
+    Q = 1 << 14
+    for k2 in range(0, Q, 4093):
+        d = [k2 & 15, (k2 >> 4) & 15, (k2 >> 8) & 15, k2 >> 12]
+        m = Q - 1 - k2
+        assert [m & 15, (m >> 4) & 15, (m >> 8) & 15, m >> 12] == [15 - d[0], 15 - d[1], 15 - d[2], 3 - d[3]]
+    return True
+
+
+def channel_gather(P, Q, M, X, ref):
+    L = 8 * P
+    B1 = L // 16
+    assert B1 == P // 2 and Q % 8 == 0
+    C = M // L
+    flat = X.reshape(-1)                         # address k1 Q + k2
+    worst = 0.0
+    for ch in range(C):
+        chan = ref[ch * L:(ch + 1) * L]          # natural-order bins of the channel
+        # stage 0 of the DIF transform: butterfly j over d0, inputs at row j + h B1, column 8 ch + c, d0 = 2 c + h
+        stage = np.zeros((16, B1), complex)
+        for j in range(B1):
+            a = np.zeros(16, complex)
+            for h in range(2):
+                for c in range(8):
+                    a[2 * c + h] = flat[(j + h * B1) * Q + 8 * ch + c]
+            assert np.allclose(a, chan[j + B1 * np.arange(16)]), "chunk mapping"
+            y = np.array([np.sum(a * np.exp(2j * np.pi * i * np.arange(16) / 16)) for i in range(16)])
+            stage[:, j] = y * np.exp(2j * np.pi * np.arange(16) * j / L)
+        # the rest of the DIF: a B1-point transform of each output chunk i gives bins i + 16 m
+        out = np.zeros(L, complex)
+        for i in range(16):
+            out[i + 16 * np.arange(B1)] = np.fft.ifft(stage[i]) * B1
+        truth = np.fft.ifft(chan) * L
+        worst = max(worst, np.abs(out - truth).max() / np.abs(truth).max())
+    assert worst < 1e-12, worst
+    return worst
+
+
+def stage0_reads_conflict_free():
+    # P = 2^11: half buffer h holds rows h 1024 .. h 1024 + 1023 as [row][8] complex (64-byte rows, dense TMA boxes).
+    # Thread t reads rows 2t, 2t + 1 (128 contiguous bytes) as eight 16-byte pieces; in iteration q lane t takes piece
+    # q ^ (t & 7). A quarter warp (8 lanes) must touch 8 distinct 16-byte bank groups.
+    NT = 512
+    for q in range(8):
+        for w0 in range(0, NT, 8):
+            groups = {((128 * t + 16 * (q ^ (t & 7))) // 16) % 8 for t in range(w0, w0 + 8)}
+            if len(groups) != 8:
+                return False
+    return True
+
+
+def table_and_zap(P, Q, M):
+    # phase table, channel-contiguous: entry ch L + 8 k1 + c holds bin k1 + P (8 ch + c); zap address of bin k
+    L = 8 * P
+    seen = np.zeros(M, bool)
+    for idx in range(M):
+        ch, r = divmod(idx, L)
+        k1, c = divmod(r, 8)
+        k = k1 + P * (8 * ch + c)
+        assert not seen[k]
+        seen[k] = True
+        assert (k % P) * Q + k // P == k1 * Q + 8 * ch + c   # the spectrum address of that bin
+    return bool(seen.all())
+
+
+def main(argv):
+    logp, logq = (int(argv[1]), int(argv[2])) if len(argv) > 2 else (5, 6)
+    P, Q, M, X, ref, err = sweeps(logp, logq)
+    print(f"P=2^{logp} Q=2^{logq}: sweeps 1 + 2 + split vs rfft, max rel err {err:.2e}")
+    assert digit_complement_ok()
+    gerr = channel_gather(P, Q, M, X, ref)
+    print(f"channel gather + stage 0 vs numpy: max rel err {gerr:.2e}")
+    ok = stage0_reads_conflict_free()
+    print("stage-0 reads conflict free:", ok)
+    assert ok
+    assert table_and_zap(P, Q, M)
+    print("phase table / zap addresses: ok")
+    return 0
+
+
+if __name__ == "__main__":
+    sys.exit(main(sys.argv))
