@@ -39,6 +39,9 @@ struct configs {
   srtb::real baseband_sample_rate = 1000 * 1e6;
   bool baseband_reserve_sample = true;
   srtb::real dm = 0;
+  // trial DMs searched on every block instead of `dm` (new with respect to the reference, whose config.hpp:128-132
+  // leaves a DM search list as a TODO): comma-separated expressions or start:stop:step ranges; empty = search `dm` only
+  std::string dm_list = "";
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

@@ -74,6 +74,25 @@ struct block_config_holder {
   }
 };
 
+/** the host series of stream s's positive boxcars: views into the pinned [streams][MAX_BOXCARS][L] buffer h_series,
+ *  which they keep alive */
+inline std::vector<srtb::work::time_series_holder> positive_series(const srtb_b200_detect_result& res,
+                                                                   const std::shared_ptr<srtb::real>& h_series, int s,
+                                                                   size_t L) {
+  std::vector<srtb::work::time_series_holder> out;
+  srtb::real* base = h_series.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * L;
+  for (int b = 0; b < res.n_boxcars; b++) {
+    if (res.signal_count[b] == 0) continue;
+    srtb::work::time_series_holder h;
+    h.time_series_length = res.series_length[b];
+    h.boxcar_length = res.boxcar_length[b];
+    h.signal_count = res.signal_count[b];
+    h.h_time_series = std::shared_ptr<srtb::real>(h_series, base + (size_t)b * L);
+    out.push_back(h);
+  }
+  return out;
+}
+
 class baseband_chain_pipe {
  protected:
   srtb::cuda_queue q;
@@ -152,16 +171,7 @@ class baseband_chain_pipe {
       w.batch_size = p.C;
       w.zero_count = res[s].zero_count;
       w.ptr = p.d_spectrum[s];
-      srtb::real* base = p.h_series.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L;
-      for (int b = 0; b < res[s].n_boxcars; b++) {
-        if (res[s].signal_count[b] == 0) continue;
-        srtb::work::time_series_holder h;
-        h.time_series_length = res[s].series_length[b];
-        h.boxcar_length = res[s].boxcar_length[b];
-        h.signal_count = res[s].signal_count[b];
-        h.h_time_series = std::shared_ptr<srtb::real>(p.h_series, base + (size_t)b * p.L);
-        w.time_series.push_back(h);
-      }
+      w.time_series = positive_series(res[s], p.h_series, s, p.L);
       out.push_back(std::move(w));
     }
   }

@@ -2,12 +2,14 @@
 // (reference: userspace/include/srtb/pipeline/dedisperse_pipe.hpp:27-48): df = bandwidth / N,
 // f_min = freq_low, f_c = freq_low + bandwidth, all float (SURVEY q7), read from config per call.
 #pragma once
+#include <algorithm>
 #include <optional>
 #include <stop_token>
 
 #include "srtb/config.hpp"
 #include "srtb/cuda_queue.hpp"
 #include "srtb/pipeline/mode.hpp"
+#include "srtb/program_options.hpp"  // parse_dm_list
 #include "srtb/work.hpp"
 
 namespace srtb {
@@ -19,6 +21,22 @@ inline size_t nsamps_reserved() {
       srtb::config.baseband_bandwidth, srtb::config.baseband_sample_rate, srtb::config.dm,
       srtb::config.baseband_reserve_sample ? 1 : 0);
   if (r == 0 && srtb::config.baseband_reserve_sample) srtb::config.baseband_reserve_sample = false;
+  return r;
+}
+
+/** the block overlap the file reader rewinds and the baseband writer trims: nsamps_reserved() without a dm_list, else
+ *  the largest srtb_b200_nsamps_reserved over the trial DMs, so the trial with the largest dispersive smear still sees
+ *  every pulse whole. The maximum is taken of the function itself: the sign of the delay depends on the signs of the DM
+ *  and the bandwidth. Each trial's detector still leaves out only its own reserved tail, so trials with a smaller smear
+ *  search part of the overlap in both blocks. */
+inline size_t nsamps_reserved_max() {
+  if (srtb::config.dm_list.empty()) return nsamps_reserved();
+  const auto& c = srtb::config;
+  size_t r = 0;
+  for (const srtb::real dm : srtb::program_options::parse_dm_list(c.dm_list))
+    r = std::max(r, srtb_b200_nsamps_reserved(c.baseband_input_count, c.spectrum_channel_count, c.baseband_freq_low,
+                                              c.baseband_bandwidth, c.baseband_sample_rate, dm,
+                                              c.baseband_reserve_sample ? 1 : 0));
   return r;
 }
 }  // namespace coherent_dedispersion

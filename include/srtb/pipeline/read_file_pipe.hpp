@@ -64,7 +64,7 @@ class read_file_pipe {
     const bool hit_eof = input_file_stream.eof();
     logical_file_pos += (std::streamoff)time_sample_bytes;
 
-    const size_t nsamps_reserved = srtb::codd::nsamps_reserved();
+    const size_t nsamps_reserved = srtb::codd::nsamps_reserved_max();
     const std::streamoff reserved_bytes =
         (std::streamoff)(nsamps_reserved * static_cast<size_t>(std::abs(srtb::config.baseband_input_bits)) /
                          srtb::BITS_PER_BYTE * streams);

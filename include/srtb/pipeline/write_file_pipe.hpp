@@ -51,9 +51,9 @@ class write_file_pipe {
     auto& out = opt_file_output_stream.value();
     const char* ptr = reinterpret_cast<const char*>(work.baseband_data.baseband_ptr.get());
     const size_t input_bytes = work.baseband_data.baseband_input_bytes;
-    // the last nsamps_reserved() samples come again at the head of the next block
+    // the last nsamps_reserved_max() samples come again at the head of the next block
     const size_t nbytes_reserved =
-        srtb::codd::nsamps_reserved() * static_cast<size_t>(std::abs(srtb::config.baseband_input_bits)) / 8;
+        srtb::codd::nsamps_reserved_max() * static_cast<size_t>(std::abs(srtb::config.baseband_input_bits)) / 8;
     size_t write_bytes = input_bytes;
     if (nbytes_reserved < input_bytes) {
       write_bytes = input_bytes - nbytes_reserved;

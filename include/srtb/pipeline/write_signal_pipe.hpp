@@ -6,6 +6,7 @@
 //   <prefix><counter>.bin            raw baseband block                                (:159-206)
 //   <prefix><counter>.<i>.npy        complex64 dynamic spectrum, shape {batch_size, count} (:209-246)
 //   <prefix><counter>.<boxcar>.tim   float32 time series per detected boxcar           (:249-280)
+// and, for a DM search (dm_list), <prefix><counter>.dm<DM>.<boxcar>.tim and <prefix><counter>.<id>.dm_sweep.csv.
 // counter = udp_packet_counter, or the timestamp when there is none (:145-148).
 // Differences: files are written synchronously on the pipe's thread (the reference posts to thread
 // pools), and the .npy index is incremented until the name is free (the reference's loop never
@@ -13,6 +14,7 @@
 #pragma once
 #include <complex>
 #include <cstdint>
+#include <cstdio>
 #include <deque>
 #include <filesystem>
 #include <fstream>
@@ -108,11 +110,37 @@ class write_signal_pipe {
       } while (std::filesystem::exists(path));
       srtb::io::npy_save(path, h.data(), std::vector<size_t>{w.batch_size, w.count});
     }
+    write_series(w, stem);
+    written_++;
+  }
+
+  /** the host-side files of a kept work: <stem>.<boxcar>.tim per series. A DM search's work (non-empty dm_trials)
+   *  names the DM its series belong to, <stem>.dm<DM>.<boxcar>.tim, and also gets <stem>.<data_stream_id>.dm_sweep.csv,
+   *  one row per trial and boxcar (one row with zero boxcar fields for a trial whose detector was disabled): the S/N
+   *  against DM that tells a dispersed pulse, which peaks at its DM, from RFI, which peaks at DM 0. */
+  static void write_series(const srtb::work::write_signal_work& w, const std::string& stem) {
+    const bool sweep = !w.dm_trials.empty();
+    auto fmt = [](const char* f, double v) {
+      char buf[64];
+      std::snprintf(buf, sizeof buf, f, v);
+      return std::string{buf};
+    };
+    const std::string dm_part = sweep ? ".dm" + fmt("%g", w.dm) : "";
     for (const auto& ts : w.time_series) {
-      std::ofstream f(stem + "." + std::to_string(ts.boxcar_length) + ".tim", std::ios::binary | std::ios::trunc);
+      std::ofstream f(stem + dm_part + "." + std::to_string(ts.boxcar_length) + ".tim", std::ios::binary | std::ios::trunc);
       f.write(reinterpret_cast<const char*>(ts.h_time_series.get()), (std::streamsize)(ts.time_series_length * sizeof(srtb::real)));
     }
-    written_++;
+    if (!sweep) return;
+    std::ofstream f(stem + "." + std::to_string(w.data_stream_id) + ".dm_sweep.csv", std::ios::trunc);
+    f << "dm,detect_enabled,boxcar_length,series_length,signal_count,threshold,peak_snr,peak_index\n";
+    for (const auto& t : w.dm_trials) {
+      const std::string head = fmt("%g", t.dm) + "," + (t.detect_enabled ? "1" : "0") + ",";
+      if (t.boxcars.empty()) f << head << "0,0,0,0,0,0\n";
+      for (const auto& b : t.boxcars)
+        f << head << b.boxcar_length << "," << b.series_length << "," << b.signal_count << ","
+          << fmt("%.9g", b.threshold) << "," << fmt("%.9g", b.peak_snr) << "," << b.peak_index << "\n";
+    }
+    if (!f) SRTB_LOGE << " [write_signal_pipe] " << "cannot write " << stem << ".dm_sweep.csv";
   }
 };
 

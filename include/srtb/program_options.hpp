@@ -177,6 +177,55 @@ inline std::vector<std::string> split_list(const std::string& value, char delimi
   return out;
 }
 
+/** the trial DMs of a dm_list value, in the order given: comma-separated items, each one expression ("2 * 281.025")
+ *  or a range start:stop:step of expressions, which expands to start + i * step for i = 0 .. floor((stop - start) /
+ *  step + 0.5), computed in double from i. An empty list gives no trials; an empty item, a non-finite value, a
+ *  step <= 0 or a stop < start throws std::invalid_argument naming the key. */
+inline std::vector<srtb::real> parse_dm_list(const std::string& value) {
+  std::vector<srtb::real> out;
+  if (trim(value).empty()) return out;
+  auto bad = [&](const std::string& why) -> std::invalid_argument {
+    return std::invalid_argument("[program_options] dm_list = \"" + value + "\": " + why);
+  };
+  auto eval = [&](const std::string& s) {
+    if (trim(s).empty()) throw bad("empty item");
+    double v = 0;
+    try {
+      v = parse(s);
+    } catch (const std::invalid_argument& e) {
+      throw bad(e.what());
+    }
+    if (!std::isfinite(v)) throw bad("\"" + trim(s) + "\" is not finite");
+    return v;
+  };
+  size_t pos = 0;
+  while (true) {
+    const size_t comma = value.find(',', pos);
+    const std::string item = value.substr(pos, comma == std::string::npos ? std::string::npos : comma - pos);
+    if (item.find(':') == std::string::npos) {
+      out.push_back(static_cast<srtb::real>(eval(item)));
+    } else {
+      std::vector<std::string> parts;
+      size_t p = 0;
+      while (true) {
+        const size_t colon = item.find(':', p);
+        parts.push_back(item.substr(p, colon == std::string::npos ? std::string::npos : colon - p));
+        if (colon == std::string::npos) break;
+        p = colon + 1;
+      }
+      if (parts.size() != 3) throw bad("range \"" + trim(item) + "\" is not start:stop:step");
+      const double start = eval(parts[0]), stop = eval(parts[1]), step = eval(parts[2]);
+      if (!(step > 0)) throw bad("range \"" + trim(item) + "\" has step <= 0");
+      if (stop < start) throw bad("range \"" + trim(item) + "\" has stop < start");
+      const double count = std::floor((stop - start) / step + 0.5);
+      for (double i = 0; i <= count; i++) out.push_back(static_cast<srtb::real>(start + i * step));
+    }
+    if (comma == std::string::npos) break;
+    pos = comma + 1;
+  }
+  return out;
+}
+
 /** "key = value" lines, '#' comments; unknown keys are rejected like Boost.Program_options does */
 inline const std::vector<std::string>& known_options() {
   static const std::vector<std::string> names = {
@@ -184,7 +233,7 @@ inline const std::vector<std::string>& known_options() {
       "gui_pixmap_height", "baseband_input_count", "baseband_input_bits", "baseband_format_type",
       "baseband_freq_low", "baseband_bandwidth", "baseband_sample_rate", "baseband_reserve_sample",
       "udp_receiver_address", "udp_receiver_port", "udp_receiver_cpu_preferred", "input_file_path",
-      "input_file_offset_bytes", "baseband_output_file_prefix", "baseband_write_all", "dm",
+      "input_file_offset_bytes", "baseband_output_file_prefix", "baseband_write_all", "dm", "dm_list",
       "dedisperse_measurement", "fft_fftw_wisdom_path", "mitigate_rfi_average_method_threshold",
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length"};
@@ -284,6 +333,12 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(baseband_sample_rate)
   SRTB_PARSE(baseband_reserve_sample)
   SRTB_PARSE(dm)
+  if (name == "dm_list") {
+    const auto trials = parse_dm_list(value);  // rejects a bad list here, before any pipe starts
+    config.dm_list = value;
+    SRTB_LOGI << " [program_options] " << "dm_list = " << value << " (" << trials.size() << " trial(s))";
+    return;
+  }
   if (name == "udp_receiver_address") {
     config.udp_receiver_address.clear();
     for (const auto& sub : split_list(value, ',')) config.udp_receiver_address.push_back(trim(sub));

@@ -180,9 +180,27 @@ struct time_series_holder {
   size_t signal_count = 0;
 };
 
+/** one trial of a DM search on one data stream: its DM, whether the detector ran, and per boxcar what it found */
+struct dm_trial_summary {
+  struct boxcar {
+    size_t boxcar_length = 0;
+    size_t series_length = 0;
+    size_t signal_count = 0;
+    float threshold = 0;
+    float peak_snr = 0;     // largest series value / sqrt(variance)
+    size_t peak_index = 0;  // first index of that value in the series
+  };
+  srtb::real dm = 0;
+  bool detect_enabled = false;
+  std::vector<boxcar> boxcars;
+};
+
 struct write_signal_work : public write_file_work {
   std::vector<time_series_holder> time_series;  // non-empty <=> has_signal
   size_t zero_count = 0;
+  // DM search only (dm_sweep_chain_pipe): the best trial's DM, which ptr and time_series belong to, and every trial
+  srtb::real dm = 0;
+  std::vector<dm_trial_summary> dm_trials;
 };
 
 /** a [batch_size][count] complex dynamic spectrum on the device, to be turned into a waterfall thumbnail

@@ -233,6 +233,34 @@ int srtb_b200_process_block_device(srtb_b200_ctx* ctx, const srtb_b200_block_con
 int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
                                      const void* baseband, size_t baseband_bytes, int on_device,
                                      const float* h_dms, size_t n_dm, srtb_b200_detect_result* h_results);
+/* DM search on one block: the sweep above, which ranks its trials and hands out the best one's candidate.
+ * With outputs == NULL it is srtb_b200_process_block_dm_sweep (same results, same launches). Otherwise:
+ *   - every trial's detector also reduces each boxcar series v (the positive one a .tim file holds) to its peak:
+ *     snr[b] = max_j v[j] / sqrt(variance[b]) (0 when the variance is 0; the detector's rule is v > snr * sqrt(var), so
+ *     this S/N is on the scale of signal_detect_signal_noise_threshold) and peak_index[b] = the smallest j reaching
+ *     the maximum. Boxcars beyond n_boxcars, and trials with detection disabled, keep a zero record;
+ *   - each stream's best trial is chosen among the trials with detect_enabled: those with some signal_count > 0 first,
+ *     then the largest max_b snr[b], then the lowest trial index; trial 0 when no trial has detection enabled;
+ *   - when h_series or d_spectrum is given, the best trial runs once more per stream (one extra trial per stream per
+ *     block) from the stream's kept spectrum: its dynamic spectrum [C][L] lands in d_spectrum[s] and its positive
+ *     series in h_series, exactly as process_block at that DM writes them. The re-run's result header must equal the
+ *     trial's in h_results bit for bit; SRTB_B200_E_CUDA if it does not.
+ * A null pointer among the required arguments, n_dm == 0, a d_spectrum given for some streams but not all, or one
+ * that is not 16-byte aligned returns SRTB_B200_E_INVALID before any launch. Synchronises the context's stream. */
+typedef struct {
+  float snr[SRTB_B200_MAX_BOXCARS];
+  uint64_t peak_index[SRTB_B200_MAX_BOXCARS]; /* index into that boxcar's series */
+} srtb_b200_peak;
+typedef struct {
+  srtb_b200_peak* h_peaks; /* [n_dm][streams], or NULL                                                          */
+  int32_t* h_best_trial;   /* [streams], or NULL                                                                */
+  float* h_series;         /* pinned, [streams][SRTB_B200_MAX_BOXCARS][L], or NULL: the best trial's positive series */
+  float* d_spectrum[4];    /* per stream: N + 2 floats, 16-byte aligned, or all NULL: the best trial's dynamic
+                              spectrum                                                                            */
+} srtb_b200_sweep_outputs;
+int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* baseband,
+                                        size_t baseband_bytes, int on_device, const float* h_dms, size_t n_dm,
+                                        srtb_b200_detect_result* h_results, const srtb_b200_sweep_outputs* outputs);
 /* pipelined ingest (the pinned-host ring of SURVEY section 8e): submit copies the block on a
  * dedicated copy stream while the previous block computes and returns a ticket (>= 0);
  * collect waits for that block and fills h_results[stream] (returns the stream count).
@@ -269,7 +297,8 @@ int srtb_b200_debug_set_submit_count(srtb_b200_ctx* ctx, uint64_t value);
 /* device pointer of stream s's dynamic spectrum after process_block (valid until next call) */
 const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int stream);
 /* test hook: device pointer of the [C][L] dynamic spectrum of the last trial of the last stream of the most recent
-   process_block_dm_sweep (valid until the next call) */
+   process_block_dm_sweep (valid until the next call; after a _ex call that re-ran the best trials into ctx memory, the
+   last stream's best trial) */
 const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx);
 
 /* simplify_spectrum_pipe_2 (pipeline/spectrum_pipe.hpp:82-143): resample_spectrum_3 with norm(),

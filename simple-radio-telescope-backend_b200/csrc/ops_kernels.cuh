@@ -694,6 +694,11 @@ struct detect_dev_result {
   float variance[32];
   float threshold[32];
 };
+// srtb_b200_peak: per boxcar, the largest series value over sqrt(variance) and the first index that reaches it
+struct detect_dev_peak {
+  float snr[32];
+  unsigned long long peak_index[32];
+};
 
 // K14 for long rows (process_block, rows above 2^14): the last waterfall sweep left per-tile (sum |y|^2, sum |y|^4);
 // one thread per channel row folds its tiles in index order and decides (rfi_mitigation.hpp:292-341; NaN -> keep)
@@ -932,11 +937,15 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
 // host_out (optional): pinned host memory [MAX_BOXCARS][row_stride] that receives, straight from this kernel, the
 // series of every boxcar with a positive count — the reference attaches the host copy of a series to the work only
 // when count_signal is positive (signal_detect_pipe.hpp:347-366,405-423); negative blocks cost no PCIe traffic.
+// PEAK (DM sweep): the counting pass also reduces (max v[j], smallest j reaching it) and writes peak->snr[nb] =
+// max / sqrt(variance) (0 when the variance is 0) and peak->peak_index[nb]; the block path launches PEAK = false.
+template <bool PEAK = false>
 __global__ void __launch_bounds__(1024) detect_boxcar_kernel(float* __restrict__ series, size_t row_stride,
                                                              const float* __restrict__ acc,
                                                              size_t ts_count, float snr,
                                                              detect_dev_result* __restrict__ res,
-                                                             float* __restrict__ host_out) {
+                                                             float* __restrict__ host_out,
+                                                             detect_dev_peak* __restrict__ peak = nullptr) {
   __shared__ double smd[32];
   __shared__ float s_thr;
   pdl_launch_dependents();
@@ -975,6 +984,8 @@ __global__ void __launch_bounds__(1024) detect_boxcar_kernel(float* __restrict__
   __syncthreads();
   const float thr = s_thr;
   double cnt = 0.0;
+  float pv = -INFINITY;      // PEAK: this thread's largest value and the smallest index holding it
+  unsigned long long pi = ~0ull;
   for (size_t i = tid; i < n; i += (size_t)8 * nt) {
     float d[8];
 #pragma unroll
@@ -983,11 +994,63 @@ __global__ void __launch_bounds__(1024) detect_boxcar_kernel(float* __restrict__
       d[e] = (j < n) ? v[j] : -INFINITY;
     }
 #pragma unroll
-    for (int e = 0; e < 8; e++)
+    for (int e = 0; e < 8; e++) {
       if (d[e] > thr) cnt += 1.0;
+      if constexpr (PEAK) {
+        // a thread visits its indices in increasing order, so a strict > keeps the first one of a tie
+        const size_t j = i + (size_t)e * nt;
+        if (j < n && (d[e] > pv || pi == ~0ull)) {
+          pv = d[e];
+          pi = j;
+        }
+      }
+    }
   }
   cnt = block_sum<double>(cnt, smd);
   if (tid == 0) res->signal_count[nb] = (unsigned long long)cnt;
+  if constexpr (PEAK) {
+    // (value, index) reduction: larger value wins, equal values take the smaller index; any order gives one answer
+    auto better = [](float av, unsigned long long ai, float bv, unsigned long long bi) {
+      if (bi == ~0ull) return false;
+      if (ai == ~0ull) return true;
+      return bv > av || (bv == av && bi < ai);
+    };
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_down_sync(0xffffffffu, pv, o);
+      const unsigned long long oi = __shfl_down_sync(0xffffffffu, pi, o);
+      if (better(pv, pi, ov, oi)) {
+        pv = ov;
+        pi = oi;
+      }
+    }
+    __shared__ float s_pv[32];
+    __shared__ unsigned long long s_pi[32];
+    const int lane = tid & 31, wid = tid >> 5;
+    if (lane == 0) {
+      s_pv[wid] = pv;
+      s_pi[wid] = pi;
+    }
+    __syncthreads();
+    if (wid == 0) {
+      pv = (lane < (nt + 31) / 32) ? s_pv[lane] : -INFINITY;
+      pi = (lane < (nt + 31) / 32) ? s_pi[lane] : ~0ull;
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_down_sync(0xffffffffu, pv, o);
+        const unsigned long long oi = __shfl_down_sync(0xffffffffu, pi, o);
+        if (better(pv, pi, ov, oi)) {
+          pv = ov;
+          pi = oi;
+        }
+      }
+      if (lane == 0) {
+        const float var = res->variance[nb];
+        peak->snr[nb] = (var > 0.f && pi != ~0ull) ? pv / sqrtf(var) : 0.f;
+        peak->peak_index[nb] = (pi != ~0ull) ? pi : 0ull;
+      }
+    }
+  }
   if (host_out) {
     __shared__ int s_hit;
     if (tid == 0) s_hit = cnt > 0.0 ? 1 : 0;

@@ -109,6 +109,8 @@ struct srtb_b200_ctx {
   bool stat_have[SRTB_B200_STAGE_COUNT] = {};
   // ring path: pinned host destination [streams][MAX_BOXCARS][L] of the current block's positive series (else null)
   float* host_series_dst = nullptr;
+  // DM sweep with outputs: device record of the current (trial, stream) that the detector fills with its peaks (else null)
+  detect_dev_peak* peak_dst = nullptr;
   bool pdl_auto = false;    // programmatic dependent launch for the current block (short kernels only)
   bool res_zeroed = false;  // block path: the per-stream result headers were zeroed before the first kernel
   // process_block
@@ -1571,8 +1573,12 @@ static int detect_tail(srtb_b200_ctx* ctx, int slot, const float2* x, size_t tim
   // one CTA per possible boxcar; CTAs beyond n_boxcars (known only on the device) exit at once
   unsigned max_nb = 1;
   for (size_t b = 2; b <= max_boxcar && b < ts_count && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2) max_nb++;
-  CK(launch_pdl(ctx, detect_boxcar_kernel, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count, (const float*)ctx->lane.acc,
-                ts_count, snr, ctx->d_res + slot, host_series));
+  if (ctx->peak_dst)
+    CK(launch_pdl(ctx, detect_boxcar_kernel<true>, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count,
+                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, ctx->peak_dst));
+  else
+    CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count,
+                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, (detect_dev_peak*)nullptr));
   ctx->launches++;
   CK(cudaGetLastError());
   ctx->slot_time_count[slot] = time_count;
@@ -2264,16 +2270,71 @@ extern "C" int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block
 // ---- DM sweep on one block (BASELINE config #4): unpack + R2C + mean once per stream, then for every
 // trial DM the s1-apply + chirp (out of place, the spectrum is kept), waterfall FFT, SK and detector.
 // Each trial's result equals process_block with cfg->dm = that DM on the same block.
+// With outputs, every trial's detector also writes its peaks, the host picks each stream's best trial, and one more
+// stream_tail per stream at that trial's DM writes its dynamic spectrum and positive series.
+
+// the best trial of stream s: among the trials with detection enabled, those with a positive boxcar first, then the
+// largest peak S/N over the boxcars, then the lowest index; trial 0 when no trial has detection enabled
+static int best_trial(const srtb_b200_detect_result* res, const detect_dev_peak* peaks, size_t n_dm, int streams,
+                      int s) {
+  int best = -1;
+  bool best_positive = false;
+  float best_snr = 0.f;
+  for (size_t j = 0; j < n_dm; j++) {
+    const srtb_b200_detect_result& r = res[j * streams + s];
+    if (!r.detect_enabled) continue;
+    bool positive = false;
+    float snr = -INFINITY;
+    for (int b = 0; b < r.n_boxcars; b++) {
+      positive = positive || r.signal_count[b] > 0;
+      snr = std::max(snr, peaks[j * streams + s].snr[b]);
+    }
+    if (best < 0 || (positive && !best_positive) || (positive == best_positive && snr > best_snr)) {
+      best = (int)j;
+      best_positive = positive;
+      best_snr = snr;
+    }
+  }
+  return best < 0 ? 0 : best;
+}
+
 extern "C" int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
                                                 const void* baseband, size_t baseband_bytes, int on_device,
                                                 const float* h_dms, size_t n_dm,
                                                 srtb_b200_detect_result* h_results /* [n_dm][streams] */) {
+  return srtb_b200_process_block_dm_sweep_ex(ctx, cfg, baseband, baseband_bytes, on_device, h_dms, n_dm, h_results,
+                                             nullptr);
+}
+
+extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
+                                                   const void* baseband, size_t baseband_bytes, int on_device,
+                                                   const float* h_dms, size_t n_dm,
+                                                   srtb_b200_detect_result* h_results /* [n_dm][streams] */,
+                                                   const srtb_b200_sweep_outputs* outputs /* or NULL */) {
   API_LOCK(ctx);
   if (!ctx || !cfg || !baseband || !h_dms || !h_results || n_dm == 0)
     return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: bad argument");
   CK(cudaSetDevice(ctx->device));
   block_params p;
   if (int rc = block_params_for(ctx, cfg, "dm_sweep", &p)) return rc;
+  const bool user_spec = outputs && outputs->d_spectrum[0];
+  if (outputs) {
+    for (int s = 0; s < p.streams; s++) {
+      if (user_spec && !outputs->d_spectrum[s])
+        return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum given for some streams only");
+      if (!user_spec && outputs->d_spectrum[s])
+        return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum given for some streams only");
+      if (user_spec && !aligned16(outputs->d_spectrum[s]))
+        return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum[" + std::to_string(s) + "] is not 16-byte aligned");
+    }
+  }
+  struct sweep_scope {  // detect_tail reads these; they are only meaningful inside this call
+    srtb_b200_ctx* c;
+    ~sweep_scope() {
+      c->peak_dst = nullptr;
+      c->host_series_dst = nullptr;
+    }
+  } sweep_scope_{ctx};
   const void* d_baseband = baseband;
   if (!on_device) {
     if (int rc = ensure(ctx, &ctx->d_baseband, &ctx->d_baseband_bytes, baseband_bytes)) return rc;
@@ -2283,26 +2344,71 @@ extern "C" int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b
   if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, p.N, p.streams)) return rc;
   if (int rc = ensure(ctx, &ctx->sweep_buf, &ctx->sweep_buf_bytes, (p.Nc + 1) * sizeof(float2))) return rc;
   float2* W = static_cast<float2*>(ctx->sweep_buf);
+  // every trial's result header is parked on the device and fetched once at the end: no host sync per trial. With
+  // outputs, the trials' peak records [n_dm][streams] follow the headers in the same allocation, then each stream's
+  // mean(|X|^2), which s1 reads from the lane and the next stream's R2C overwrites
+  const size_t n_rec = n_dm * p.streams;
+  if (int rc = ensure(ctx, &ctx->sweep_res, &ctx->sweep_res_bytes,
+                      n_rec * (sizeof(detect_dev_result) + (outputs ? sizeof(detect_dev_peak) : 0)) +
+                          (outputs ? 4 * sizeof(float) : 0)))
+    return rc;
+  detect_dev_result* d_sweep = static_cast<detect_dev_result*>(ctx->sweep_res);
+  detect_dev_peak* const d_peaks = outputs ? reinterpret_cast<detect_dev_peak*>(d_sweep + n_rec) : nullptr;
+  float* const d_means = outputs ? reinterpret_cast<float*>(d_peaks + n_rec) : nullptr;
+  // zeroed once before the first kernel: a memset between kernels would break the dependent-launch chain
+  if (outputs) CK(cudaMemsetAsync(d_peaks, 0, n_rec * sizeof(detect_dev_peak), ctx->lane.stream));
   block_input in{d_baseband, baseband_bytes, ctx->stream_buf};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
-  // every trial's result header is parked on the device and fetched once at the end: no host sync per trial
-  if (int rc = ensure(ctx, &ctx->sweep_res, &ctx->sweep_res_bytes, n_dm * p.streams * sizeof(detect_dev_result))) return rc;
-  detect_dev_result* d_sweep = static_cast<detect_dev_result*>(ctx->sweep_res);
   for (int s = 0; s < p.streams; s++) {
     if (int rc = r2c_stream(ctx, p, &in, s, /*fork=*/false)) return rc;
+    if (d_means)
+      CK(cudaMemcpyAsync(d_means + s, ctx->lane.mean, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
     float2* buf = reinterpret_cast<float2*>(ctx->stream_buf[s]);
     if (chirp_on_load(p.L))  // the manual zap does not depend on the DM: once, on the kept spectrum
       if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
     for (size_t j = 0; j < n_dm; j++) {
+      if (d_peaks) ctx->peak_dst = d_peaks + j * p.streams + s;
       if (int rc = stream_tail(ctx, p, 0, W, buf, h_dms[j], /*phase_table=*/false)) return rc;
       CK(cudaMemcpyAsync(d_sweep + j * p.streams + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToDevice,
                          ctx->lane.stream));
     }
   }
+  ctx->peak_dst = nullptr;
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
-  CK(cudaMemcpyAsync(h_results, d_sweep, n_dm * p.streams * sizeof(detect_dev_result), cudaMemcpyDeviceToHost,
-                     ctx->lane.stream));
+  static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
+  CK(cudaMemcpyAsync(h_results, d_sweep, n_rec * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
+  if (!outputs) {
+    CK(cudaStreamSynchronize(ctx->lane.stream));
+    return p.streams;
+  }
+  std::vector<detect_dev_peak> own_peaks(outputs->h_peaks ? 0 : n_rec);
+  detect_dev_peak* h_peaks = outputs->h_peaks ? reinterpret_cast<detect_dev_peak*>(outputs->h_peaks) : own_peaks.data();
+  CK(cudaMemcpyAsync(h_peaks, d_peaks, n_rec * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, ctx->lane.stream));
   CK(cudaStreamSynchronize(ctx->lane.stream));
+  int best[4] = {0, 0, 0, 0};
+  for (int s = 0; s < p.streams; s++) {
+    best[s] = best_trial(h_results, h_peaks, n_dm, p.streams, s);
+    if (outputs->h_best_trial) outputs->h_best_trial[s] = best[s];
+  }
+  if (!outputs->h_series && !user_spec) return p.streams;
+  // the best trial once more per stream, from the kept spectrum: its spectrum to d_spectrum[s], its positive series
+  // straight from the detector kernel to h_series' row of the stream, its header to h_res[s]
+  for (int s = 0; s < p.streams; s++) {
+    ctx->host_series_dst = outputs->h_series ? outputs->h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr;
+    float2* dst = user_spec ? reinterpret_cast<float2*>(outputs->d_spectrum[s]) : W;
+    CK(cudaMemcpyAsync(ctx->lane.mean, d_means + s, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
+    if (int rc = stream_tail(ctx, p, 0, dst, reinterpret_cast<float2*>(ctx->stream_buf[s]), h_dms[best[s]],
+                             /*phase_table=*/false))
+      return rc;
+    CK(cudaMemcpyAsync(ctx->h_res + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
+  }
+  ctx->host_series_dst = nullptr;
+  CK(cudaStreamSynchronize(ctx->lane.stream));
+  // same kernels on the same input: the re-run must reproduce the loop's header of that trial bit for bit
+  for (int s = 0; s < p.streams; s++)
+    if (std::memcmp(ctx->h_res + s, h_results + (size_t)best[s] * p.streams + s, sizeof(detect_dev_result)) != 0)
+      return fail(ctx, SRTB_B200_E_CUDA,
+                  "dm_sweep: the best trial's re-run of stream " + std::to_string(s) + " differs from its trial");
   return p.streams;
 }
 

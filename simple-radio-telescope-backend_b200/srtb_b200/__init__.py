@@ -71,6 +71,17 @@ class BlockOutputs(C.Structure):
     _fields_ = [("d_spectrum", C.c_void_p * 4), ("h_series", C.c_void_p)]
 
 
+class Peak(C.Structure):
+    """srtb_b200_peak: per boxcar, the series' peak S/N and the first index of its maximum"""
+    _fields_ = [("snr", C.c_float * MAX_BOXCARS), ("peak_index", C.c_uint64 * MAX_BOXCARS)]
+
+
+class SweepOutputs(C.Structure):
+    """srtb_b200_sweep_outputs: what a DM sweep hands out besides its result headers (members may be NULL)"""
+    _fields_ = [("h_peaks", C.c_void_p), ("h_best_trial", C.c_void_p), ("h_series", C.c_void_p),
+                ("d_spectrum", C.c_void_p * 4)]
+
+
 class SrtbError(RuntimeError):
     def __init__(self, code: int, message: str):
         super().__init__(f"srtb_b200 error {code}: {message}")
@@ -114,6 +125,8 @@ SYMBOLS = {
     "srtb_b200_process_block_device": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ, C.POINTER(DetectResult), _P, _I]),
     "srtb_b200_process_block_dm_sweep": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ, _I, C.POINTER(_F), _SZ,
                                               C.POINTER(DetectResult)]),
+    "srtb_b200_process_block_dm_sweep_ex": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ, _I, C.POINTER(_F), _SZ,
+                                                 C.POINTER(DetectResult), C.POINTER(SweepOutputs)]),
     "srtb_b200_submit_block": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ]),
     "srtb_b200_submit_block_device": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ]),
     "srtb_b200_collect_block": (_I, [_P, _I, C.POINTER(DetectResult)]),
@@ -268,14 +281,47 @@ class Context:
         n = self._ck(fn(self.h, C.byref(cfg), _ptr(baseband), nbytes, res, _ptr(h_series), int(copy_all)))
         return [res[i] for i in range(n)]
 
-    def process_block_dm_sweep(self, cfg: BlockConfig, baseband, nbytes: int, dms, on_device: bool = False):
-        """one block, many trial DMs: returns results[dm_index][stream]"""
+    def process_block_dm_sweep(self, cfg: BlockConfig, baseband, nbytes: int, dms, on_device: bool = False,
+                               outputs: bool = False, h_series=None, d_spectrum=None):
+        """one block, many trial DMs: returns results[dm_index][stream].
+        outputs=True: returns (results, peaks, best_trial, h_series, d_spectrum) instead, where peaks = (snr, index),
+        numpy arrays [n_dm][streams][n_boxcars] (n_boxcars = the most any trial used), best_trial = [streams] ints,
+        h_series = pinned [streams][MAX_BOXCARS][L] float32 tensor holding the best trials' positive series and
+        d_spectrum = per-stream device tensors of N + 2 float32 holding the best trials' dynamic spectra. The caller may
+        pass h_series and d_spectrum in (the same shapes); they are allocated otherwise."""
         n_dm = len(dms)
         arr = (C.c_float * n_dm)(*[float(d) for d in dms])
         res = (DetectResult * (4 * n_dm))()
-        streams = self._ck(self.lib.srtb_b200_process_block_dm_sweep(self.h, C.byref(cfg), _ptr(baseband), nbytes,
-                                                                      int(on_device), arr, n_dm, res))
-        return [[res[j * streams + s] for s in range(streams)] for j in range(n_dm)]
+        if not outputs:
+            streams = self._ck(self.lib.srtb_b200_process_block_dm_sweep(self.h, C.byref(cfg), _ptr(baseband), nbytes,
+                                                                          int(on_device), arr, n_dm, res))
+            return [[res[j * streams + s] for s in range(streams)] for j in range(n_dm)]
+        import numpy as np
+        import torch
+        streams = FORMAT_STREAMS[cfg.baseband_format]
+        n = cfg.baseband_input_count
+        L = n // 2 // min(cfg.spectrum_channel_count, n // 2)
+        if h_series is None:
+            h_series = torch.zeros((streams, MAX_BOXCARS, L), dtype=torch.float32).pin_memory()
+        if d_spectrum is None:
+            d_spectrum = [torch.empty(n + 2, dtype=torch.float32, device=f"cuda:{self.device}") for _ in range(streams)]
+        peaks = (Peak * (4 * n_dm))()
+        best = (C.c_int32 * 4)()
+        out = SweepOutputs()
+        out.h_peaks = C.cast(peaks, C.c_void_p)
+        out.h_best_trial = C.cast(best, C.c_void_p)
+        out.h_series = _ptr(h_series)
+        for i, t in enumerate(d_spectrum):
+            out.d_spectrum[i] = _ptr(t)
+        streams = self._ck(self.lib.srtb_b200_process_block_dm_sweep_ex(
+            self.h, C.byref(cfg), _ptr(baseband), nbytes, int(on_device), arr, n_dm, res, C.byref(out)))
+        results = [[res[j * streams + s] for s in range(streams)] for j in range(n_dm)]
+        nb = max([r.n_boxcars for row in results for r in row] + [0])
+        snr = np.array([[list(peaks[j * streams + s].snr)[:nb] for s in range(streams)] for j in range(n_dm)],
+                       np.float32).reshape(n_dm, streams, nb)
+        idx = np.array([[list(peaks[j * streams + s].peak_index)[:nb] for s in range(streams)] for j in range(n_dm)],
+                       np.uint64).reshape(n_dm, streams, nb)
+        return results, (snr, idx), [int(best[s]) for s in range(streams)], h_series, list(d_spectrum)
 
     def submit_block(self, cfg: BlockConfig, h_baseband, nbytes: int) -> int:
         """pipelined ingest: H2D on the copy stream overlaps the previous block's compute"""

@@ -18,6 +18,10 @@
 //                           R samples/s per receiver like a NIC would (0 = as fast as it is taken); with
 //   --synthetic_duration S  seconds of stream (default 10); prints one JSON line with blocks, rate and lost packets
 //   --discard_output 1      count results instead of writing candidate files
+// With dm_list set (a srtb::configs key: --dm_list "0:100:5" or a .cfg line), every block is searched over those trial
+// DMs by dm_sweep_chain_pipe instead of baseband_chain_pipe at `dm` (which is then not used); its pipes run without a
+// ring, so --ring_depth is ignored. The sink then writes the best trial's files and a per-stream S/N-versus-DM table.
+#include <algorithm>
 #include <atomic>
 #include <chrono>
 #include <csignal>
@@ -33,6 +37,7 @@
 #include "srtb/io/udp_block_assembler.hpp"
 #include "srtb/memory.hpp"
 #include "srtb/pipeline/baseband_chain_pipe.hpp"
+#include "srtb/pipeline/dm_sweep_chain_pipe.hpp"
 #include "srtb/pipeline/framework/pipe.hpp"
 #include "srtb/pipeline/framework/pipe_io.hpp"
 #include "srtb/pipeline/read_file_pipe.hpp"
@@ -207,8 +212,24 @@ int main(int argc, char** argv) {
   } else {
     for (const auto& s : srtb::program_options::split_list(devices_opt, ',')) devices.push_back(std::atoi(s.c_str()));
   }
-  SRTB_LOGI << " [main] " << devices.size() << " GPU(s), " << chains_per_gpu << " chain pipe(s) each, ring depth "
-            << ring_depth;
+  const std::vector<srtb::real> dm_trials = srtb::program_options::parse_dm_list(cfg.dm_list);
+  const bool dm_sweep = !dm_trials.empty();
+  if (dm_sweep) {
+    SRTB_LOGI << " [main] " << "DM search: " << dm_trials.size() << " trial DM(s) from "
+              << *std::min_element(dm_trials.begin(), dm_trials.end()) << " to "
+              << *std::max_element(dm_trials.begin(), dm_trials.end()) << "; dm = " << cfg.dm << " is not used";
+    SRTB_LOGI << " [main] " << devices.size() << " GPU(s), " << chains_per_gpu
+              << " DM-sweep pipe(s) each; --ring_depth is ignored (no ring in a DM sweep)";
+  } else {
+    SRTB_LOGI << " [main] " << devices.size() << " GPU(s), " << chains_per_gpu << " chain pipe(s) each, ring depth "
+              << ring_depth;
+  }
+  // the device chain between source and sink: one DM, or the trial DMs of dm_list
+  auto start_chain = [&](auto in, auto out, int dev) {
+    if (dm_sweep) return start_pipe<dm_sweep_chain_pipe>(in, out, srtb::cuda_queue{dev});
+    return start_pipe<baseband_chain_pipe>(in, out, srtb::cuda_queue{dev}, false, ring_depth);
+  };
+  const int blocks_in_flight = dm_sweep ? 1 : ring_depth;
 
   auto submitted = std::make_shared<std::atomic<uint64_t>>(0);
   auto done = std::make_shared<std::atomic<uint64_t>>(0);
@@ -232,18 +253,17 @@ int main(int argc, char** argv) {
       // that block's side-branch decision has been made
       auto thumb_q = std::make_shared<thumbnail_out_functor::queue>(srtb::work_queue_capacity);
       for (int c = 0; c < chains_per_gpu; c++)
-        threads.push_back(start_pipe<baseband_chain_pipe>(
+        threads.push_back(start_chain(
             idle_queue_in_functor{gpu_queues.back()},
             multiple_works_out_functor{multiple_out_functors_functor{
                 thumbnail_out_functor{thumb_q, thumbnails_open, thumbnails_accepted, thumbnails_dropped}, queue_out_functor{out_q}}},
-            srtb::cuda_queue{dev}, false, ring_depth));
+            dev));
       threads.push_back(start_pipe<simplify_spectrum_pipe_2>(queue_in_functor{thumb_q}, queue_out_functor{draw_q},
                                                              srtb::cuda_queue{dev}));
     } else {
       for (int c = 0; c < chains_per_gpu; c++)
-        threads.push_back(start_pipe<baseband_chain_pipe>(idle_queue_in_functor{gpu_queues.back()},
-                                                          multiple_works_out_functor{queue_out_functor{out_q}},
-                                                          srtb::cuda_queue{dev}, false, ring_depth));
+        threads.push_back(start_chain(idle_queue_in_functor{gpu_queues.back()},
+                                      multiple_works_out_functor{queue_out_functor{out_q}}, dev));
     }
   }
   if (cfg.gui_enable)
@@ -275,7 +295,7 @@ int main(int argc, char** argv) {
     auto h_zero = srtb::host_allocator.allocate_shared<std::byte>(block_bytes);
     std::memset(h_zero.get(), 0, block_bytes);
     uint64_t pushed = 0;
-    for (int round = 0; round < chains_per_gpu * (ring_depth + 1); round++)
+    for (int round = 0; round < chains_per_gpu * (blocks_in_flight + 1); round++)
       for (auto& gq : gpu_queues) {
         srtb::work::copy_to_device_work w;
         w.ptr = nullptr;

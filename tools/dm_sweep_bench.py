@@ -1,8 +1,11 @@
 #!/usr/bin/env python
 """BASELINE config #4 shape: one 2^27-sample 8-bit block swept over 21 trial DMs (0..1000, step 50) with
 srtb_b200_process_block_dm_sweep (unpack + R2C once, then per DM: s1 + chirp + waterfall FFT + SK + detect).
-Prints one JSON line: blocks/s, trial-Gsamples/s (samples x trials / time) and ms per trial."""
+Prints one JSON line: blocks/s, trial-Gsamples/s (samples x trials / time) and ms per trial.
+--outputs: time the plain entry and srtb_b200_process_block_dm_sweep_ex with every output (peaks, best trial, the best
+trial's series and spectrum) alternating in one run, and print both, their ratio and the card with its power limit."""
 import json
+import subprocess
 import sys
 import time
 from pathlib import Path
@@ -16,8 +19,10 @@ sys.path.insert(0, str(ROOT / "simple-radio-telescope-backend_b200"))
 import bench  # noqa: E402
 import srtb_b200  # noqa: E402
 
-log2n = int(sys.argv[1]) if len(sys.argv) > 1 else 27
-reps = int(sys.argv[2]) if len(sys.argv) > 2 else 5
+args = [a for a in sys.argv[1:] if a != "--outputs"]
+with_outputs = "--outputs" in sys.argv[1:]
+log2n = int(args[0]) if len(args) > 0 else 27
+reps = int(args[1]) if len(args) > 1 else 5
 n = 1 << log2n
 dms = [50.0 * i for i in range(21)]
 torch.cuda.set_device(0)
@@ -32,6 +37,29 @@ cfg.signal_detect_max_boxcar_length = 256
 blk = torch.from_numpy(bench.synth_block(n, 1, 4).view(np.uint8)).cuda()
 ctx.process_block_dm_sweep(cfg, blk, n, dms, on_device=True)
 torch.cuda.synchronize()
+if with_outputs:
+    # both entries are synchronous: a host clock around each call times it whole
+    L = n // 2 // cfg.spectrum_channel_count
+    h_series = torch.zeros((1, srtb_b200.MAX_BOXCARS, L), dtype=torch.float32).pin_memory()
+    d_spec = [torch.empty(n + 2, dtype=torch.float32, device="cuda")]
+    ctx.process_block_dm_sweep(cfg, blk, n, dms, on_device=True, outputs=True, h_series=h_series, d_spectrum=d_spec)
+    plain, ex = [], []
+    for _ in range(reps):
+        t0 = time.perf_counter()
+        ctx.process_block_dm_sweep(cfg, blk, n, dms, on_device=True)
+        plain.append(time.perf_counter() - t0)
+        t0 = time.perf_counter()
+        ctx.process_block_dm_sweep(cfg, blk, n, dms, on_device=True, outputs=True, h_series=h_series,
+                                   d_spectrum=d_spec)
+        ex.append(time.perf_counter() - t0)
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader", "-i", "0"],
+                          capture_output=True, text=True).stdout.strip()
+    p_ms, e_ms = 1e3 * float(np.median(plain)), 1e3 * float(np.median(ex))
+    print(json.dumps({"workload": f"config4 shape: 2^{log2n} samples x {len(dms)} trial DMs", "reps": reps,
+                      "plain_ms_per_block": p_ms, "outputs_ms_per_block": e_ms, "outputs_over_plain": e_ms / p_ms,
+                      "one_trial_share": 1.0 / len(dms), "plain_ms_all": [1e3 * t for t in plain],
+                      "outputs_ms_all": [1e3 * t for t in ex], "card": card}))
+    sys.exit(0)
 t0 = time.perf_counter()
 for _ in range(reps):
     res = ctx.process_block_dm_sweep(cfg, blk, n, dms, on_device=True)
