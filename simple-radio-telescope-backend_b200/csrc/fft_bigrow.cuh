@@ -51,6 +51,10 @@ struct bigrow {
   static constexpr size_t off_mbar = off_tab + (size_t)TABN * sizeof(float2);
   static constexpr size_t off_red = off_mbar + 24 * 8;   // 3 buffers x 8 chunk barriers
   static constexpr size_t bytes = off_red + 4 * 32 * sizeof(float);
+  // the sweep-order load (SRC = 1) lands 128-byte-swizzled tensor boxes, whose destinations must be 1024-byte aligned:
+  // half buffers rounded up to 1 KiB, and 1 KiB more to align the base of the dynamic shared memory
+  static constexpr int HALF_SW = (HALF + 127) / 128 * 128;
+  static constexpr size_t bytes_sw = bytes + 3 * (size_t)(HALF_SW - HALF) * sizeof(float2) + 1024;
 };
 
 // ---- column-sum cells in global memory, kept in L2 across the rows a CTA adds into them
@@ -147,14 +151,15 @@ __device__ __forceinline__ void bigrow_stage_table(float2* __restrict__ p, const
 //   4 = two and two, 2 = a correctly rounded reciprocal for every bin (widely spaced bins of short test blocks)
 // SRC: where the rows come from and what is stored.
 //   0 = rows of `in` (natural order), natural-order rows to `out`;
-//   1 = channel `row` of a spectrum left in sweep order by SRC = 2 (bin k = k1 + P k2 at k1 L + k2, P = L / 8): the
-//       box of all P rows k1 by the 8 columns k2 = 8 row .. 8 row + 7, fetched through `tmap` as 8 boxes of 256 rows x
-//       8 elements (dense 64-byte rows, one mbarrier each). Chunk d0 of the channel is column d0 >> 1, rows from
-//       (P / 2) (d0 & 1): buffer A holds rows k1 < P / 2, buffer B the rest, and stage 0 gathers butterfly j from rows
-//       j and j + P / 2 before it stores the standard layout (tools/proto_r2c_sweep_order.py);
-//   2 = the R2C row sweep, run as clusters of two CTAs: nrows = P rows of the in-place scratch, the cluster's CTAs
-//       take rows i and P - i (cluster 0: rows 0 and P / 2, each its own mirror), transform them forward and store
-//       the split spectrum X[k1 + P k2] in place, reading the mirror row's Z through distributed shared memory.
+//   1 = channel `row` of a spectrum left channel-blocked by SRC = 2 (bin k = k1 + P k2 at (k2 >> 3) L + 8 k1 + (k2 & 7),
+//       P = L / 8): one contiguous range of L elements laid out [k1][k2 & 7], fetched through `tmap` as 8 boxes of 128
+//       lines x 128 bytes (a quarter of a half buffer each, one mbarrier each), 128-byte swizzled: 16-byte piece q of
+//       line t lands at piece q ^ (t & 7). Chunk d0 of the channel is column d0 >> 1, rows from (P / 2) (d0 & 1):
+//       buffer A holds rows k1 < P / 2, buffer B the rest, and stage 0 gathers butterfly j from rows j and j + P / 2
+//       before it stores the standard layout (tools/proto_r2c_sweep_order.py);
+//   2 = the R2C row sweep, run as clusters of two CTAs: nrows = P rows of the scratch `in`, the cluster's CTAs take
+//       rows i and P - i (cluster 0: rows 0 and P / 2, each its own mirror), transform them forward and store the split
+//       spectrum X[k1 + P k2] channel-blocked to `out`, reading the mirror row's Z through distributed shared memory.
 // The body is shared by three entry points: fft_bigrow_kernel (SRC = 0) and the two kernels of the sweep-order R2C
 // route below it.
 template <int LOGL, bool FWD, bool SK, int CHIRP, int SRC>
@@ -166,15 +171,31 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
                 "sweep-order routes: rows of 2^14");
   using C = bigrow<LOGL>;
   constexpr int L = C::L, R3 = C::R3, B1 = C::B1, B2 = C::B2, S1 = C::S1, S2 = C::S2, NT = C::NT, NW = C::NW;
-  constexpr int HALF = C::HALF;
+  constexpr int HALF = (SRC == 1) ? C::HALF_SW : C::HALF;  // stride of the half buffers, elements
+  constexpr size_t off_tab = 3 * (size_t)HALF * sizeof(float2);
+  constexpr size_t off_mbar = off_tab + (size_t)C::TABN * sizeof(float2);
+  constexpr size_t off_red = off_mbar + 24 * 8;
   extern __shared__ __align__(128) unsigned char smraw[];
-  float2* const hbuf = reinterpret_cast<float2*>(smraw);  // three half-row buffers
-  float2* const T0 = reinterpret_cast<float2*>(smraw + C::off_tab);
+  unsigned char* const sm = (SRC == 1) ? smraw + ((0u - smem_u32(smraw)) & 1023u) : smraw;
+  float2* const hbuf = reinterpret_cast<float2*>(sm);  // three half-row buffers
+  float2* const T0 = reinterpret_cast<float2*>(sm + off_tab);
   float2* const T1 = T0 + B1;
   float2* const T2 = T1 + 15 * B2;
-  uint64_t* const mbar = reinterpret_cast<uint64_t*>(smraw + C::off_mbar);  // [3 buffers][8 chunks]
-  float* const red = reinterpret_cast<float*>(smraw + C::off_red);  // [2 slots][s2 | s4][32]
+  uint64_t* const mbar = reinterpret_cast<uint64_t*>(sm + off_mbar);  // [3 buffers][8 chunks]
+  float* const red = reinterpret_cast<float*>(sm + off_red);  // [2 slots][s2 | s4][32]
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  // SRC = 2: the per-row addresses of stage 2, of the last stage and of the split come from a thread index read afresh
+  // (volatile), so they cost a few integer operations per row instead of registers kept live through the butterflies
+  // (a spill)
+  auto tid_row = [&]() -> int {
+    if constexpr (SRC == 2) {
+      unsigned t;
+      asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
+      return (int)t;
+    } else {
+      return tid;
+    }
+  };
 
   for (int i = tid; i < C::TABN; i += NT) T0[i] = __ldg(&tabs[i]);
   if (tid < 24) mbar_init(&mbar[tid], 1);
@@ -194,9 +215,9 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
   auto issue_half = [&](unsigned row, int which, int hb) {
     fence_proxy_async();
     if constexpr (SRC == 1) {
-      if (lane < 4) {  // rows (P / 2) which + 256 lane .. + 255, columns 8 row .. 8 row + 7
+      if (lane < 4) {  // rows k1 = (P / 2) which + 256 lane .. + 255 of channel `row`: 128 lines of 128 bytes
         mbar_expect_tx(&mbar[hb * 8 + lane], (uint32_t)(256 * 8 * sizeof(float2)));
-        tma_load_2d(hbuf + hb * HALF + lane * 2048, tmap, (int)(8 * row), which * (L / 16) + 256 * lane,
+        tma_load_2d(hbuf + hb * HALF + lane * 2048, tmap, 0, (int)(row * (L / 16) + (L / 32) * which + 128 * lane),
                     &mbar[hb * 8 + lane]);
       }
     } else if (lane < 8) {
@@ -270,40 +291,23 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
       float2* const pb = bufB + j;
       float2 a[16], b[16];
       if constexpr (SRC == 1) {
-        // rows j, j + 1 of each half are 128 contiguous bytes: eight 16-byte pieces (columns 2 (p & 3), 2 (p & 3) + 1
-        // of row j + (p >> 2)), read in the lane-rotated order p = q ^ (tid & 7) so that a quarter warp touches eight
-        // distinct bank groups, s1 + chirp applied in that order (the phases of piece p are the p-th pair of the
-        // row pair's 16 table entries), then put back in order by three conditional swaps
+        // rows j, j + 1 of each half are line tid, 128 contiguous bytes: eight 16-byte pieces (columns 2 (p & 3),
+        // 2 (p & 3) + 1 of row j + (p >> 2)). The swizzled load left piece p at p ^ (tid & 7), so a quarter warp reading
+        // piece p touches eight distinct bank groups; the phases of piece p are the p-th pair of the row pair's 16
+        // table entries
         const int rot = tid & 7, box = tid >> 7;
         const float2* const ph = reinterpret_cast<const float2*>(cp.phase + (size_t)row * L + 8 * j);
 #pragma unroll
         for (int h = 0; h < 2; h++) {
           mbar_wait(&mbar[(h ? hB : hA) * 8 + box], h ? parB : parA);
           const float4* const src = reinterpret_cast<const float4*>((h ? bufB : bufA) + 8 * j);
-          float4 v[8];
-#pragma unroll
-          for (int q = 0; q < 8; q++) {
-            const float2 g = __ldg(ph + (size_t)h * (L / 16) * 4 + (q ^ rot));
-            const float4 x = src[q ^ rot];
-            const float2 y0 = chirp_point_tab(make_float2(x.x, x.y), g.x, limit, cp.coef);
-            const float2 y1 = chirp_point_tab(make_float2(x.z, x.w), g.y, limit, cp.coef);
-            v[q] = make_float4(y0.x, y0.y, y1.x, y1.y);
-          }
-#pragma unroll
-          for (int bit = 1; bit < 8; bit <<= 1) {
-            const bool sw = (rot & bit) != 0;
-#pragma unroll
-            for (int p = 0; p < 8; p++)
-              if (!(p & bit)) {
-                const float4 x0 = v[p], x1 = v[p | bit];
-                v[p] = sw ? x1 : x0;
-                v[p | bit] = sw ? x0 : x1;
-              }
-          }
 #pragma unroll
           for (int p = 0; p < 8; p++) {
+            const float2 g = __ldg(ph + (size_t)h * (L / 16) * 4 + p);
+            const float4 x = src[p ^ rot];
             const int c = 2 * (p & 3);  // columns c, c + 1 -> d0 = 2 c + h, 2 c + 2 + h
-            const float2 y0 = make_float2(v[p].x, v[p].y), y1 = make_float2(v[p].z, v[p].w);
+            const float2 y0 = chirp_point_tab(make_float2(x.x, x.y), g.x, limit, cp.coef);
+            const float2 y1 = chirp_point_tab(make_float2(x.z, x.w), g.y, limit, cp.coef);
             if (p < 4) {
               a[2 * c + h] = y0;
               a[2 * c + 2 + h] = y1;
@@ -313,6 +317,9 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
             }
           }
         }
+        // every thread has gathered its rows before the layout is rewritten; the barrier comes before the butterflies
+        // so that their stores can follow the twiddles one by one (after them, all 64 results would be live at once)
+        __syncthreads();
       } else if constexpr (CHIRP == 5) {
         // tabulated phases (two adjacent bins per 8-byte load, prefetched into L2 while the previous row was stored):
         // s1 + chirp applied as the pairs are taken out of shared memory, no pass of its own and no fp64
@@ -380,7 +387,6 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
       const float4 w = *reinterpret_cast<const float4*>(T0 + j);
       bigrow_twiddle_powers(a, make_float2(w.x, w.y));
       bigrow_twiddle_powers(b, make_float2(w.z, w.w));
-      if constexpr (SRC == 1) __syncthreads();  // every thread has gathered its rows before the layout is rewritten
 #pragma unroll
       for (int i = 0; i < 16; i++)
         *reinterpret_cast<float4*>((i < 8 ? pa : pb) + (i & 7) * S1) = make_float4(a[i].x, a[i].y, b[i].x, b[i].y);
@@ -394,17 +400,19 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
     __syncthreads();
     // ---- stage 2: block (d0, d1), butterflies over d2 (stride R3), pair of [0, R3); lanes vary d0
     {
-      const int d0 = tid & 15, rest = tid >> 4, jp = rest % (R3 / 2), d1 = rest / (R3 / 2);
+      const int t = tid_row();
+      const int d0 = t & 15, rest = t >> 4, jp = rest % (R3 / 2), d1 = rest / (R3 / 2);
       bigrow_stage_table<FWD, R3, R3>(half_of(d0) + d1 * S2 + 2 * jp, T2 + 2 * jp);
     }
     __syncthreads();
     // ---- last stage, pass 1: radix R3 on R3 contiguous elements, in place; row statistics for SK
     float s2 = 0.f, s4 = 0.f;
     if constexpr (R3 == 4) {
+      const int t = tid_row();
 #pragma unroll
       for (int g = 0; g < 8; g++) {
-        const int rest = (tid >> 4) + (NT / 16) * g;  // lanes vary d0; (d1, d2) = rest
-        float2* const p = half_of(tid & 15) + (rest >> 4) * S2 + (rest & 15) * 4;
+        const int rest = (t >> 4) + (NT / 16) * g;  // lanes vary d0; (d1, d2) = rest
+        float2* const p = half_of(t & 15) + (rest >> 4) * S2 + (rest & 15) * 4;
         const float4 q0 = *reinterpret_cast<const float4*>(p), q1 = *reinterpret_cast<const float4*>(p + 2);
         float2 x0 = make_float2(q0.x, q0.y), x1 = make_float2(q0.z, q0.w);
         float2 x2 = make_float2(q1.x, q1.y), x3 = make_float2(q1.z, q1.w);
@@ -468,8 +476,9 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
     }
     if (live(it + 1)) prefetch_phase(row_of(it + 1));
     if constexpr (SRC == 2) {
-      // ---- R2C split and natural-order store of row k1 = row: X[k1 + P k2] from Z[k1][k2] and the mirror Z[M - k],
+      // ---- R2C split and channel-blocked store of row k1 = row: X[k1 + P k2] from Z[k1][k2] and the mirror Z[M - k],
       // which the partner CTA holds (itself for rows 0 and P / 2). Lanes as in pass 2 below.
+      const int t = tid_row(), lane = t & 31, wid = t >> 5;
       const int pd0 = lane & 15, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
       const float2* const base = half_of(pd0) + pd1 * S2 + 2 * sel;
       const unsigned prank = (row == 0 || 2 * row == nrows) ? crank : (crank ^ 1);
@@ -487,7 +496,13 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
       auto pos = [&](int k) {  // shared-memory position of natural-order k2 (pass 2's digit map)
         return half_of(k & 15) + ((k >> 4) & 15) * S2 + ((k >> 8) & 15) * R3 + (k >> 12);
       };
-      float2* const o = out + (size_t)row * L + kb;
+      // X[k1 + P k2] goes to (k2 >> 3) L + 8 k1 + (k2 & 7): channel k2 >> 3 (L = 8 P bins) is one contiguous range,
+      // the order of the phase table and of the waterfall kernel's load. Lanes 2m and 2m + 1 hold k2 and k2 + 1 (kb even
+      // and odd): they trade halves, and each stores a 16-byte pair, the even lane at d3 = 2 sel, the odd one at
+      // d3 = 2 sel + 1. A warp's store covers eight 64-byte pieces; rows 2m and 2m + 1 fill the two halves of each line.
+      const unsigned odd = lane & 1;
+      const int ks = kb + (int)odd * 4095;  // k2 of the pair's first element (i2 = 0)
+      float2* const o = out + (size_t)(ks >> 3) * L + 8 * (size_t)row + (ks & 7);
       float ps = 0.f;
 #pragma unroll 4
       for (int i2 = 0; i2 < 16; i2++) {
@@ -506,8 +521,10 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
         const float2 w1 = c_mul(w0, make_float2(0.70710678118654752440f, -0.70710678118654752440f));  // k2 + L / 4
         const float2 x0 = r2c_split_point(make_float2(q.x, q.y), m0, w0);
         const float2 x1 = r2c_split_point(make_float2(q.z, q.w), m1, w1);
-        o[256 * i2] = x0;
-        o[256 * i2 + 4096] = x1;
+        const float2 mine = odd ? x0 : x1;
+        const float2 theirs = make_float2(__shfl_xor_sync(0xffffffffu, mine.x, 1), __shfl_xor_sync(0xffffffffu, mine.y, 1));
+        *reinterpret_cast<float4*>(o + (size_t)i2 * (32 * L)) =
+            odd ? make_float4(theirs.x, theirs.y, x1.x, x1.y) : make_float4(x0.x, x0.y, theirs.x, theirs.y);
         ps += (x0.x * x0.x + x0.y * x0.y) + (x1.x * x1.x + x1.y * x1.y);
       }
       psum += (double)ps;
@@ -588,13 +605,14 @@ __global__ void __launch_bounds__(bigrow<LOGL>::NT, bigrow<LOGL>::CTAS)
 }
 
 // the sweep-order R2C route of 2^25-point blocks with rows of 2^14 (srtb_b200.cu, r2c_sweep_order): the paired row
-// sweep with the split (clusters of two CTAs, in place on the [P][L] scratch) ...
+// sweep with the split (clusters of two CTAs, from the [P][L] scratch z to the channel-blocked spectrum) ...
 __global__ void __launch_bounds__(bigrow<14>::NT, 1)
-    r2c_rows_split_kernel(float2* __restrict__ z, unsigned nrows, const float2* __restrict__ tabs, r2c_rows_params rr) {
-  bigrow_body<14, true, false, 0, 2>(z, z, nrows, tabs, row_sk_params{}, row_chirp_params{}, nullptr, rr);
+    r2c_rows_split_kernel(const float2* __restrict__ z, float2* __restrict__ out, unsigned nrows,
+                          const float2* __restrict__ tabs, r2c_rows_params rr) {
+  bigrow_body<14, true, false, 0, 2>(z, out, nrows, tabs, row_sk_params{}, row_chirp_params{}, nullptr, rr);
 }
 
-// ... and the whole-row waterfall kernel reading channel `row` of that spectrum through a tensor map
+// ... and the whole-row waterfall kernel reading channel `row` of that spectrum through a swizzling tensor map
 __global__ void __launch_bounds__(bigrow<14>::NT, 1)
     waterfall_sweep_order_kernel(const float2* __restrict__ in, float2* __restrict__ out, unsigned nrows,
                                  const float2* __restrict__ tabs, row_sk_params skp, row_chirp_params cp,

@@ -544,7 +544,8 @@ __global__ void __launch_bounds__(256) rfi_s1_apply_kernel(float2* __restrict__ 
 }
 
 // K11 manual zap (S/spectrum/rfi_mitigation.hpp:137-143): blockIdx.y = range
-// logp != 0: the spectrum is in sweep order, bin k at (k mod 2^logp) 2^logq + k / 2^logp
+// logp != 0: the spectrum is channel-blocked (r2c_rows_split_kernel): bin k = k1 + 2^logp k2 at
+// (k2 >> 3) 2^logq + 8 k1 + (k2 & 7), channels of 2^logq = 8 2^logp bins
 struct bin_ranges {
   unsigned long long lo[16], hi[16];
   unsigned logp, logq;
@@ -555,8 +556,10 @@ __global__ void __launch_bounds__(256) rfi_zero_ranges_kernel(float2* __restrict
   const size_t lo = r.lo[blockIdx.y], hi = r.hi[blockIdx.y];
   const size_t stride = (size_t)gridDim.x * blockDim.x;
   const size_t pmask = ((size_t)1 << r.logp) - 1;
-  for (size_t i = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i <= hi; i += stride)
-    x[((i & pmask) << r.logq) + (i >> r.logp)] = make_float2(0.f, 0.f);
+  for (size_t i = lo + (size_t)blockIdx.x * blockDim.x + threadIdx.x; i <= hi; i += stride) {
+    const size_t k1 = i & pmask, k2 = i >> r.logp;
+    x[r.logp ? ((k2 >> 3) << r.logq) + 8 * k1 + (k2 & 7) : i] = make_float2(0.f, 0.f);
+  }
 }
 
 // ------------------------------------------------------------------------------

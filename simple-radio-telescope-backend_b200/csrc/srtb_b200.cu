@@ -640,14 +640,15 @@ static encode_tiled_fn get_encode_tiled() {
 // complex64 elements are described to TMA as 8-byte integers; dims/box are innermost first
 static bool make_tensor_map(tensor_map_blob* out, const void* base, int rank, const cuuint64_t* dims,
                             const cuuint64_t* strides_bytes /* rank-1 */, const cuuint32_t* box,
-                            CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_INT64) {
+                            CUtensorMapDataType dtype = CU_TENSOR_MAP_DATA_TYPE_INT64,
+                            CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_NONE) {
   encode_tiled_fn enc = get_encode_tiled();
   if (!enc) return false;
   static_assert(sizeof(CUtensorMap) <= sizeof(tensor_map_blob), "tensor map size");
   cuuint32_t estr[3] = {1, 1, 1};
   CUtensorMap m;
   const CUresult r = enc(&m, dtype, (cuuint32_t)rank, const_cast<void*>(base), dims, strides_bytes,
-                         box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                         box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return false;
   std::memcpy(out->bytes, &m, sizeof(m));
@@ -990,7 +991,7 @@ static int get_bigrow_tables(srtb_b200_ctx* ctx, bool fwd, const float2** out) {
 }
 
 // sk != nullptr: SK + column sums in the epilogue (sk->partial is filled in here); chirp != nullptr: s1 + chirp on load.
-// sweep_order: `in` is the [P][L] spectrum r2c_sweep_order leaves (P = nrows = L / 8), read channel by channel
+// sweep_order: `in` is the channel-blocked spectrum r2c_sweep_order leaves (P = nrows = L / 8), read channel by channel
 template <int LOGL, bool FWD>
 static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size_t nrows, row_sk_params* sk,
                          const row_chirp_params* chirp, size_t* chunks_out, bool sweep_order = false) {
@@ -1000,7 +1001,7 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
   if (int rc = get_bigrow_tables<LOGL>(ctx, FWD, &tabs)) return rc;
   unsigned grid = 1;
   auto go = [&](auto kern, bool with_sk, auto... extra) -> int {
-    const size_t smem = C::bytes;
+    const size_t smem = sweep_order ? C::bytes_sw : C::bytes;
     if (int rc = persistent_grid(ctx, kern, C::NT, smem, smem, nrows, &grid)) return rc;
     row_sk_params p{};
     if (with_sk) {
@@ -1019,11 +1020,13 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
     if (sweep_order) {
       if (!(sk && chirp && chirp->newton == 5) || nrows * 8 != (size_t)C::L)
         return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: the sweep-order load needs the phase table and P = L / 8");
-      const cuuint64_t dims[2] = {(cuuint64_t)C::L, (cuuint64_t)nrows};
-      const cuuint64_t strides[1] = {(cuuint64_t)C::L * sizeof(float2)};
-      const cuuint32_t box[2] = {8u, 256u};
+      // the spectrum as lines of 16 elements (128 bytes); a box is a quarter of a half channel, 128 lines, swizzled so
+      // that stage 0's gather is conflict free without moving registers around
+      const cuuint64_t dims[2] = {16u, (cuuint64_t)nrows * C::L / 16};
+      const cuuint64_t strides[1] = {16 * sizeof(float2)};
+      const cuuint32_t box[2] = {16u, 128u};
       tensor_map_blob tm;
-      if (!make_tensor_map(&tm, in, 2, dims, strides, box))
+      if (!make_tensor_map(&tm, in, 2, dims, strides, box, CU_TENSOR_MAP_DATA_TYPE_INT64, CU_TENSOR_MAP_SWIZZLE_128B))
         return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: tensor map of the sweep-order spectrum refused");
       return go(waterfall_sweep_order_kernel, true, tm);
     }
@@ -1040,9 +1043,9 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
   return go(fft_bigrow_kernel<LOGL, FWD, false, 0>, false);
 }
 
-// the R2C row sweep of the sweep-order route: P rows of 2^14 points in place on s (clusters of two CTAs),
-// leaving mean(|X_k|^2, k < M) in the lane's `mean`
-static int launch_r2c_rows(srtb_b200_ctx* ctx, float2* s, size_t P) {
+// the R2C row sweep of the sweep-order route: P rows of 2^14 points of the scratch s (clusters of two CTAs), the
+// spectrum channel-blocked to out, leaving mean(|X_k|^2, k < M) in the lane's `mean`
+static int launch_r2c_rows(srtb_b200_ctx* ctx, const float2* s, float2* out, size_t P) {
   using C = bigrow<14>;
   auto kern = r2c_rows_split_kernel;
   const float2* tabs = nullptr;
@@ -1074,7 +1077,8 @@ static int launch_r2c_rows(srtb_b200_ctx* ctx, float2* s, size_t P) {
   if (2 * clusters > 4096) return fail(ctx, SRTB_B200_E_SIZE, "r2c: partial buffer too small");
   cfg.gridDim = dim3(2 * clusters);
   cfg.numAttrs = ctx->pdl_auto ? 2 : 1;
-  CK(cudaLaunchKernelEx(&cfg, kern, s, (unsigned)P, tabs, r2c_rows_params{ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean}));
+  CK(cudaLaunchKernelEx(&cfg, kern, s, out, (unsigned)P, tabs,
+                        r2c_rows_params{ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean}));
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -1392,7 +1396,7 @@ extern "C" int srtb_b200_rfi_range_to_bins(float f1, float f2, float freq_low, f
 }
 
 // mitigate_rfi_manual (rfi_mitigation.hpp:97-158): zero the listed bin ranges, 16 ranges per launch. logp != 0: x holds
-// the spectrum in sweep order (bin k at (k mod 2^logp) 2^logq + k / 2^logp, r2c_sweep_order)
+// the spectrum channel-blocked (bin k1 + 2^logp k2 at (k2 >> 3) 2^logq + 8 k1 + (k2 & 7), r2c_sweep_order)
 static int zero_bin_ranges(srtb_b200_ctx* ctx, float2* x, const std::vector<size_t>& bins, unsigned logp = 0,
                            unsigned logq = 0) {
   for (size_t r0 = 0; r0 < bins.size() / 2; r0 += 16) {
@@ -2058,10 +2062,11 @@ static int block_input_init(srtb_b200_ctx* ctx, const block_params& p, block_inp
 
 // The sweep-order route of 2^25-point R2Cs with rows of 2^14 (config #3): M = P Q, P = 2^11, Q = L = 2^14. Sweep 1 is the
 // raw-fused 2^11-point column sweep into the lane's scratch, sweep 2 the R2C row sweep (2^14-point rows, split, Σ|X|^2)
-// in place; bin k = k1 + P k2 then sits at k1 Q + k2, channel c is the box of all P rows by columns 8c .. 8c + 7, and
-// the whole-row waterfall kernel reads it from there (24 bytes per sample per stream instead of 32: no third sweep,
-// no fix-up). Taken when the unpack is fused (8-bit samples), the geometry is this one, every buffer is 16-byte
-// aligned and TMA tensor maps can be encoded; everything else keeps the three-sweep plan.
+// from the scratch into the stream's buffer, channel-blocked: bin k = k1 + P k2 sits at (k2 >> 3) Q + 8 k1 + (k2 & 7),
+// so channel c (L = 8 P bins) is one contiguous range, laid out [k1][k2 & 7], and the whole-row waterfall kernel
+// transforms it in place (24 bytes per sample per stream instead of 32: no third sweep, no fix-up). Taken when the
+// unpack is fused (8-bit samples), the geometry is this one, every buffer is 16-byte aligned and TMA tensor maps can
+// be encoded; everything else keeps the three-sweep plan.
 constexpr unsigned SWEEP_LOGP = 11, SWEEP_LOGQ = 14;
 static bool r2c_sweep_order(const block_params& p, const block_input& in) {
   if (!in.fuse_unpack || in.raw[0].bits != 0 || p.L != ((size_t)1 << SWEEP_LOGQ) ||
@@ -2074,16 +2079,14 @@ static bool r2c_sweep_order(const block_params& p, const block_input& in) {
 }
 
 static int r2c_sweep_order_stream(srtb_b200_ctx* ctx, const block_params& p, const block_input& in, int s,
-                                  float2** spectrum) {
+                                  float2* spectrum) {
   const size_t P = (size_t)1 << SWEEP_LOGP, Q = (size_t)1 << SWEEP_LOGQ;
   if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, P * Q * sizeof(float2))) return rc;
   float2* const z = static_cast<float2*>(ctx->lane.fft_scratch);
   bool done = false;
   if (int rc = dispatch_col_raw(ctx, (int)SWEEP_LOGP, in.raw[s], z, Q, &done)) return rc;
   if (!done) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "r2c: the raw 2^11-point column sweep refused the block");
-  if (int rc = launch_r2c_rows(ctx, z, P)) return rc;
-  *spectrum = z;
-  return 0;
+  return launch_r2c_rows(ctx, z, spectrum, P);
 }
 
 // R2C of stream s in its buffer, leaving mean(|X|^2) in the lane's `mean`. When the fused route refuses this size or
@@ -2194,14 +2197,13 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     float2* buf = reinterpret_cast<float2*>(bufs[s]);
     if (two_lanes) CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
     if (sweep_order) {
-      float2* z = nullptr;
       {
         stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
                            (double)p.N * (double)std::abs(p.cfg->baseband_input_bits) / 8.0 + 4.0 * (double)p.N);
-        if (int rc = r2c_sweep_order_stream(ctx, p, in, s, &z)) return rc;
+        if (int rc = r2c_sweep_order_stream(ctx, p, in, s, buf)) return rc;
       }
-      if (int rc = zero_bin_ranges(ctx, z, p.bins, SWEEP_LOGP, SWEEP_LOGQ)) return rc;
-      return stream_tail(ctx, p, s, buf, z, p.cfg->dm, /*phase_table=*/true, SWEEP_LOGP);
+      if (int rc = zero_bin_ranges(ctx, buf, p.bins, SWEEP_LOGP, SWEEP_LOGQ)) return rc;
+      return stream_tail(ctx, p, s, buf, buf, p.cfg->dm, /*phase_table=*/true, SWEEP_LOGP);
     }
     {
       stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,

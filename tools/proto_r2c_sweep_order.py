@@ -129,6 +129,49 @@ def table_and_zap(P, Q, M):
     return bool(seen.all())
 
 
+def channel_blocked_addr(k1, k2, Q):
+    """address of bin k1 + P k2 in the channel-blocked layout the row sweep stores (r2c_rows_split_kernel): channel
+    k2 >> 3 (L = Q = 8 P bins) is one contiguous range laid out [k1][k2 & 7]"""
+    return (k2 >> 3) * Q + 8 * k1 + (k2 & 7)
+
+
+def channel_blocked(P, Q, M, X, ref):
+    """(a) the row sweep's outputs placed at channel_blocked_addr give every channel contiguously, in the [k1][8] order
+    of stage 0's gather; (b) that order is the phase table's; (c) the manual zap's addresses of ranges across channel
+    and k2' edges hit exactly the bins of the range"""
+    L = 8 * P
+    assert Q == L
+    out = np.full(M, np.nan + 0j)
+    k1 = np.arange(P)[:, None]
+    k2 = np.arange(Q)[None, :]
+    out[channel_blocked_addr(k1, k2, Q)] = X            # X[k1][k2] = bin k1 + P k2, as the row sweep holds it
+    assert not np.isnan(out).any()
+    for ch in range(M // L):
+        blk = out[ch * L:(ch + 1) * L].reshape(P, 8)    # [k1][k2']: column c = bins k1 + P (8 ch + c)
+        chan = ref[ch * L:(ch + 1) * L]                  # natural-order bins of the channel
+        assert np.array_equal(blk, chan.reshape(8, P).T), "channel-blocked order"
+    # the phase table's entry ch L + 8 k1 + c holds bin k1 + P (8 ch + c): the same address
+    idx = np.arange(M)
+    ch, r = idx // L, idx % L
+    bins = r // 8 + P * (8 * ch + r % 8)
+    assert np.array_equal(channel_blocked_addr(bins % P, bins // P, Q), idx), "phase-table order"
+    # zap: ranges straddling a channel edge (bin L), a k2' edge (bin P (8 + 3)) and both (bin 2 L), as
+    # rfi_zero_ranges_kernel addresses them
+    logp, logq = P.bit_length() - 1, Q.bit_length() - 1
+    for edge in (L, P * 11, 2 * L):
+        lo, hi = edge - 3, edge + 2
+        z = out.copy()
+        for i in range(lo, hi + 1):
+            kk1, kk2 = i & (P - 1), i >> logp
+            z[((kk2 >> 3) << logq) + 8 * kk1 + (kk2 & 7)] = 0
+        back = np.empty(M, complex)
+        back[bins] = z                                   # natural order again
+        zapped = np.nonzero(back == 0)[0]
+        assert np.array_equal(zapped, np.arange(lo, hi + 1)), (edge, zapped)
+        assert np.array_equal(back[:lo], ref[:lo]) and np.array_equal(back[hi + 1:], ref[hi + 1:])
+    return True
+
+
 def main(argv):
     logp, logq = (int(argv[1]), int(argv[2])) if len(argv) > 2 else (5, 6)
     P, Q, M, X, ref, err = sweeps(logp, logq)
@@ -141,6 +184,16 @@ def main(argv):
     assert ok
     assert table_and_zap(P, Q, M)
     print("phase table / zap addresses: ok")
+    return 0
+
+
+def main_channel_blocked(logp=5, logq=8):
+    """the channel-blocked store (Q = L = 8 P) against numpy.fft.rfft"""
+    P, Q, M, X, ref, err = sweeps(logp, logq)
+    X64 = X.astype(np.complex128)
+    assert channel_blocked(P, Q, M, X64, X64.T.reshape(-1))
+    assert np.abs(X64.T.reshape(-1) - ref).max() < 1e-12 * np.abs(ref).max()
+    print(f"P=2^{logp} Q=2^{logq}: channel-blocked store, phase-table order and zap addresses: ok")
     return 0
 
 
