@@ -42,6 +42,10 @@ struct configs {
   // trial DMs searched on every block instead of `dm` (new with respect to the reference, whose config.hpp:128-132
   // leaves a DM search list as a TODO): comma-separated expressions or start:stop:step ranges; empty = search `dm` only
   std::string dm_list = "";
+  // trial DMs searched incoherently around `dm` on every block's dynamic spectrum (semi-coherent search: coherent at
+  // `dm`, then each trial's residual delay between channels as a whole-sample shift); same syntax as dm_list, and
+  // not together with it. Empty = no incoherent search
+  std::string incoherent_dm_list = "";
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

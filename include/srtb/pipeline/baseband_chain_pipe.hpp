@@ -23,6 +23,7 @@
 #include "srtb/memory.hpp"
 #include "srtb/pipeline/rfi_mitigation_pipe.hpp"  // srtb::spectrum::eval_rfi_ranges
 #include "srtb/pipeline/unpack_pipe.hpp"          // resolve_format_alias
+#include "srtb/program_options.hpp"               // parse_dm_list
 #include "srtb/work.hpp"
 
 namespace srtb {
@@ -75,19 +76,21 @@ struct block_config_holder {
 };
 
 /** the host series of stream s's positive boxcars: views into the pinned [streams][MAX_BOXCARS][L] buffer h_series,
- *  which they keep alive */
+ *  which they keep alive. row_stride: the distance between a stream's boxcar rows (0 = L; the incoherent search writes
+ *  rows of T <= L) */
 inline std::vector<srtb::work::time_series_holder> positive_series(const srtb_b200_detect_result& res,
                                                                    const std::shared_ptr<srtb::real>& h_series, int s,
-                                                                   size_t L) {
+                                                                   size_t L, size_t row_stride = 0) {
   std::vector<srtb::work::time_series_holder> out;
   srtb::real* base = h_series.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * L;
+  if (row_stride == 0) row_stride = L;
   for (int b = 0; b < res.n_boxcars; b++) {
     if (res.signal_count[b] == 0) continue;
     srtb::work::time_series_holder h;
     h.time_series_length = res.series_length[b];
     h.boxcar_length = res.boxcar_length[b];
     h.signal_count = res.signal_count[b];
-    h.h_time_series = std::shared_ptr<srtb::real>(h_series, base + (size_t)b * L);
+    h.h_time_series = std::shared_ptr<srtb::real>(h_series, base + (size_t)b * row_stride);
     out.push_back(h);
   }
   return out;
@@ -163,6 +166,11 @@ class baseband_chain_pipe {
     srtb_b200_detect_result res[4];
     const int n = srtb_b200_collect_block_ex(q.ctx(), p.ticket, res, nullptr, nullptr);
     q.check(n);
+    // incoherent_dm_list: the trial DMs searched around dm on each stream's dynamic spectrum
+    const std::vector<srtb::real> inc_dms = srtb::program_options::parse_dm_list(srtb::config.incoherent_dm_list);
+    std::shared_ptr<srtb::real> h_inc;
+    if (!inc_dms.empty())
+      h_inc = srtb::host_allocator.allocate_shared<srtb::real>((size_t)p.streams * SRTB_B200_MAX_BOXCARS * p.L);
     for (int s = 0; s < n; s++) {
       srtb::work::write_signal_work w;
       w.copy_parameter_from(p.work);
@@ -171,8 +179,42 @@ class baseband_chain_pipe {
       w.batch_size = p.C;
       w.zero_count = res[s].zero_count;
       w.ptr = p.d_spectrum[s];
-      w.time_series = positive_series(res[s], p.h_series, s, p.L);
+      if (inc_dms.empty())
+        w.time_series = positive_series(res[s], p.h_series, s, p.L);
+      else
+        incoherent_search(w, p, s, res[s], inc_dms, h_inc);
       out.push_back(std::move(w));
+    }
+  }
+
+  /** the incoherent search of stream s's spectrum: fills w's DM-search fields as dm_sweep_chain_pipe does (best trial's
+   *  DM and positive series, one summary per trial), so write_signal_pipe writes its .dm<DM>.<boxcar>.tim files and
+   *  dm_sweep.csv; the work is positive when the best trial is */
+  void incoherent_search(srtb::work::write_signal_work& w, const pending_block& p, int s,
+                         const srtb_b200_detect_result& block_res, const std::vector<srtb::real>& dms,
+                         const std::shared_ptr<srtb::real>& h_inc) {
+    const auto& cfg = holder.cfg;
+    const size_t n_dm = dms.size();
+    std::vector<srtb_b200_detect_result> tr(n_dm);
+    std::vector<srtb_b200_peak> peaks(n_dm);
+    int32_t best = 0;
+    q.check(srtb_b200_incoherent_dm_search(
+        q.ctx(), p.d_spectrum[s].get(), p.L, p.C, p.L - block_res.time_series_count, cfg.baseband_freq_low,
+        cfg.baseband_bandwidth, cfg.baseband_sample_rate, cfg.dm, dms.data(), n_dm,
+        cfg.signal_detect_signal_noise_threshold, cfg.signal_detect_channel_threshold,
+        cfg.signal_detect_max_boxcar_length, tr.data(), peaks.data(), &best,
+        h_inc.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L));
+    const srtb_b200_detect_result& r = tr[best];
+    w.time_series = positive_series(r, h_inc, s, p.L, r.time_series_count);
+    w.dm = dms[best];
+    for (size_t j = 0; j < n_dm; j++) {
+      srtb::work::dm_trial_summary d;
+      d.dm = dms[j];
+      d.detect_enabled = tr[j].detect_enabled != 0;
+      for (int b = 0; b < tr[j].n_boxcars; b++)
+        d.boxcars.push_back({tr[j].boxcar_length[b], tr[j].series_length[b], tr[j].signal_count[b],
+                             tr[j].threshold[b], peaks[j].snr[b], peaks[j].peak_index[b]});
+      w.dm_trials.push_back(std::move(d));
     }
   }
 };

@@ -4,7 +4,10 @@
 #pragma once
 #include <algorithm>
 #include <optional>
+#include <stdexcept>
 #include <stop_token>
+#include <string>
+#include <vector>
 
 #include "srtb/config.hpp"
 #include "srtb/cuda_queue.hpp"
@@ -24,12 +27,34 @@ inline size_t nsamps_reserved() {
   return r;
 }
 
-/** the block overlap the file reader rewinds and the baseband writer trims: nsamps_reserved() without a dm_list, else
+/** the block overlap the file reader rewinds and the baseband writer trims. With incoherent_dm_list (and
+ *  baseband_reserve_sample): nsamps_reserved() + 2C (S+ + S-). Otherwise nsamps_reserved() without a dm_list, else
  *  the largest srtb_b200_nsamps_reserved over the trial DMs, so the trial with the largest dispersive smear still sees
  *  every pulse whole. The maximum is taken of the function itself: the sign of the delay depends on the signs of the DM
  *  and the bandwidth. Each trial's detector still leaves out only its own reserved tail, so trials with a smaller smear
  *  search part of the overlap in both blocks. */
+/** S+ + S-: the samples of the dynamic spectrum the incoherent search (incoherent_dm_list) shifts its trials over, the
+ *  C of the block path (spectrum_channel_count, at most N / 2); 0 without a list */
+inline uint64_t incoherent_span() {
+  const auto& c = srtb::config;
+  const std::vector<srtb::real> dms = srtb::program_options::parse_dm_list(c.incoherent_dm_list);
+  if (dms.empty()) return 0;
+  const size_t C = std::min<size_t>(c.spectrum_channel_count, c.baseband_input_count / 2);
+  uint64_t s_plus = 0, s_minus = 0;
+  if (srtb_b200_incoherent_shifts(C, c.baseband_freq_low, c.baseband_bandwidth, c.baseband_sample_rate, c.dm,
+                                  dms.data(), dms.size(), nullptr, &s_plus, &s_minus) != 0)
+    throw std::invalid_argument("[dedisperse] incoherent_dm_list: " + std::string{srtb_b200_last_error(nullptr)});
+  return s_plus + s_minus;
+}
+
 inline size_t nsamps_reserved_max() {
+  if (!srtb::config.incoherent_dm_list.empty()) {
+    // the incoherent search's trials read S+ + S- spectrum samples (2C baseband samples each) past the series it
+    // searches: the next block repeats them, so a pulse there is searched whole in one of the two blocks
+    if (!srtb::config.baseband_reserve_sample) return nsamps_reserved();
+    const size_t C = std::min<size_t>(srtb::config.spectrum_channel_count, srtb::config.baseband_input_count / 2);
+    return nsamps_reserved() + 2 * C * (size_t)incoherent_span();
+  }
   if (srtb::config.dm_list.empty()) return nsamps_reserved();
   const auto& c = srtb::config;
   size_t r = 0;

@@ -234,6 +234,7 @@ inline const std::vector<std::string>& known_options() {
       "baseband_freq_low", "baseband_bandwidth", "baseband_sample_rate", "baseband_reserve_sample",
       "udp_receiver_address", "udp_receiver_port", "udp_receiver_cpu_preferred", "input_file_path",
       "input_file_offset_bytes", "baseband_output_file_prefix", "baseband_write_all", "dm", "dm_list",
+      "incoherent_dm_list",
       "dedisperse_measurement", "fft_fftw_wisdom_path", "mitigate_rfi_average_method_threshold",
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length"};
@@ -339,6 +340,17 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
     SRTB_LOGI << " [program_options] " << "dm_list = " << value << " (" << trials.size() << " trial(s))";
     return;
   }
+  if (name == "incoherent_dm_list") {
+    std::vector<srtb::real> trials;
+    try {
+      trials = parse_dm_list(value);  // the same syntax; a bad list is rejected here, named by its own key
+    } catch (const std::invalid_argument& e) {
+      throw std::invalid_argument(std::string{"[program_options] incoherent_dm_list: "} + e.what());
+    }
+    config.incoherent_dm_list = value;
+    SRTB_LOGI << " [program_options] " << "incoherent_dm_list = " << value << " (" << trials.size() << " trial(s))";
+    return;
+  }
   if (name == "udp_receiver_address") {
     config.udp_receiver_address.clear();
     for (const auto& sub : split_list(value, ',')) config.udp_receiver_address.push_back(trim(sub));
@@ -373,8 +385,18 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_LOGW << " [program_options] " << "Unrecognized config: name = " << name << ", value = " << value;
 }
 
+/** a coherent DM sweep (dm_list) and an incoherent search around dm (incoherent_dm_list) are two ways to search one
+ *  block; both set is rejected, naming both keys */
+inline void check_dm_search_keys(const srtb::configs& config) {
+  if (!trim(config.dm_list).empty() && !trim(config.incoherent_dm_list).empty())
+    throw std::invalid_argument(
+        "[program_options] dm_list and incoherent_dm_list are both set: choose the coherent DM sweep (dm_list) or the "
+        "incoherent search around dm (incoherent_dm_list)");
+}
+
 inline void apply_changed_configs(const std::map<std::string, std::string>& changed, srtb::configs& config) {
   for (const auto& [name, value] : changed) evaluate_and_apply_changed_config(name, value, config);
+  check_dm_search_keys(config);
 }
 
 }  // namespace program_options

@@ -301,6 +301,41 @@ const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int stream);
    last stream's best trial) */
 const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx);
 
+/* ---- semi-coherent DM search on one stream's dynamic spectrum ----------------------------------------------------
+ * The block path leaves x[C][L] (complex64, time contiguous), coherently dedispersed at `dm`, SK-flagged channels
+ * stored as zeros. Trial DMs near dm are then searched incoherently: each channel's power is shifted by the residual
+ * delay between channels and summed over channels.
+ * Shifts (host, float64): f_ref = float(freq_low + bandwidth) (the chirp's f_c: the top edge for a positive
+ * bandwidth, the bottom one for a negative one), f(c) = freq_low + bandwidth (c + 0.5) / C,
+ *   s[d][c] = llround(4.148808e3 (DM_d - dm) (1/f(c)^2 - 1/f_ref^2) sample_rate / (2C)),
+ * S+ = max(0, max s), S- = max(0, -min s) over every trial and channel.
+ * srtb_b200_incoherent_shifts writes s ([n_dm][C], or shifts == NULL), S+ and S- (either may be NULL). A zero
+ * chan_count, a null h_dms or n_dm == 0 returns SRTB_B200_E_INVALID; a shift that is not finite SRTB_B200_E_INVALID. */
+int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, float bandwidth, float sample_rate, float dm,
+                                const float* h_dms, size_t n_dm, int64_t* shifts, uint64_t* s_plus, uint64_t* s_minus);
+/* The search. With ts = time_count - time_reserved_count and T = ts - S+ - S-, trial d's series is
+ *   v_d[j] = sum_c |x[c][j + S- + s[d][c]]|^2, j < T (fp32, channels added in index order: two calls agree bit for bit),
+ * so every trial has the same length and time origin. Each v_d goes through signal_detect_pipe_2's detector as the block
+ * path runs it (zero_count and detect_enabled from the spectrum's first sample per channel, mean removal, boxcars of 1,
+ * 2, 4, ... up to max_boxcar_length, each < T, at most 32; time_series_count = T) into h_results[d], and its peaks into
+ * h_peaks[d] as srtb_b200_process_block_dm_sweep_ex defines them. The best trial (its rule too) goes to *h_best_trial
+ * and its positive boxcar series to h_series ([SRTB_B200_MAX_BOXCARS][T] floats, rows of other boxcars untouched).
+ * With a single trial at DM = dm every shift is 0 and v is the block path's column sum.
+ * Three kernel launches per call whatever n_dm. Stream-ordered on the ctx's stream; synchronises it once before it
+ * returns, and once more when h_series is given and the best trial has a positive boxcar.
+ * Before any launch: a null ctx, d_spectrum, h_dms or h_results, n_dm == 0, a zero size or an 8-byte misaligned spectrum
+ * returns SRTB_B200_E_INVALID; time_reserved_count >= time_count, T < 2, n_dm > SRTB_B200_INCOHERENT_MAX_DMS or
+ * time_count > 2^30 returns SRTB_B200_E_SIZE.
+ * Scratch the ctx grows on demand and keeps: at most n_dm (12 C + 132 T + 1448) bytes of device memory (shift tables,
+ * the series of every boxcar, the scans, headers and peaks), and the shift tables on the host. */
+#define SRTB_B200_INCOHERENT_MAX_DMS 4096
+int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count, size_t chan_count,
+                                   size_t time_reserved_count, float freq_low, float bandwidth, float sample_rate,
+                                   float dm, const float* h_dms, size_t n_dm, float snr, float channel_threshold,
+                                   size_t max_boxcar_length, srtb_b200_detect_result* h_results /* [n_dm] */,
+                                   srtb_b200_peak* h_peaks /* [n_dm] or NULL */, int32_t* h_best_trial /* or NULL */,
+                                   float* h_series /* [SRTB_B200_MAX_BOXCARS][T] or NULL */);
+
 /* simplify_spectrum_pipe_2 (pipeline/spectrum_pipe.hpp:82-143): resample_spectrum_3 with norm(),
  * normalize_with_average_value, generate_pixmap. d_spectrum is [in_height][in_width] complex64
  * (time contiguous, as a block leaves it); d_intensity [out_height][out_width] floats receives the

@@ -785,7 +785,8 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
                                                                  size_t time_count, size_t chan_count,
                                                                  float chan_thr, size_t max_boxcar,
                                                                  unsigned* __restrict__ ticket,
-                                                                 detect_dev_result* __restrict__ res) {
+                                                                 detect_dev_result* __restrict__ res,
+                                                                 size_t ts_trial_stride, size_t acc_trial_stride) {
   __shared__ float sm[32][33];
   __shared__ double smd[32];
   __shared__ double warp_tot[32];
@@ -794,12 +795,23 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
   pdl_launch_dependents();
   pdl_wait();
   const int tid = threadIdx.x, lx = tid & 31, ly = tid >> 5;
+  // batched over trials (incoherent DM search): blockIdx.y selects the trial's series, scan, ticket and header; the
+  // block path launches one row of CTAs, so y = 0
+  {
+    const size_t y = blockIdx.y;
+    if (partial) partial += y * chunks * ts_count;
+    ts += y * ts_trial_stride;
+    acc += y * acc_trial_stride;
+    ticket += y;
+    res += y;
+  }
   // one wave of CTAs, each walking its share of the 32-column groups: the grid-wide fence + ticket at the end then
   // costs one round of latency instead of one per wave. The partial rows of a group are loaded eight at a time
-  // (independent loads in flight) and added in index order.
+  // (independent loads in flight) and added in index order. partial == nullptr: ts already holds the series
+  // (the incoherent search writes it there), only the zero count, mean removal and scan run.
   const size_t per = (chunks + 31) / 32;
   const size_t c0 = (size_t)ly * per, c1 = min(c0 + per, chunks);
-  for (size_t grp = blockIdx.x; grp * 32 < ts_count; grp += gridDim.x) {
+  for (size_t grp = blockIdx.x; partial && grp * 32 < ts_count; grp += gridDim.x) {
     const size_t j = grp * 32 + lx;
     float a = 0.f;
     if (j < ts_count) {
@@ -940,6 +952,7 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
 // host_out (optional): pinned host memory [MAX_BOXCARS][row_stride] that receives, straight from this kernel, the
 // series of every boxcar with a positive count — the reference attaches the host copy of a series to the work only
 // when count_signal is positive (signal_detect_pipe.hpp:347-366,405-423); negative blocks cost no PCIe traffic.
+// gridDim.y > 1 runs one trial per y (series, acc, res and peak advanced by the given strides and one record).
 // PEAK (DM sweep): the counting pass also reduces (max v[j], smallest j reaching it) and writes peak->snr[nb] =
 // max / sqrt(variance) (0 when the variance is 0) and peak->peak_index[nb]; the block path launches PEAK = false.
 template <bool PEAK = false>
@@ -948,11 +961,19 @@ __global__ void __launch_bounds__(1024) detect_boxcar_kernel(float* __restrict__
                                                              size_t ts_count, float snr,
                                                              detect_dev_result* __restrict__ res,
                                                              float* __restrict__ host_out,
-                                                             detect_dev_peak* __restrict__ peak = nullptr) {
+                                                             detect_dev_peak* __restrict__ peak,
+                                                             size_t series_trial_stride, size_t acc_trial_stride) {
   __shared__ double smd[32];
   __shared__ float s_thr;
   pdl_launch_dependents();
   pdl_wait();
+  {  // batched over trials (incoherent DM search, host_out == nullptr there): blockIdx.y = trial; else y = 0
+    const size_t y = blockIdx.y;
+    series += y * series_trial_stride;
+    acc += y * acc_trial_stride;
+    res += y;
+    if (PEAK) peak += y;
+  }
   const int nb = blockIdx.x;
   if (nb >= res->n_boxcars) return;
   const int tid = threadIdx.x, nt = blockDim.x;

@@ -23,6 +23,7 @@
 #include "ops_kernels.cuh"
 #include "thumbnail.cuh"
 #include "correlator.cuh"
+#include "incoherent.cuh"
 
 using namespace srtb_b200;
 
@@ -137,6 +138,19 @@ struct srtb_b200_ctx {
   void* corr_partial = nullptr;
   size_t corr_partial_bytes = 0;
   unsigned* corr_tickets = nullptr;
+  // incoherent DM search: the shift tables of the last (geometry, dm, trial list), on the host and the device, and the
+  // per-trial series [n_dm][nb][T], scans [n_dm][T], result headers, peaks and tickets
+  std::vector<double> inc_key;
+  std::vector<int64_t> inc_shifts;  // [n_dm][C]
+  uint64_t inc_s_plus = 0, inc_s_minus = 0;
+  std::vector<int> inc_off, inc_order;            // [C][n_dm] s + S- in sorted order; [n_dm] trial of each sorted slot
+  std::vector<int2> inc_gspan, inc_groups;        // [groups][C] (min, max) of a group's offsets; [groups] (first, count)
+  unsigned inc_spread = 0;                         // largest max - min of any group and channel
+  bool inc_tab_uploaded = false;
+  void* inc_tab = nullptr;
+  size_t inc_tab_bytes = 0;
+  void* inc_work = nullptr;
+  size_t inc_work_bytes = 0;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -318,6 +332,8 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   cudaFree(ctx->corr_rows);
   cudaFree(ctx->corr_partial);
   cudaFree(ctx->corr_tickets);
+  cudaFree(ctx->inc_tab);
+  cudaFree(ctx->inc_work);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
     cudaFree(ctx->slot_baseband[i]);
     for (auto& p : ctx->slot_stream_buf[i]) cudaFree(p);
@@ -1571,7 +1587,7 @@ static int detect_tail(srtb_b200_ctx* ctx, int slot, const float2* x, size_t tim
   stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_DETECT_TAIL, 4.0 * (double)chunks * (double)ts_count);
   CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>((ts_count + 31) / 32, (size_t)ctx->sm_count)),
                 dim3(1024), 0, (const float*)ctx->lane.colsum_partial, ts_count, chunks, ctx->series[slot], ctx->lane.acc, x, zero_stride,
-                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot));
+                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0));
   ctx->launches++;
   CK(cudaGetLastError());
   // one CTA per possible boxcar; CTAs beyond n_boxcars (known only on the device) exit at once
@@ -1579,10 +1595,12 @@ static int detect_tail(srtb_b200_ctx* ctx, int slot, const float2* x, size_t tim
   for (size_t b = 2; b <= max_boxcar && b < ts_count && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2) max_nb++;
   if (ctx->peak_dst)
     CK(launch_pdl(ctx, detect_boxcar_kernel<true>, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count,
-                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, ctx->peak_dst));
+                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, ctx->peak_dst, (size_t)0,
+                  (size_t)0));
   else
     CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count,
-                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, (detect_dev_peak*)nullptr));
+                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, (detect_dev_peak*)nullptr,
+                  (size_t)0, (size_t)0));
   ctx->launches++;
   CK(cudaGetLastError());
   ctx->slot_time_count[slot] = time_count;
@@ -2412,6 +2430,213 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
       return fail(ctx, SRTB_B200_E_CUDA,
                   "dm_sweep: the best trial's re-run of stream " + std::to_string(s) + " differs from its trial");
   return p.streams;
+}
+
+// ---- incoherent DM search on one stream's dynamic spectrum (incoherent.cuh): every trial's series in one kernel, then
+// the detector's scan and boxcars batched over the trials, the best trial chosen on the host by best_trial().
+
+// s[d][c] = llround(K (DM_d - dm) (1/f(c)^2 - 1/f_ref^2) sample_rate / (2C)), f_ref = float(freq_low + bandwidth) (the
+// chirp's f_c), f(c) = freq_low + bandwidth (c + 0.5) / C, all in double; S+ / S- = max(0, max s) / max(0, -min s)
+static int incoherent_shift_table(size_t C, float freq_low, float bandwidth, float sample_rate, float dm,
+                                  const float* dms, size_t n_dm, std::vector<int64_t>* shifts, uint64_t* s_plus,
+                                  uint64_t* s_minus) {
+  constexpr double D = 4.148808e3;
+  const double f_ref = (double)(float)(freq_low + bandwidth);
+  const double scale = (double)sample_rate / (2.0 * (double)C);
+  shifts->assign(n_dm * C, 0);
+  int64_t hi = 0, lo = 0;
+  for (size_t c = 0; c < C; c++) {
+    const double f = (double)freq_low + (double)bandwidth * ((double)c + 0.5) / (double)C;
+    const double k = (1.0 / (f * f) - 1.0 / (f_ref * f_ref)) * scale * D;
+    for (size_t d = 0; d < n_dm; d++) {
+      const double v = ((double)dms[d] - (double)dm) * k;
+      if (!std::isfinite(v)) return SRTB_B200_E_INVALID;
+      if (std::fabs(v) > 4.0e18) return SRTB_B200_E_SIZE;
+      const int64_t sh = std::llround(v);
+      (*shifts)[d * C + c] = sh;
+      hi = std::max(hi, sh);
+      lo = std::min(lo, sh);
+    }
+  }
+  *s_plus = (uint64_t)hi;
+  *s_minus = (uint64_t)(-lo);
+  return 0;
+}
+
+extern "C" int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, float bandwidth, float sample_rate,
+                                           float dm, const float* h_dms, size_t n_dm, int64_t* shifts,
+                                           uint64_t* s_plus, uint64_t* s_minus) {
+  if (chan_count == 0 || !h_dms || n_dm == 0)
+    return fail(nullptr, SRTB_B200_E_INVALID, "incoherent_shifts: bad argument");
+  std::vector<int64_t> tab;
+  uint64_t sp = 0, sm = 0;
+  if (int rc = incoherent_shift_table(chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm, &tab, &sp, &sm))
+    return fail(nullptr, rc, "incoherent_shifts: a shift is not finite or out of range");
+  if (shifts) std::memcpy(shifts, tab.data(), tab.size() * sizeof(int64_t));
+  if (s_plus) *s_plus = sp;
+  if (s_minus) *s_minus = sm;
+  return 0;
+}
+
+// the shift tables of (C, band, dm, trials), cached: the host table, and the kernel's sorted offsets and groups. The
+// trials are sorted by DM and cut greedily into groups of at most INC_GROUP whose spread over every channel is at most
+// INC_SPREAD_MAX (a single trial has none), so neighbouring trials share a group whatever order they came in.
+static int incoherent_tables(srtb_b200_ctx* ctx, size_t C, float freq_low, float bandwidth, float sample_rate,
+                             float dm, const float* dms, size_t n_dm) {
+  std::vector<double> key = {(double)C, freq_low, bandwidth, sample_rate, dm};
+  key.insert(key.end(), dms, dms + n_dm);
+  if (key == ctx->inc_key) return 0;
+  ctx->inc_key.clear();
+  if (int rc = incoherent_shift_table(C, freq_low, bandwidth, sample_rate, dm, dms, n_dm, &ctx->inc_shifts,
+                                      &ctx->inc_s_plus, &ctx->inc_s_minus))
+    return fail(ctx, rc, "incoherent_dm_search: a shift is not finite or out of range");
+  const std::vector<int64_t>& sh = ctx->inc_shifts;
+  const int64_t s_minus = (int64_t)ctx->inc_s_minus;
+  std::vector<int>& order = ctx->inc_order;
+  order.resize(n_dm);
+  for (size_t d = 0; d < n_dm; d++) order[d] = (int)d;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return dms[a] < dms[b]; });
+  ctx->inc_groups.clear();
+  ctx->inc_gspan.clear();
+  ctx->inc_spread = 0;
+  std::vector<int64_t> gmin(C), gmax(C), nmin(C), nmax(C);
+  size_t first = 0;
+  while (first < n_dm) {
+    for (size_t c = 0; c < C; c++) gmin[c] = gmax[c] = sh[(size_t)order[first] * C + c];
+    size_t count = 1;
+    while (first + count < n_dm && count < (size_t)INC_GROUP) {
+      const size_t d = (size_t)order[first + count];
+      bool fits = true;
+      for (size_t c = 0; c < C && fits; c++) {
+        nmin[c] = std::min(gmin[c], sh[d * C + c]);
+        nmax[c] = std::max(gmax[c], sh[d * C + c]);
+        fits = nmax[c] - nmin[c] <= INC_SPREAD_MAX;
+      }
+      if (!fits) break;
+      gmin.swap(nmin);
+      gmax.swap(nmax);
+      count++;
+    }
+    ctx->inc_groups.push_back(make_int2((int)first, (int)count));
+    for (size_t c = 0; c < C; c++) {
+      ctx->inc_gspan.push_back(make_int2((int)(gmin[c] + s_minus), (int)(gmax[c] + s_minus)));
+      ctx->inc_spread = std::max(ctx->inc_spread, (unsigned)(gmax[c] - gmin[c]));
+    }
+    first += count;
+  }
+  ctx->inc_off.resize(C * n_dm);
+  for (size_t c = 0; c < C; c++)
+    for (size_t i = 0; i < n_dm; i++) ctx->inc_off[c * n_dm + i] = (int)(sh[(size_t)order[i] * C + c] + s_minus);
+  ctx->inc_tab_uploaded = false;
+  ctx->inc_key = std::move(key);
+  return 0;
+}
+
+extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count,
+                                              size_t chan_count, size_t time_reserved_count, float freq_low,
+                                              float bandwidth, float sample_rate, float dm, const float* h_dms,
+                                              size_t n_dm, float snr, float channel_threshold,
+                                              size_t max_boxcar_length, srtb_b200_detect_result* h_results,
+                                              srtb_b200_peak* h_peaks, int32_t* h_best_trial, float* h_series) {
+  API_LOCK(ctx);
+  if (!ctx || !d_spectrum || !h_dms || !h_results || n_dm == 0 || time_count == 0 || chan_count == 0)
+    return fail(ctx, SRTB_B200_E_INVALID, "incoherent_dm_search: bad argument");
+  if (!aligned8(d_spectrum)) return fail(ctx, SRTB_B200_E_INVALID, "incoherent_dm_search: spectrum not 8-byte aligned");
+  if (time_reserved_count >= time_count)
+    return fail(ctx, SRTB_B200_E_SIZE, "incoherent_dm_search: time_reserved_count >= time_count");
+  if (n_dm > SRTB_B200_INCOHERENT_MAX_DMS)
+    return fail(ctx, SRTB_B200_E_SIZE, "incoherent_dm_search: more than SRTB_B200_INCOHERENT_MAX_DMS trials");
+  if (time_count > ((size_t)1 << 30))
+    return fail(ctx, SRTB_B200_E_SIZE, "incoherent_dm_search: time_count above 2^30");
+  CK(cudaSetDevice(ctx->device));
+  if (int rc = incoherent_tables(ctx, chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm)) return rc;
+  const size_t ts = time_count - time_reserved_count;
+  const uint64_t span = ctx->inc_s_plus + ctx->inc_s_minus;
+  if (span + 2 > ts)
+    return fail(ctx, SRTB_B200_E_SIZE, "incoherent_dm_search: T = ts - S+ - S- = " +
+                                           std::to_string((long long)ts - (long long)span) + " < 2");
+  const size_t T = ts - span;
+  unsigned max_nb = 1;
+  for (size_t b = 2; b <= max_boxcar_length && b < T && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2) max_nb++;
+  const size_t n_groups = ctx->inc_groups.size();
+  // device tables: off [C][n_dm] int, order [n_dm] int, gspan [groups][C] int2, groups [groups] int2
+  const size_t off_b = chan_count * n_dm * sizeof(int), order_b = n_dm * sizeof(int);
+  const size_t gspan_o = (off_b + order_b + 15) & ~(size_t)15, gspan_b = n_groups * chan_count * sizeof(int2);
+  const size_t groups_o = gspan_o + gspan_b, tab_b = groups_o + n_groups * sizeof(int2);
+  if (ctx->inc_tab_bytes < tab_b) ctx->inc_tab_uploaded = false;
+  if (int rc = ensure(ctx, &ctx->inc_tab, &ctx->inc_tab_bytes, tab_b)) return rc;
+  // work: series [n_dm][max_nb][T], scans [n_dm][T], headers [n_dm], peaks [n_dm], tickets [n_dm]
+  const size_t series_stride = (size_t)max_nb * T;
+  const size_t series_b = n_dm * series_stride * sizeof(float), acc_b = n_dm * T * sizeof(float);
+  const size_t res_o = (series_b + acc_b + 255) & ~(size_t)255;
+  const size_t peak_o = res_o + n_dm * sizeof(detect_dev_result);
+  const size_t ticket_o = peak_o + n_dm * sizeof(detect_dev_peak);
+  const size_t work_b = ticket_o + n_dm * sizeof(unsigned);
+  if (int rc = ensure(ctx, &ctx->inc_work, &ctx->inc_work_bytes, work_b)) return rc;
+  char* tab = static_cast<char*>(ctx->inc_tab);
+  char* work = static_cast<char*>(ctx->inc_work);
+  float* d_series = reinterpret_cast<float*>(work);
+  float* d_acc = reinterpret_cast<float*>(work + series_b);
+  detect_dev_result* d_res = reinterpret_cast<detect_dev_result*>(work + res_o);
+  detect_dev_peak* d_peak = reinterpret_cast<detect_dev_peak*>(work + peak_o);
+  unsigned* d_ticket = reinterpret_cast<unsigned*>(work + ticket_o);
+  cudaStream_t st = ctx->lane.stream;
+  if (!ctx->inc_tab_uploaded) {  // the host vectors live in the ctx, so the copies may complete after we return
+    CK(cudaMemcpyAsync(tab, ctx->inc_off.data(), off_b, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tab + off_b, ctx->inc_order.data(), order_b, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tab + gspan_o, ctx->inc_gspan.data(), gspan_b, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tab + groups_o, ctx->inc_groups.data(), n_groups * sizeof(int2), cudaMemcpyHostToDevice, st));
+    ctx->inc_tab_uploaded = true;
+  }
+  CK(cudaMemsetAsync(work + res_o, 0, work_b - res_o, st));  // headers (zero_count is atomically added), peaks, tickets
+  const unsigned spread = ctx->inc_spread;
+  const size_t smem = incoherent_smem_bytes(spread);
+  if (smem > 48 * 1024) {
+    const void* key = reinterpret_cast<const void*>(incoherent_dedisperse_kernel);
+    if (!ctx->configured.count(key)) {  // once, for the largest spread any group may have
+      CK(cudaFuncSetAttribute(incoherent_dedisperse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              (int)incoherent_smem_bytes(INC_SPREAD_MAX)));
+      ctx->configured.insert(key);
+    }
+  }
+  const dim3 grid((unsigned)n_groups, (unsigned)((T + INC_TILE - 1) / INC_TILE));
+  incoherent_dedisperse_kernel<<<grid, INC_THREADS, smem, st>>>(
+      static_cast<const float2*>(d_spectrum), time_count, chan_count, T, n_dm, reinterpret_cast<const int*>(tab),
+      reinterpret_cast<const int2*>(tab + gspan_o), reinterpret_cast<const int2*>(tab + groups_o),
+      reinterpret_cast<const int*>(tab + off_b), INC_TILE + spread, d_series, series_stride);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  // the series are already in place: no partial sums (partial == nullptr); one CTA per trial zero-counts and scans
+  colsum_final_scan_kernel<<<dim3(1, (unsigned)n_dm), 1024, 0, st>>>(
+      nullptr, T, 0, d_series, d_acc, static_cast<const float2*>(d_spectrum), time_count, chan_count, channel_threshold,
+      max_boxcar_length, d_ticket, d_res, series_stride, T);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  detect_boxcar_kernel<true><<<dim3(max_nb, (unsigned)n_dm), 1024, 0, st>>>(
+      d_series, T, d_acc, T, snr, d_res, nullptr, d_peak, series_stride, T);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
+  static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
+  std::vector<srtb_b200_peak> own_peaks(h_peaks ? 0 : n_dm);
+  srtb_b200_peak* peaks = h_peaks ? h_peaks : own_peaks.data();
+  CK(cudaMemcpyAsync(h_results, d_res, n_dm * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(peaks, d_peak, n_dm * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  const int best = best_trial(h_results, reinterpret_cast<const detect_dev_peak*>(peaks), n_dm, 1, 0);
+  if (h_best_trial) *h_best_trial = best;
+  if (!h_series) return 0;
+  // the best trial's positive series, rows of T floats as process_block writes them (only the positive rows)
+  const srtb_b200_detect_result& r = h_results[best];
+  bool any = false;
+  for (int b = 0; b < r.n_boxcars; b++) {
+    if (r.signal_count[b] == 0) continue;
+    CK(cudaMemcpyAsync(h_series + (size_t)b * T, d_series + (size_t)best * series_stride + (size_t)b * T,
+                       r.series_length[b] * sizeof(float), cudaMemcpyDeviceToHost, st));
+    any = true;
+  }
+  if (any) CK(cudaStreamSynchronize(st));
+  return 0;
 }
 
 // tickets wrap at a multiple of the slot count, so ticket % SRTB_B200_RING_SLOTS is always the slot that was used

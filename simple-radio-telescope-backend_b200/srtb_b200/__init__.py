@@ -140,7 +140,12 @@ SYMBOLS = {
     "srtb_b200_correlate": (_I, [_P, _P, _P, _SZ, _P]),
     "srtb_b200_correlate_accumulate": (_I, [_P, _P, _P, _I, _SZ, _SZ, _P, _I]),
     "srtb_b200_correlate_finish": (_I, [_P, _P, _SZ, C.c_uint64, _P]),
+    "srtb_b200_incoherent_shifts": (_I, [_SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _P, C.POINTER(C.c_uint64),
+                                         C.POINTER(C.c_uint64)]),
+    "srtb_b200_incoherent_dm_search": (_I, [_P, _P, _SZ, _SZ, _SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _F, _F, _SZ,
+                                            C.POINTER(DetectResult), _P, _P, _P]),
 }
+INCOHERENT_MAX_DMS = 4096
 
 _lib = None
 
@@ -323,6 +328,34 @@ class Context:
                        np.uint64).reshape(n_dm, streams, nb)
         return results, (snr, idx), [int(best[s]) for s in range(streams)], h_series, list(d_spectrum)
 
+    def incoherent_dm_search(self, d_spectrum, time_count: int, chan_count: int, time_reserved_count: int,
+                             freq_low: float, bandwidth: float, sample_rate: float, dm: float, dms, snr: float,
+                             channel_threshold: float, max_boxcar_length: int, h_series=None):
+        """semi-coherent DM search of one stream's [chan_count][time_count] complex64 dynamic spectrum (coherently
+        dedispersed at dm) over the trial DMs `dms`. Returns (results, (snr, idx), best_trial, h_series): results[d] per
+        trial, peaks as numpy arrays [n_dm][n_boxcars] (n_boxcars = the most any trial used), the best trial's index,
+        and h_series, a [MAX_BOXCARS][T] float32 array (or the caller's buffer of that size) holding the best trial's
+        positive series; T = results[0].time_series_count."""
+        import numpy as np
+        n_dm = len(dms)
+        arr = (C.c_float * n_dm)(*[float(d) for d in dms])
+        res = (DetectResult * n_dm)()
+        peaks = (Peak * n_dm)()
+        best = C.c_int32()
+        if h_series is None:
+            _, sp, sm = incoherent_shifts(chan_count, freq_low, bandwidth, sample_rate, dm, dms, table=False)
+            T = max(time_count - time_reserved_count - sp - sm, 1)
+            h_series = np.zeros((MAX_BOXCARS, T), np.float32)
+        self._ck(self.lib.srtb_b200_incoherent_dm_search(
+            self.h, _ptr(d_spectrum), time_count, chan_count, time_reserved_count, freq_low, bandwidth, sample_rate,
+            dm, arr, n_dm, snr, channel_threshold, max_boxcar_length, res, C.cast(peaks, C.c_void_p),
+            C.byref(best), _ptr(h_series)))
+        results = [res[d] for d in range(n_dm)]
+        nb = max([r.n_boxcars for r in results] + [0])
+        snr_a = np.array([list(peaks[d].snr)[:nb] for d in range(n_dm)], np.float32).reshape(n_dm, nb)
+        idx_a = np.array([list(peaks[d].peak_index)[:nb] for d in range(n_dm)], np.uint64).reshape(n_dm, nb)
+        return results, (snr_a, idx_a), int(best.value), h_series
+
     def submit_block(self, cfg: BlockConfig, h_baseband, nbytes: int) -> int:
         """pipelined ingest: H2D on the copy stream overlaps the previous block's compute"""
         return self._ck(self.lib.srtb_b200_submit_block(self.h, C.byref(cfg), _ptr(h_baseband), nbytes))
@@ -420,3 +453,20 @@ def nsamps_reserved(baseband_input_count: int, channel_count: int, freq_low: flo
                     sample_rate: float, dm: float, reserve_sample: bool) -> int:
     return int(load_library().srtb_b200_nsamps_reserved(baseband_input_count, channel_count, freq_low,
                                                          bandwidth, sample_rate, dm, int(reserve_sample)))
+
+
+def incoherent_shifts(chan_count: int, freq_low: float, bandwidth: float, sample_rate: float, dm: float, dms,
+                      table: bool = True):
+    """the incoherent DM search's channel shifts: (s [n_dm][chan_count] int64 numpy array, or None when table is
+    False; S+; S-), exactly as srtb_b200_incoherent_dm_search uses them"""
+    import numpy as np
+    lib = load_library()
+    n_dm = len(dms)
+    arr = (C.c_float * n_dm)(*[float(d) for d in dms])
+    out = np.zeros((n_dm, chan_count), np.int64) if table else None
+    sp, sm = C.c_uint64(), C.c_uint64()
+    rc = lib.srtb_b200_incoherent_shifts(chan_count, freq_low, bandwidth, sample_rate, dm, arr, n_dm,
+                                         None if out is None else out.ctypes.data, C.byref(sp), C.byref(sm))
+    if rc < 0:
+        raise SrtbError(rc, lib.srtb_b200_last_error(None).decode())
+    return out, int(sp.value), int(sm.value)

@@ -21,6 +21,9 @@
 // With dm_list set (a srtb::configs key: --dm_list "0:100:5" or a .cfg line), every block is searched over those trial
 // DMs by dm_sweep_chain_pipe instead of baseband_chain_pipe at `dm` (which is then not used); its pipes run without a
 // ring, so --ring_depth is ignored. The sink then writes the best trial's files and a per-stream S/N-versus-DM table.
+// With incoherent_dm_list set instead (--incoherent_dm_list, same syntax), baseband_chain_pipe dedisperses coherently at
+// `dm` and then searches those trial DMs incoherently on each stream's dynamic spectrum; the ring is kept and the sink
+// writes the same files for the best incoherent trial.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -223,6 +226,28 @@ int main(int argc, char** argv) {
   } else {
     SRTB_LOGI << " [main] " << devices.size() << " GPU(s), " << chains_per_gpu << " chain pipe(s) each, ring depth "
               << ring_depth;
+  }
+  const std::vector<srtb::real> inc_trials = srtb::program_options::parse_dm_list(cfg.incoherent_dm_list);
+  if (!inc_trials.empty()) {
+    uint64_t s_plus = 0, s_minus = 0;
+    const size_t C = std::min<size_t>(cfg.spectrum_channel_count, cfg.baseband_input_count / 2);
+    if (srtb_b200_incoherent_shifts(C, cfg.baseband_freq_low, cfg.baseband_bandwidth, cfg.baseband_sample_rate, cfg.dm,
+                                    inc_trials.data(), inc_trials.size(), nullptr, &s_plus, &s_minus) != 0) {
+      std::fprintf(stderr, "srtb_b200: incoherent_dm_list: %s\n", srtb_b200_last_error(nullptr));
+      return 2;
+    }
+    const size_t overlap = srtb::codd::nsamps_reserved_max();
+    if (overlap >= cfg.baseband_input_count) {
+      std::fprintf(stderr,
+                   "srtb_b200: incoherent_dm_list needs a block overlap of %zu samples (S+ = %llu, S- = %llu spectrum "
+                   "samples), not less than baseband_input_count = %zu: narrow the trial DMs or enlarge the block\n",
+                   overlap, (unsigned long long)s_plus, (unsigned long long)s_minus, (size_t)cfg.baseband_input_count);
+      return 2;
+    }
+    SRTB_LOGI << " [main] " << "incoherent DM search around dm = " << cfg.dm << ": " << inc_trials.size()
+              << " incoherent trial DM(s) from " << *std::min_element(inc_trials.begin(), inc_trials.end()) << " to "
+              << *std::max_element(inc_trials.begin(), inc_trials.end()) << ", S+ = " << s_plus << ", S- = " << s_minus
+              << " spectrum samples, block overlap " << overlap << " samples";
   }
   // the device chain between source and sink: one DM, or the trial DMs of dm_list
   auto start_chain = [&](auto in, auto out, int dev) {
