@@ -46,6 +46,10 @@ struct configs {
   // `dm`, then each trial's residual delay between channels as a whole-sample shift); same syntax as dm_list, and
   // not together with it. Empty = no incoherent search
   std::string incoherent_dm_list = "";
+  // also run the single-pulse detector on the total intensity of a block's streams (polarisations), sum_s |x_s|^2 over
+  // the channels no stream masks: sqrt(2) the S/N of either polarisation for an unpolarised pulse. Needs a format of
+  // two or more streams; not with dm_list or incoherent_dm_list
+  bool signal_detect_sum_polarizations = false;
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

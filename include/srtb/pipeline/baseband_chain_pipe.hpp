@@ -65,6 +65,7 @@ struct block_config_holder {
     cfg.signal_detect_signal_noise_threshold = static_cast<float>(c.signal_detect_signal_noise_threshold);
     cfg.signal_detect_channel_threshold = static_cast<float>(c.signal_detect_channel_threshold);
     cfg.signal_detect_max_boxcar_length = c.signal_detect_max_boxcar_length;
+    cfg.signal_detect_sum_streams = c.signal_detect_sum_polarizations ? 1 : 0;
     rfi_pairs.clear();
     for (const auto& r : srtb::spectrum::eval_rfi_ranges(c.mitigate_rfi_freq_list)) {
       rfi_pairs.push_back(r.first);
@@ -107,7 +108,8 @@ class baseband_chain_pipe {
     srtb::work::copy_to_device_work work;
     // what the block leaves behind, owned by the work items it turns into (zero copy, like the reference's d_in):
     std::vector<std::shared_ptr<srtb::complex<srtb::real>>> d_spectrum;  // per stream: N + 2 floats, [C][L] when done
-    std::shared_ptr<srtb::real> h_series;                                 // pinned [streams][MAX_BOXCARS][L]
+    std::shared_ptr<srtb::real> h_series;  // pinned [streams (+ 1 with the sum)][MAX_BOXCARS][L]
+    bool sum = false;                       // signal_detect_sum_streams: the sum's result follows the streams'
   };
   std::deque<pending_block> pending;  // blocks in the pinned-host ring of this queue's context
 
@@ -151,7 +153,9 @@ class baseband_chain_pipe {
       p.d_spectrum.push_back(srtb::device_allocator.allocate_shared<srtb::complex<srtb::real>>(Nc + 1));
       outputs.d_spectrum[s] = reinterpret_cast<float*>(p.d_spectrum.back().get());
     }
-    p.h_series = srtb::host_allocator.allocate_shared<srtb::real>((size_t)p.streams * SRTB_B200_MAX_BOXCARS * p.L);
+    p.sum = cfg.signal_detect_sum_streams != 0;
+    p.h_series = srtb::host_allocator.allocate_shared<srtb::real>((size_t)(p.streams + (p.sum ? 1 : 0)) *
+                                                                  SRTB_B200_MAX_BOXCARS * p.L);
     outputs.h_series = p.h_series.get();
     p.ticket = srtb_b200_submit_block_ex(q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(),
                                          in_work.baseband_data.baseband_input_bytes, /*on_device=*/0, &outputs);
@@ -163,9 +167,12 @@ class baseband_chain_pipe {
   void collect_front(out_type& out) {
     pending_block p = std::move(pending.front());
     pending.pop_front();
-    srtb_b200_detect_result res[4];
+    srtb_b200_detect_result res[5];
     const int n = srtb_b200_collect_block_ex(q.ctx(), p.ticket, res, nullptr, nullptr);
     q.check(n);
+    bool sum_positive = false;
+    if (p.sum)
+      for (int b = 0; b < res[n].n_boxcars; b++) sum_positive = sum_positive || res[n].signal_count[b] > 0;
     // incoherent_dm_list: the trial DMs searched around dm on each stream's dynamic spectrum
     const std::vector<srtb::real> inc_dms = srtb::program_options::parse_dm_list(srtb::config.incoherent_dm_list);
     std::shared_ptr<srtb::real> h_inc;
@@ -179,6 +186,13 @@ class baseband_chain_pipe {
       w.batch_size = p.C;
       w.zero_count = res[s].zero_count;
       w.ptr = p.d_spectrum[s];
+      w.sum_positive = sum_positive;
+      if (p.sum && s == 0) {
+        w.carries_sum = true;
+        w.sum_zero_count = res[n].zero_count;
+        for (int b = 0; b < res[n].n_boxcars; b++) w.sum_signal_count.push_back(res[n].signal_count[b]);
+        w.sum_time_series = positive_series(res[n], p.h_series, n, p.L);
+      }
       if (inc_dms.empty())
         w.time_series = positive_series(res[s], p.h_series, s, p.L);
       else

@@ -7,6 +7,8 @@
 //   <prefix><counter>.<i>.npy        complex64 dynamic spectrum, shape {batch_size, count} (:209-246)
 //   <prefix><counter>.<boxcar>.tim   float32 time series per detected boxcar           (:249-280)
 // and, for a DM search (dm_list), <prefix><counter>.dm<DM>.<boxcar>.tim and <prefix><counter>.<id>.dm_sweep.csv.
+// With signal_detect_sum_polarizations, a block whose total intensity is positive keeps every stream's work, and the
+// first stream's work writes the sum's series as <prefix><counter>.sum.<boxcar>.tim (once per block).
 // counter = udp_packet_counter, or the timestamp when there is none (:145-148).
 // Differences: files are written synchronously on the pipe's thread (the reference posts to thread
 // pools), and the .npy index is incremented until the name is free (the reference's loop never
@@ -53,7 +55,7 @@ class write_signal_pipe {
   /** the keep/drop decision alone (host logic; testable without a GPU) */
   std::optional<srtb::work::write_signal_work> select(srtb::work::write_signal_work work) {
     std::optional<srtb::work::write_signal_work> keep;
-    const bool has_signal = !work.time_series.empty();
+    const bool has_signal = !work.time_series.empty() || work.sum_positive;
     const bool real_time = srtb::config.input_file_path.empty();
     const double window = 0.45 * 1e9 * (double)srtb::config.baseband_input_count / srtb::config.baseband_sample_rate;
     auto near_positive = [&](uint64_t ts) {
@@ -114,7 +116,8 @@ class write_signal_pipe {
     written_++;
   }
 
-  /** the host-side files of a kept work: <stem>.<boxcar>.tim per series. A DM search's work (non-empty dm_trials)
+  /** the host-side files of a kept work: <stem>.<boxcar>.tim per series, <stem>.sum.<boxcar>.tim per positive series of
+   *  the total-intensity detector (first stream's work only). A DM search's work (non-empty dm_trials)
    *  names the DM its series belong to, <stem>.dm<DM>.<boxcar>.tim, and also gets <stem>.<data_stream_id>.dm_sweep.csv,
    *  one row per trial and boxcar (one row with zero boxcar fields for a trial whose detector was disabled): the S/N
    *  against DM that tells a dispersed pulse, which peaks at its DM, from RFI, which peaks at DM 0. */
@@ -128,6 +131,10 @@ class write_signal_pipe {
     const std::string dm_part = sweep ? ".dm" + fmt("%g", w.dm) : "";
     for (const auto& ts : w.time_series) {
       std::ofstream f(stem + dm_part + "." + std::to_string(ts.boxcar_length) + ".tim", std::ios::binary | std::ios::trunc);
+      f.write(reinterpret_cast<const char*>(ts.h_time_series.get()), (std::streamsize)(ts.time_series_length * sizeof(srtb::real)));
+    }
+    for (const auto& ts : w.sum_time_series) {
+      std::ofstream f(stem + ".sum." + std::to_string(ts.boxcar_length) + ".tim", std::ios::binary | std::ios::trunc);
       f.write(reinterpret_cast<const char*>(ts.h_time_series.get()), (std::streamsize)(ts.time_series_length * sizeof(srtb::real)));
     }
     if (!sweep) return;

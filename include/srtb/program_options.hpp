@@ -237,7 +237,8 @@ inline const std::vector<std::string>& known_options() {
       "incoherent_dm_list",
       "dedisperse_measurement", "fft_fftw_wisdom_path", "mitigate_rfi_average_method_threshold",
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
-      "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length"};
+      "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length",
+      "signal_detect_sum_polarizations"};
   return names;
 }
 
@@ -370,6 +371,7 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(signal_detect_signal_noise_threshold)
   SRTB_PARSE(signal_detect_channel_threshold)
   SRTB_PARSE(signal_detect_max_boxcar_length)
+  SRTB_PARSE(signal_detect_sum_polarizations)
   SRTB_PARSE(thread_query_work_wait_time)
   SRTB_PARSE(gui_enable)
   SRTB_PARSE(gui_pixmap_width)
@@ -392,6 +394,22 @@ inline void check_dm_search_keys(const srtb::configs& config) {
     throw std::invalid_argument(
         "[program_options] dm_list and incoherent_dm_list are both set: choose the coherent DM sweep (dm_list) or the "
         "incoherent search around dm (incoherent_dm_list)");
+}
+
+/** signal_detect_sum_polarizations adds the streams of a block: it needs two or more (`streams`, the format's count),
+ *  and it is a block-path detector, so neither DM search (dm_list, incoherent_dm_list) takes it */
+inline void check_sum_polarizations(const srtb::configs& config, size_t streams) {
+  if (!config.signal_detect_sum_polarizations) return;
+  if (streams < 2)
+    throw std::invalid_argument("[program_options] signal_detect_sum_polarizations needs a format with two or more "
+                                "streams, but baseband_format_type = " + config.baseband_format_type + " has " +
+                                std::to_string(streams));
+  if (!trim(config.dm_list).empty())
+    throw std::invalid_argument("[program_options] signal_detect_sum_polarizations and dm_list are both set: the "
+                                "coherent DM sweep has no total-intensity detector");
+  if (!trim(config.incoherent_dm_list).empty())
+    throw std::invalid_argument("[program_options] signal_detect_sum_polarizations and incoherent_dm_list are both set: "
+                                "the incoherent search has no total-intensity detector");
 }
 
 inline void apply_changed_configs(const std::map<std::string, std::string>& changed, srtb::configs& config) {

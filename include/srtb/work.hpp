@@ -198,6 +198,13 @@ struct dm_trial_summary {
 struct write_signal_work : public write_file_work {
   std::vector<time_series_holder> time_series;  // non-empty <=> has_signal
   size_t zero_count = 0;
+  // signal_detect_sum_polarizations: every stream's work of a block whose total-intensity detector is positive has
+  // sum_positive set (the sink keeps it); the block's first stream also carries that detector's result
+  bool sum_positive = false;
+  bool carries_sum = false;
+  size_t sum_zero_count = 0;
+  std::vector<size_t> sum_signal_count;               // per boxcar
+  std::vector<time_series_holder> sum_time_series;    // its positive series
   // DM search only (dm_sweep_chain_pipe): the best trial's DM, which ptr and time_series belong to, and every trial
   srtb::real dm = 0;
   std::vector<dm_trial_summary> dm_trials;

@@ -208,11 +208,31 @@ typedef struct {
   uint64_t signal_detect_max_boxcar_length;
   const float* rfi_freq_pairs;   /* MHz pairs parsed from mitigate_rfi_freq_list        */
   uint64_t n_rfi_freq_pairs;
+  int32_t signal_detect_sum_streams; /* non-zero: also detect on the streams' total intensity (below); 0 = off    */
 } srtb_b200_block_config;
+
+/* ---- the detector on total intensity (signal_detect_sum_streams != 0) ---------------------------------------------
+ * A block of S >= 2 streams gets one more result, computed from the streams' final dynamic spectra x_s[C][L] (after s1,
+ * the chirp, the waterfall FFT and SK, as the block leaves them). Channel c is dropped when |x_s[c][0]|^2 == 0 in any
+ * stream (the zero_count proxy, so a channel SK zapped in one stream is left out of every stream); K = the kept ones.
+ *   v[j] = sum_{c in K} sum_s |x_s[c][j]|^2, j < L' (the streams' time_series_count), in fp32 with a fixed operation
+ * order: the same bits with one lane or two, through process_block or the ring. v then goes through the block's detector
+ * unchanged (mean removal, scan, boxcars, count_signal). Its header: zero_count = C - |K|, detect_enabled by the
+ * reference's rule with that count, time_series_count = L'. For an unpolarised pulse with equal noise in both
+ * polarisations the sum has sqrt(2) times the S/N of either stream.
+ * Every stream's own header and series are bit-identical to a call with the field 0. Where the result goes:
+ *   - process_block[_device], collect_block[_ex]: h_results[streams] (h_results needs streams + 1 entries); the return
+ *     value stays the stream count;
+ *   - the positive series: slot `streams` of h_series, [streams + 1][SRTB_B200_MAX_BOXCARS][L] floats in all (the same
+ *     for srtb_b200_block_outputs.h_series; the ring's own buffer grows to that size).
+ * On the device the first lane waits for the second with an event once both streams' chains are enqueued (no host
+ * synchronisation); blocks with the field 0 keep the lanes free-running. Four kernels per block.
+ * Before any launch: a single-stream format returns SRTB_B200_E_INVALID; the DM sweep entries
+ * (srtb_b200_process_block_dm_sweep[_ex]) return SRTB_B200_E_UNSUPPORTED. */
 
 /* h_baseband: host (ideally pinned) bytes of one block, all streams interleaved as the
  * format says; the call copies them to the device, runs every stage for every stream and
- * fills h_results[stream]. d_spectrum_out (optional): per-stream device pointers that
+ * fills h_results[stream] (and h_results[streams] with signal_detect_sum_streams). d_spectrum_out (optional): per-stream device pointers that
  * receive the dynamic spectrum [C][L] (else it stays in ctx scratch).
  * Returns the number of streams processed (>0) or a negative status.
  * Baseband alignment (the rules of srtb_b200_unpack): a SIMPLE baseband must be aligned to its sample width (any

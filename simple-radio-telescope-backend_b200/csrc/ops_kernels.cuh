@@ -786,7 +786,8 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
                                                                  float chan_thr, size_t max_boxcar,
                                                                  unsigned* __restrict__ ticket,
                                                                  detect_dev_result* __restrict__ res,
-                                                                 size_t ts_trial_stride, size_t acc_trial_stride) {
+                                                                 size_t ts_trial_stride, size_t acc_trial_stride,
+                                                                 float* __restrict__ raw) {
   __shared__ float sm[32][33];
   __shared__ double smd[32];
   __shared__ double warp_tot[32];
@@ -808,7 +809,8 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
   // one wave of CTAs, each walking its share of the 32-column groups: the grid-wide fence + ticket at the end then
   // costs one round of latency instead of one per wave. The partial rows of a group are loaded eight at a time
   // (independent loads in flight) and added in index order. partial == nullptr: ts already holds the series
-  // (the incoherent search writes it there), only the zero count, mean removal and scan run.
+  // (the incoherent search writes it there), only the zero count, mean removal and scan run. raw (optional, y = 0
+// only): also receives the un-centred column sums (the total-intensity sum of stream_sum.cuh adds them).
   const size_t per = (chunks + 31) / 32;
   const size_t c0 = (size_t)ly * per, c1 = min(c0 + per, chunks);
   for (size_t grp = blockIdx.x; partial && grp * 32 < ts_count; grp += gridDim.x) {
@@ -831,6 +833,7 @@ __global__ void __launch_bounds__(1024) colsum_final_scan_kernel(const float* __
 #pragma unroll
       for (int g = 1; g < 32; g++) t += sm[g][lx];
       ts[j] = t;
+      if (raw) raw[j] = t;
     }
   }
   // K16: channels whose first sample is zero; every CTA takes a slice, integer atomics (exact)

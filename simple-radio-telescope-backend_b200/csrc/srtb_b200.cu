@@ -24,10 +24,14 @@
 #include "thumbnail.cuh"
 #include "correlator.cuh"
 #include "incoherent.cuh"
+#include "stream_sum.cuh"
 
 using namespace srtb_b200;
 
 static thread_local std::string g_last_error;
+
+// result headers per block: one per data stream (at most 4), then the total-intensity sum's (signal_detect_sum_streams)
+constexpr int RES_GROUP = 5, SUM_SLOT = 4;
 
 // what one chain of kernels writes through: the data streams of a block are independent until their result headers
 // are read back, so a context runs the odd-numbered ones on a second lane with its own CUDA stream and scratch (one
@@ -74,12 +78,20 @@ struct srtb_b200_ctx {
   float2* tw[13] = {nullptr};
   std::map<int, float2*> bigtw;  // log2(n_i) -> [3 << q]
   float2* bigrow_tab[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [logl - 13][forward] whole-row kernel tables
-  // detect (slots = streams in flight)
-  float* series[4] = {nullptr, nullptr, nullptr, nullptr};
+  // detect (slots = streams in flight, then SUM_SLOT)
+  float* series[RES_GROUP] = {};
   size_t series_elems = 0;
-  detect_dev_result* d_res = nullptr;
-  detect_dev_result* h_res = nullptr;  // pinned, 4 slots
-  size_t slot_time_count[4] = {0, 0, 0, 0};
+  detect_dev_result* d_res = nullptr;  // RES_GROUP slots
+  detect_dev_result* h_res = nullptr;  // pinned, RES_GROUP slots for process_block, then RES_GROUP per ring slot
+  size_t slot_time_count[RES_GROUP] = {};
+  // total-intensity sum: the streams' raw column sums [1 + RING_SLOTS][4][L] (group 0: process_block, 1 + slot: the
+  // ring; slot-owned, so a lane's next block cannot overwrite what the sum of this one still reads), and the mask
+  // kernel's output (mask float2[C], mismatched channels uint2[C], their count)
+  float* sum_raw = nullptr;
+  size_t sum_raw_bytes = 0;
+  void* sum_mask = nullptr;
+  size_t sum_mask_bytes = 0;
+  float* raw_dst = nullptr;  // block path with the sum: this block's raw column sums [4][L] (else null)
   // pipelined ingest ring
   cudaStream_t copy_stream = nullptr;
   void* slot_baseband[SRTB_B200_RING_SLOTS] = {nullptr};
@@ -89,6 +101,7 @@ struct srtb_b200_ctx {
   bool slot_busy[SRTB_B200_RING_SLOTS] = {false};
   cudaEvent_t slot_done_alt[SRTB_B200_RING_SLOTS] = {nullptr};  // second lane's completion of the slot's block
   bool slot_alt_used[SRTB_B200_RING_SLOTS] = {false};
+  bool slot_sum[SRTB_B200_RING_SLOTS] = {false};  // the slot's block carries the total-intensity sum's header
   int slot_ticket[SRTB_B200_RING_SLOTS] = {0};
   // per-slot outputs: ctx-owned working buffers / pinned series unless the caller supplied its own (submit_block_ex)
   float* slot_stream_buf[SRTB_B200_RING_SLOTS][4] = {};
@@ -287,9 +300,9 @@ int srtb_b200_ctx_create(int device, void* cuda_stream, srtb_b200_ctx** out) {
   e = cudaSetDevice(device);
   if (e == cudaSuccess) e = cudaDeviceGetAttribute(&ctx->sm_count, cudaDevAttrMultiProcessorCount, device);
   if (e == cudaSuccess) e = lane_alloc(&ctx->lane);
-  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_res, sizeof(detect_dev_result) * 4);
-  if (e == cudaSuccess) e = cudaMemset(ctx->d_res, 0, sizeof(detect_dev_result) * 4);
-  if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_res, sizeof(detect_dev_result) * 4 * (1 + SRTB_B200_RING_SLOTS));
+  if (e == cudaSuccess) e = cudaMalloc(&ctx->d_res, sizeof(detect_dev_result) * RES_GROUP);
+  if (e == cudaSuccess) e = cudaMemset(ctx->d_res, 0, sizeof(detect_dev_result) * RES_GROUP);
+  if (e == cudaSuccess) e = cudaMallocHost(&ctx->h_res, sizeof(detect_dev_result) * RES_GROUP * (1 + SRTB_B200_RING_SLOTS));
   if (e != cudaSuccess) {
     const std::string msg = std::string("ctx_create: ") + cudaGetErrorString(e);
     srtb_b200_ctx_destroy(ctx);  // frees whatever was allocated before the failure
@@ -334,6 +347,8 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   cudaFree(ctx->corr_tickets);
   cudaFree(ctx->inc_tab);
   cudaFree(ctx->inc_work);
+  cudaFree(ctx->sum_raw);
+  cudaFree(ctx->sum_mask);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
     cudaFree(ctx->slot_baseband[i]);
     for (auto& p : ctx->slot_stream_buf[i]) cudaFree(p);
@@ -1584,10 +1599,11 @@ static int detect_tail(srtb_b200_ctx* ctx, int slot, const float2* x, size_t tim
                        size_t zero_stride = 0) {
   if (zero_stride == 0) zero_stride = time_count;
   float* const host_series = ctx->host_series_dst ? ctx->host_series_dst + (size_t)slot * SRTB_B200_MAX_BOXCARS * time_count : nullptr;
+  float* const raw = ctx->raw_dst ? ctx->raw_dst + (size_t)slot * time_count : nullptr;
   stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_DETECT_TAIL, 4.0 * (double)chunks * (double)ts_count);
   CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>((ts_count + 31) / 32, (size_t)ctx->sm_count)),
                 dim3(1024), 0, (const float*)ctx->lane.colsum_partial, ts_count, chunks, ctx->series[slot], ctx->lane.acc, x, zero_stride,
-                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0));
+                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0, raw));
   ctx->launches++;
   CK(cudaGetLastError());
   // one CTA per possible boxcar; CTAs beyond n_boxcars (known only on the device) exit at once
@@ -2031,6 +2047,9 @@ static int block_params_for(srtb_b200_ctx* ctx, const srtb_b200_block_config* cf
   p->cfg = cfg;
   p->streams = format_streams(cfg->baseband_format);
   if (!p->streams) return fail(ctx, SRTB_B200_E_UNSUPPORTED, std::string(who) + ": unknown format");
+  if (cfg->signal_detect_sum_streams && p->streams < 2)
+    return fail(ctx, SRTB_B200_E_INVALID,
+                std::string(who) + ": signal_detect_sum_streams needs a format with two or more streams");
   p->N = cfg->baseband_input_count;
   if (p->N < 2 || !is_pow2(p->N))
     return fail(ctx, SRTB_B200_E_SIZE, "[fft] n must be a power of 2, got " + std::to_string(p->N));
@@ -2175,12 +2194,63 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
                         cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length);
 }
 
+// the detector on the total intensity of the block's streams (stream_sum.cuh), on the first lane once every stream's
+// chain has run: mask, sum, then the detector's tail on the summed series, header in d_res[SUM_SLOT]. raw: the streams'
+// raw column sums [4][L]; host_series (optional): the block's pinned series, whose slot `streams` receives the sum's
+// positive series
+static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* bufs, const float* raw,
+                    float* host_series) {
+  const srtb_b200_block_config* cfg = p.cfg;
+  const size_t L = p.L, C = p.batch, reserved = p.reserved(cfg->dm);
+  const size_t ts = (L <= reserved) ? L : L - reserved;
+  if (int rc = detect_prepare(ctx, SUM_SLOT, L, 1)) return rc;
+  if (int rc = ensure(ctx, &ctx->sum_mask, &ctx->sum_mask_bytes, C * (sizeof(float2) + sizeof(uint2)) + sizeof(unsigned)))
+    return rc;
+  float2* const mask = static_cast<float2*>(ctx->sum_mask);
+  uint2* const mis = reinterpret_cast<uint2*>(mask + C);
+  unsigned* const n_mis = reinterpret_cast<unsigned*>(mis + C);
+  stream_sum_inputs in{};
+  for (int s = 0; s < p.streams; s++) {
+    in.x[s] = reinterpret_cast<const float2*>(bufs[s]);
+    in.raw[s] = raw + (size_t)s * L;
+  }
+  CK(cudaMemsetAsync(ctx->d_res + SUM_SLOT, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  stream_sum_mask_kernel<<<1, 1024, 0, ctx->lane.stream>>>(in, p.streams, L, C, mask, mis, n_mis);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  float* const v = ctx->series[SUM_SLOT];
+  CK(launch_pdl(ctx, stream_sum_kernel, dim3(grid_for(ctx, ts, 256)), dim3(256), 0, in, p.streams, L, ts,
+                (const uint2*)mis, (const unsigned*)n_mis, v));
+  ctx->launches++;
+  CK(cudaGetLastError());
+  // the tail counts the mask's zeros (stride 1): the union count. The first lane's ticket and scan buffer are free here:
+  // its own stream's tail has finished in stream order.
+  CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>((C + 1023) / 1024, (size_t)ctx->sm_count)),
+                dim3(1024), 0, (const float*)nullptr, ts, (size_t)0, v, ctx->lane.acc, (const float2*)mask, (size_t)1, C,
+                cfg->signal_detect_channel_threshold, (size_t)cfg->signal_detect_max_boxcar_length,
+                ctx->lane.detect_ticket, ctx->d_res + SUM_SLOT, (size_t)0, (size_t)0, (float*)nullptr));
+  ctx->launches++;
+  CK(cudaGetLastError());
+  unsigned max_nb = 1;
+  for (size_t b = 2; b <= cfg->signal_detect_max_boxcar_length && b < ts && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2)
+    max_nb++;
+  float* const host_out = host_series ? host_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * L : nullptr;
+  CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, v, L, (const float*)ctx->lane.acc, ts,
+                cfg->signal_detect_signal_noise_threshold, ctx->d_res + SUM_SLOT, host_out, (detect_dev_peak*)nullptr,
+                (size_t)0, (size_t)0));
+  ctx->launches++;
+  CK(cudaGetLastError());
+  ctx->slot_time_count[SUM_SLOT] = L;
+  return 0;
+}
+
 // enqueue every stage of one block (no host sync); results land in ctx->h_res[res_base .. res_base + streams) once the
 // lanes reach their D2H copies. bufs[s]: working buffer of stream s (N + 2 floats, 16-byte aligned for the fused
 // routes), which holds the dynamic spectrum [C][L] when the block is done. host_series (optional): pinned host memory
 // that receives positive series. join_lanes: the first lane waits for the second at the end (process_block); the ring
 // leaves the lanes free-running (each copies its own result headers back, *alt_used tells the caller to record a
-// completion event on both).
+// completion event on both). With cfg->signal_detect_sum_streams the first lane then waits for the second on the device
+// and runs sum_tail; its header lands in h_res[res_base + SUM_SLOT].
 static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* d_baseband, size_t baseband_bytes,
                          int res_base, float* const* bufs, float* host_series, bool join_lanes = true,
                          bool* alt_used = nullptr) {
@@ -2188,12 +2258,21 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     srtb_b200_ctx* c;
     ~series_dst_scope() {
       c->host_series_dst = nullptr;
+      c->raw_dst = nullptr;
       c->res_zeroed = false;
       c->pdl_auto = false;
     }
   } series_scope_{ctx};
   ctx->host_series_dst = host_series;
   ctx->pdl_auto = p.N <= ((size_t)1 << 25);
+  const bool sum = p.cfg->signal_detect_sum_streams != 0;
+  if (sum) {
+    const size_t group = (size_t)(res_base / RES_GROUP);
+    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->sum_raw), &ctx->sum_raw_bytes,
+                        (1 + SRTB_B200_RING_SLOTS) * 4 * p.L * sizeof(float)))
+      return rc;
+    ctx->raw_dst = ctx->sum_raw + group * 4 * p.L;
+  }
   // the data streams of a block are independent: odd ones go to the context's second lane (per-stage timing wants the
   // kernels alone, so it keeps one lane)
   const bool two_lanes = ctx->lanes >= 2 && p.streams >= 2 && !ctx->stats_on;
@@ -2245,14 +2324,17 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     if (alt) lane_swap(ctx);
     if (rc) return rc;
   }
-  if (two_lanes) {
-    if (join_lanes) {
-      CK(cudaEventRecord(ctx->lane_join, ctx->alt.stream));
-      CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->lane_join, 0));
-    }
-  } else {
+  if (two_lanes && (join_lanes || sum)) {
+    CK(cudaEventRecord(ctx->lane_join, ctx->alt.stream));
+    CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->lane_join, 0));
+  }
+  if (!two_lanes)
     CK(cudaMemcpyAsync(ctx->h_res + res_base, ctx->d_res, sizeof(detect_dev_result) * p.streams, cudaMemcpyDeviceToHost,
                        ctx->lane.stream));
+  if (sum) {
+    if (int rc = sum_tail(ctx, p, bufs, ctx->raw_dst, host_series)) return rc;
+    CK(cudaMemcpyAsync(ctx->h_res + res_base + SUM_SLOT, ctx->d_res + SUM_SLOT, sizeof(detect_dev_result),
+                       cudaMemcpyDeviceToHost, ctx->lane.stream));
   }
   return 0;
 }
@@ -2272,6 +2354,10 @@ extern "C" int srtb_b200_process_block_device(srtb_b200_ctx* ctx, const srtb_b20
   for (int s = 0; s < p.streams; s++)
     if (int rc = detect_collect(ctx, s, h_results + s, h_series ? h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
                                 copy_all))
+      return rc;
+  if (cfg->signal_detect_sum_streams)
+    if (int rc = detect_collect(ctx, SUM_SLOT, h_results + p.streams,
+                                h_series ? h_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * p.L : nullptr, copy_all))
       return rc;
   return p.streams;
 }
@@ -2334,6 +2420,8 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
   API_LOCK(ctx);
   if (!ctx || !cfg || !baseband || !h_dms || !h_results || n_dm == 0)
     return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: bad argument");
+  if (cfg->signal_detect_sum_streams)
+    return fail(ctx, SRTB_B200_E_UNSUPPORTED, "dm_sweep: signal_detect_sum_streams is not supported by the DM sweep");
   CK(cudaSetDevice(ctx->device));
   block_params p;
   if (int rc = block_params_for(ctx, cfg, "dm_sweep", &p)) return rc;
@@ -2609,7 +2697,7 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   // the series are already in place: no partial sums (partial == nullptr); one CTA per trial zero-counts and scans
   colsum_final_scan_kernel<<<dim3(1, (unsigned)n_dm), 1024, 0, st>>>(
       nullptr, T, 0, d_series, d_acc, static_cast<const float2*>(d_spectrum), time_count, chan_count, channel_threshold,
-      max_boxcar_length, d_ticket, d_res, series_stride, T);
+      max_boxcar_length, d_ticket, d_res, series_stride, T, nullptr);
   ctx->launches++;
   CK(cudaGetLastError());
   detect_boxcar_kernel<true><<<dim3(max_nb, (unsigned)n_dm), 1024, 0, st>>>(
@@ -2684,7 +2772,7 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
   }
   float* h_series = outputs ? outputs->h_series : nullptr;
   if (!h_series) {
-    const size_t need = (size_t)p.streams * SRTB_B200_MAX_BOXCARS * p.L;
+    const size_t need = (size_t)(p.streams + (cfg->signal_detect_sum_streams ? 1 : 0)) * SRTB_B200_MAX_BOXCARS * p.L;
     if (ctx->slot_h_series_elems[slot] < need) {
       if (int rc = sync_lanes(ctx)) return rc;
       if (ctx->slot_h_series[slot]) CK(cudaFreeHost(ctx->slot_h_series[slot]));
@@ -2709,10 +2797,11 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
     d_baseband = ctx->slot_baseband[slot];
   }
   bool alt_used = false;
-  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, 4 * (1 + slot), bufs, h_series, /*join_lanes=*/false,
+  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, RES_GROUP * (1 + slot), bufs, h_series, /*join_lanes=*/false,
                              &alt_used))
     return rc;
   ctx->slot_streams[slot] = p.streams;
+  ctx->slot_sum[slot] = cfg->signal_detect_sum_streams != 0;
   CK(cudaEventRecord(ctx->slot_done[slot], ctx->lane.stream));
   ctx->slot_alt_used[slot] = alt_used;
   if (alt_used) {
@@ -2755,7 +2844,9 @@ extern "C" int srtb_b200_collect_block_ex(srtb_b200_ctx* ctx, int ticket, srtb_b
     api_lock_.lock();
   }
   const int streams = ctx->slot_streams[slot];
-  std::memcpy(h_results, ctx->h_res + 4 * (1 + slot), sizeof(srtb_b200_detect_result) * streams);
+  std::memcpy(h_results, ctx->h_res + RES_GROUP * (1 + slot), sizeof(srtb_b200_detect_result) * streams);
+  if (ctx->slot_sum[slot])
+    std::memcpy(h_results + streams, ctx->h_res + RES_GROUP * (1 + slot) + SUM_SLOT, sizeof(srtb_b200_detect_result));
   if (h_series) *h_series = ctx->slot_out_series[slot];
   if (d_spectrum)
     for (int s = 0; s < 4; s++) d_spectrum[s] = s < streams ? ctx->slot_out_spectrum[slot][s] : nullptr;

@@ -63,6 +63,8 @@ class BlockConfig(C.Structure):
         ("signal_detect_max_boxcar_length", C.c_uint64),
         ("rfi_freq_pairs", C.POINTER(C.c_float)),
         ("n_rfi_freq_pairs", C.c_uint64),
+        # non-zero: one more result per block, the detector on the streams' total intensity (include/srtb_b200.h)
+        ("signal_detect_sum_streams", C.c_int32),
     ]
 
 
@@ -194,6 +196,7 @@ class Context:
             raise SrtbError(rc, self.lib.srtb_b200_last_error(None).decode())
         self.h = h
         self.device = device
+        self._sum_tickets = {}  # ring ticket -> submitted with signal_detect_sum_streams
 
     def close(self):
         if getattr(self, "h", None):
@@ -281,10 +284,12 @@ class Context:
 
     def process_block(self, cfg: BlockConfig, baseband, nbytes: int, h_series=None, copy_all: bool = False,
                       on_device: bool = False):
-        res = (DetectResult * 4)()
+        """results per stream, then the total-intensity sum's when cfg.signal_detect_sum_streams is set (h_series then
+        has streams + 1 slots)"""
+        res = (DetectResult * 5)()
         fn = self.lib.srtb_b200_process_block_device if on_device else self.lib.srtb_b200_process_block
         n = self._ck(fn(self.h, C.byref(cfg), _ptr(baseband), nbytes, res, _ptr(h_series), int(copy_all)))
-        return [res[i] for i in range(n)]
+        return [res[i] for i in range(n + (1 if cfg.signal_detect_sum_streams else 0))]
 
     def process_block_dm_sweep(self, cfg: BlockConfig, baseband, nbytes: int, dms, on_device: bool = False,
                                outputs: bool = False, h_series=None, d_spectrum=None):
@@ -356,36 +361,48 @@ class Context:
         idx_a = np.array([list(peaks[d].peak_index)[:nb] for d in range(n_dm)], np.uint64).reshape(n_dm, nb)
         return results, (snr_a, idx_a), int(best.value), h_series
 
+    def _submitted(self, cfg: BlockConfig, ticket: int) -> int:
+        self._sum_tickets[ticket] = bool(cfg.signal_detect_sum_streams)
+        return ticket
+
     def submit_block(self, cfg: BlockConfig, h_baseband, nbytes: int) -> int:
         """pipelined ingest: H2D on the copy stream overlaps the previous block's compute"""
-        return self._ck(self.lib.srtb_b200_submit_block(self.h, C.byref(cfg), _ptr(h_baseband), nbytes))
+        return self._submitted(cfg, self._ck(self.lib.srtb_b200_submit_block(self.h, C.byref(cfg), _ptr(h_baseband),
+                                                                             nbytes)))
 
     def submit_block_device(self, cfg: BlockConfig, d_baseband, nbytes: int) -> int:
-        return self._ck(self.lib.srtb_b200_submit_block_device(self.h, C.byref(cfg), _ptr(d_baseband), nbytes))
+        return self._submitted(cfg, self._ck(self.lib.srtb_b200_submit_block_device(self.h, C.byref(cfg),
+                                                                                    _ptr(d_baseband), nbytes)))
+
+    def _sum_result(self, ticket: int) -> int:
+        return 1 if self._sum_tickets.pop(ticket, False) else 0
 
     def collect_block(self, ticket: int):
-        res = (DetectResult * 4)()
+        """results per stream, then the sum's when the block was submitted with signal_detect_sum_streams"""
+        res = (DetectResult * 5)()
         n = self._ck(self.lib.srtb_b200_collect_block(self.h, ticket, res))
-        return [res[i] for i in range(n)]
+        return [res[i] for i in range(n + self._sum_result(ticket))]
 
     def submit_block_ex(self, cfg: BlockConfig, baseband, nbytes: int, on_device: bool = False, d_spectrum=None,
                         h_series=None) -> int:
         """ring submission with caller-owned outputs: d_spectrum = per-stream device buffers of N + 2 floats (the
-        dynamic spectrum stays there), h_series = pinned host buffer [streams][MAX_BOXCARS][L] for positive series"""
+        dynamic spectrum stays there), h_series = pinned host buffer [streams][MAX_BOXCARS][L] for positive series
+        ([streams + 1][MAX_BOXCARS][L] with cfg.signal_detect_sum_streams)"""
         out = BlockOutputs()
         for i, t in enumerate(d_spectrum or []):
             out.d_spectrum[i] = _ptr(t)
         out.h_series = _ptr(h_series)
-        return self._ck(self.lib.srtb_b200_submit_block_ex(self.h, C.byref(cfg), _ptr(baseband), nbytes,
-                                                           int(on_device), C.byref(out)))
+        return self._submitted(cfg, self._ck(self.lib.srtb_b200_submit_block_ex(self.h, C.byref(cfg), _ptr(baseband),
+                                                                                nbytes, int(on_device), C.byref(out))))
 
     def collect_block_ex(self, ticket: int):
-        """(results, host pointer of the series buffer, [device pointers of the streams' dynamic spectra])"""
-        res = (DetectResult * 4)()
+        """(results, host pointer of the series buffer, [device pointers of the streams' dynamic spectra]); results end
+        with the sum's when the block was submitted with signal_detect_sum_streams"""
+        res = (DetectResult * 5)()
         series = C.c_void_p()
         spec = (C.c_void_p * 4)()
         n = self._ck(self.lib.srtb_b200_collect_block_ex(self.h, ticket, res, C.byref(series), spec))
-        return [res[i] for i in range(n)], series.value, [spec[i] for i in range(n)]
+        return [res[i] for i in range(n + self._sum_result(ticket))], series.value, [spec[i] for i in range(n)]
 
     def debug_set_submit_count(self, value: int):
         self._ck(self.lib.srtb_b200_debug_set_submit_count(self.h, value))

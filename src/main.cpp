@@ -89,11 +89,21 @@ struct round_robin_out_functor {
 };
 
 /** sink wrapper: counts finished works so file replays know when everything has drained */
+// signal_detect_sum_polarizations: one line per block with the total-intensity detector's counts
+void log_sum(const srtb::work::write_signal_work& w) {
+  if (!w.carries_sum) return;
+  std::string counts;
+  for (size_t c : w.sum_signal_count) counts += (counts.empty() ? "" : ",") + std::to_string(c);
+  SRTB_LOGI << " [main] " << "block " << w.timestamp << ": total intensity " << (w.sum_positive ? "positive" : "negative")
+            << ", masked channels " << w.sum_zero_count << ", signal counts per boxcar [" << counts << "]";
+}
+
 template <typename Sink>
 struct counting_sink {
   std::shared_ptr<Sink> sink;
   std::shared_ptr<std::atomic<uint64_t>> done;
   std::optional<srtb::work::dummy_work> operator()(std::stop_token st, srtb::work::write_signal_work w) {
+    log_sum(w);
     (*sink)(st, std::move(w));
     (*done)++;
     return srtb::work::dummy_work{};
@@ -120,6 +130,7 @@ std::string take_option(std::vector<std::string>& args, const std::string& name,
 struct discard_sink {
   std::shared_ptr<std::atomic<uint64_t>> done, positives;
   std::optional<srtb::work::dummy_work> operator()(std::stop_token, srtb::work::write_signal_work w) {
+    log_sum(w);
     if (!w.time_series.empty()) (*positives)++;
     (*done)++;
     return srtb::work::dummy_work{};
@@ -201,6 +212,13 @@ int main(int argc, char** argv) {
   if (cfg.gui_enable && (cfg.gui_pixmap_width == 0 || cfg.gui_pixmap_height == 0)) {
     std::fprintf(stderr, "srtb_b200: gui_enable needs a non-zero gui_pixmap_width and gui_pixmap_height (got %zu x %zu)\n",
                  (size_t)cfg.gui_pixmap_width, (size_t)cfg.gui_pixmap_height);
+    return 2;
+  }
+  try {
+    srtb::program_options::check_sum_polarizations(
+        cfg, srtb::io::backend_registry::get_data_stream_count(cfg.baseband_format_type));
+  } catch (const std::exception& e) {
+    std::fprintf(stderr, "srtb_b200: %s\n", e.what());
     return 2;
   }
 
