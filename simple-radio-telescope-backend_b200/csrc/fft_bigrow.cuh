@@ -51,6 +51,9 @@ struct bigrow {
   static constexpr size_t off_mbar = off_tab + (size_t)TABN * sizeof(float2);
   static constexpr size_t off_red = off_mbar + 24 * 8;   // 3 buffers x 8 chunk barriers
   static constexpr size_t bytes = off_red + 4 * 32 * sizeof(float);
+  // the R2C row sweep (SRC = 2) adds one double per thread (its group's Σ|X|^2 over the rows, handed over by whichever
+  // CTA summed it) and the mbarrier on which the partner CTA releases half buffer B
+  static constexpr size_t bytes_r2c = bytes + NT * sizeof(double) + 8;
   // the sweep-order load (SRC = 1) lands 128-byte-swizzled tensor boxes, whose destinations must be 1024-byte aligned:
   // half buffers rounded up to 1 KiB, and 1 KiB more to align the base of the dynamic shared memory
   static constexpr int HALF_SW = (HALF + 127) / 128 * 128;
@@ -85,6 +88,18 @@ __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t a) {
   float4 v;
   asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a) : "memory");
   return v;
+}
+// arrive on an mbarrier of a CTA of the cluster without waiting for this thread's earlier stores
+__device__ __forceinline__ void mbar_arrive_dsmem_relaxed(uint32_t a) {
+  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(a) : "memory");
+}
+__device__ __forceinline__ double ld_dsmem_f64(uint32_t a) {
+  double v;
+  asm volatile("ld.shared::cluster.f64 %0, [%1];" : "=d"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_dsmem_f64(uint32_t a, double v) {
+  asm volatile("st.shared::cluster.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory");
 }
 
 // R2C split of bin k = k1 + P k2 from Z[k] and Z[M - k] (w = e^{-i pi k / M}):
@@ -159,7 +174,8 @@ __device__ __forceinline__ void bigrow_stage_table(float2* __restrict__ p, const
 //       before it stores the standard layout (tools/proto_r2c_sweep_order.py);
 //   2 = the R2C row sweep, run as clusters of two CTAs: nrows = P rows of the scratch `in`, the cluster's CTAs take
 //       rows i and P - i (cluster 0: rows 0 and P / 2, each its own mirror), transform them forward and store the split
-//       spectrum X[k1 + P k2] channel-blocked to `out`, reading the mirror row's Z through distributed shared memory.
+//       spectrum X[k1 + P k2] channel-blocked to `out`, each CTA splitting half of the pair's mirror pairs for both rows
+//       and reading their mirror halves through distributed shared memory.
 // The body is shared by three entry points: fft_bigrow_kernel (SRC = 0) and the two kernels of the sweep-order R2C
 // route below it.
 template <int LOGL, bool FWD, bool SK, int CHIRP, int SRC>
@@ -197,8 +213,21 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
     }
   };
 
+  // SRC = 2: per thread t of a one-group-per-thread split, its group's Σ|X|^2 over the rows; the mbarrier on which the
+  // CTA holding the mirror row signals that it has read this CTA's half buffer B. Their addresses are formed afresh at
+  // each use (volatile), not kept live through the butterflies (a spill)
+  auto gsum_at = [&]() {
+    unsigned o;
+    asm volatile("mov.u32 %0, %1;" : "=r"(o) : "n"((unsigned)C::bytes));
+    return reinterpret_cast<double*>(sm + o);
+  };
+  auto bfree_at = [&]() { return reinterpret_cast<uint64_t*>(gsum_at() + NT); };
   for (int i = tid; i < C::TABN; i += NT) T0[i] = __ldg(&tabs[i]);
   if (tid < 24) mbar_init(&mbar[tid], 1);
+  if constexpr (SRC == 2) {
+    gsum_at()[tid] = 0.0;
+    if (tid == 0) mbar_init(bfree_at(), 1);
+  }
   if (tid == 0) fence_mbar_init();
   __syncthreads();
   // this thread's 32 column-sum cells: time samples kcell + 256 (c >> 1) + 4096 (c & 1) of the CTA's partial row,
@@ -220,10 +249,13 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
         tma_load_2d(hbuf + hb * HALF + lane * 2048, tmap, 0, (int)(row * (L / 16) + (L / 32) * which + 128 * lane),
                     &mbar[hb * 8 + lane]);
       }
-    } else if (lane < 8) {
-      mbar_expect_tx(&mbar[hb * 8 + lane], (uint32_t)(B1 * sizeof(float2)));
-      bulk_g2s(hbuf + hb * HALF + lane * S1, in + (size_t)row * L + (size_t)(which * 8 + lane) * B1,
-               (uint32_t)(B1 * sizeof(float2)), &mbar[hb * 8 + lane]);
+    } else {
+      const int c = tid_row() & 31;  // the lane
+      if (c < 8) {
+        mbar_expect_tx(&mbar[hb * 8 + c], (uint32_t)(B1 * sizeof(float2)));
+        bulk_g2s(hbuf + hb * HALF + c * S1, in + (size_t)row * L + (size_t)(which * 8 + c) * B1,
+                 (uint32_t)(B1 * sizeof(float2)), &mbar[hb * 8 + c]);
+      }
     }
   };
 
@@ -242,6 +274,12 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
       return blockIdx.x + it * gridDim.x;
     }
   };
+  // SRC = 2: rows 0 and P / 2 are their own mirrors; the CTA holding the mirror row of `r` (the partner, or this one)
+  auto self_paired = [&](unsigned r) { return r == 0 || 2 * r == nrows; };
+  auto mirror_rank = [&](unsigned r) { return self_paired(r) ? crank : (crank ^ 1); };
+  // SRC = 2: thread t of the split holds group t & ~8 (pd0 < 8) of a one-group-per-thread map, whose thread indices
+  // the Σ|X|^2 fold keeps; its mirror group (15 - pd0, 15 - pd1, 1 - sel) is that map's thread NT - 1 - (t & ~8)
+  auto mirror_slot = [](int t) { return NT - 1 - (t & ~8); };
   auto live = [&](unsigned it) -> bool {
     if constexpr (SRC == 2) return (blockIdx.x >> 1) + it * (gridDim.x >> 1) < nrows / 2;
     else return row_of(it) < nrows;
@@ -269,7 +307,7 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
     }
     __syncthreads();
   }
-  double psum = 0.0;  // SRC = 2: this thread's Σ|X|^2
+  double psum = 0.0;  // SRC = 2: Σ|X|^2 of the thread's own group (threads h = 1 of the split)
   if (wid == 0) {
     if (live(0)) {
       issue_half(row_of(0), 0, 0);
@@ -394,7 +432,8 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
     __syncthreads();
     // ---- stage 1: block d0, butterflies over d1 (stride S2), pair of [0, B2)
     {
-      const int d0 = tid / (B2 / 2), jp = tid % (B2 / 2);
+      const int t = tid_row();
+      const int d0 = t / (B2 / 2), jp = t % (B2 / 2);
       bigrow_stage_table<FWD, S2, B2>(half_of(d0) + 2 * jp, T1 + 2 * jp);
     }
     __syncthreads();
@@ -476,58 +515,98 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
     }
     if (live(it + 1)) prefetch_phase(row_of(it + 1));
     if constexpr (SRC == 2) {
-      // ---- R2C split and channel-blocked store of row k1 = row: X[k1 + P k2] from Z[k1][k2] and the mirror Z[M - k],
-      // which the partner CTA holds (itself for rows 0 and P / 2). Lanes as in pass 2 below.
+      // ---- R2C split and channel-blocked store of the pair: X[k1 + P k2] of row k1 = row and of its mirror row prow
+      // (P - row; row itself for rows 0 and P / 2, which the partner CTA does not share). X[k] and X[M - k] come from
+      // the same two inputs Z[k], Z[M - k], so each pair is read once and split once for both bins: this CTA takes the
+      // pairs whose own bin has d0 < 8 (its half buffer A, local) and reads their mirrors, d0 >= 8, from half buffer B
+      // of the mirror row (remote: 64 KiB per row). The groups are those of a one-group-per-thread map, thread
+      // (pd0, pd1, sel) holding 32 bins: k2 = pd0 + 16 pd1 + 256 i2 + 4096 d3, d3 = 2 sel, 2 sel + 1. A thread here
+      // takes group (pd0 < 8, pd1, sel) at i2 = 0..7 (h = 0) or 15..8 (h = 1), and the mirror group
+      // (15 - pd0, 15 - pd1, 1 - sel) at 15 - i2 (tools/proto_r2c_sweep_order.py, paired_split). For k1 != 0 the mirror
+      // of k2 is L - 1 - k2: every digit complemented, (d0, d1, d2, d3) -> (15 - d0, 15 - d1, 15 - d2, 3 - d3), so the
+      // mirror group's 16-byte pair at 15 - i2 holds the two mirrors with its halves swapped.
+      const unsigned prow = self_paired(row) ? row : nrows - row, prank = mirror_rank(row);
       const int t = tid_row(), lane = t & 31, wid = t >> 5;
-      const int pd0 = lane & 15, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
-      const float2* const base = half_of(pd0) + pd1 * S2 + 2 * sel;
-      const unsigned prank = (row == 0 || 2 * row == nrows) ? crank : (crank ^ 1);
-      // for k1 != 0 the mirror of k2 is L - 1 - k2: every digit complemented, (d0, d1, d2, d3) -> (15 - d0, 15 - d1,
-      // 15 - d2, 3 - d3), i.e. the 16-byte pair at sel' = 1 - sel with its halves swapped
-      const uint32_t mbase = dsmem_addr(half_of(15 - pd0) + (15 - pd1) * S2 + 2 * (1 - sel), prank);
-      const int kb = pd0 + 16 * pd1 + 4096 * (2 * sel);  // k2 of d2 = 0, d3 = 2 sel
-      float2 wb;  // e^{-i pi (k1 + P kb) / M}; both fractions are exact in fp32
+      const int pd0 = lane & 7, h = (lane >> 3) & 1, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
+      const float2* const base = bufA + pd0 * S1 + pd1 * S2 + 2 * sel;
+      const uint32_t mbase = dsmem_addr(bufB + (7 - pd0) * S1 + (15 - pd1) * S2 + 2 * (1 - sel), prank);
+      const int kb = pd0 + 16 * pd1 + 4096 * (2 * sel);                   // k2 of d2 = 0, d3 = 2 sel
+      const int kbm = (15 - pd0) + 16 * (15 - pd1) + 4096 * (2 * (1 - sel));  // the same of the mirror group
+      float2 wb, wbm;  // e^{-i pi (k1 + P kb) / M} of each group; both fractions are exact in fp32
       {
         float sn, cs;
         sincospif(-((float)row / ((float)nrows * (float)L) + (float)kb / (float)L), &sn, &cs);
         wb = make_float2(cs, sn);
+        sincospif(-((float)prow / ((float)nrows * (float)L) + (float)kbm / (float)L), &sn, &cs);
+        wbm = make_float2(cs, sn);
       }
       const float2* const htw = reinterpret_cast<const float2*>(red);
       auto pos = [&](int k) {  // shared-memory position of natural-order k2 (pass 2's digit map)
         return half_of(k & 15) + ((k >> 4) & 15) * S2 + ((k >> 8) & 15) * R3 + (k >> 12);
       };
       // X[k1 + P k2] goes to (k2 >> 3) L + 8 k1 + (k2 & 7): channel k2 >> 3 (L = 8 P bins) is one contiguous range,
-      // the order of the phase table and of the waterfall kernel's load. Lanes 2m and 2m + 1 hold k2 and k2 + 1 (kb even
-      // and odd): they trade halves, and each stores a 16-byte pair, the even lane at d3 = 2 sel, the odd one at
-      // d3 = 2 sel + 1. A warp's store covers eight 64-byte pieces; rows 2m and 2m + 1 fill the two halves of each line.
+      // the order of the phase table and of the waterfall kernel's load. Lanes 2m and 2m + 1 hold k2 and k2 + 1 (pd0 even
+      // and odd; of the mirror groups, odd and even): they trade halves, and each stores a 16-byte pair, the even one at
+      // d3 = 2 sel, the odd one at d3 = 2 sel + 1. Eight lanes store two whole 64-byte pieces; rows 2m and 2m + 1 fill
+      // the two halves of each line.
       const unsigned odd = lane & 1;
-      const int ks = kb + (int)odd * 4095;  // k2 of the pair's first element (i2 = 0)
+      const int ks = kb + (int)odd * 4095, ksm = kbm + (int)(odd ^ 1) * 4095;  // k2 of the stored pair's first element
       float2* const o = out + (size_t)(ks >> 3) * L + 8 * (size_t)row + (ks & 7);
-      float ps = 0.f;
-#pragma unroll 4
-      for (int i2 = 0; i2 < 16; i2++) {
+      float2* const om = out + (size_t)(ksm >> 3) * L + 8 * (size_t)prow + (ksm & 7);
+      auto store_pair = [&](float2* p, unsigned od, float2 x0, float2 x1) {
+        const float2 mine = od ? x0 : x1;
+        const float2 theirs = make_float2(__shfl_xor_sync(0xffffffffu, mine.x, 1), __shfl_xor_sync(0xffffffffu, mine.y, 1));
+        *reinterpret_cast<float4*>(p) = od ? make_float4(theirs.x, theirs.y, x1.x, x1.y) : make_float4(x0.x, x0.y, theirs.x, theirs.y);
+      };
+      auto norm2 = [](float2 x0, float2 x1) { return (x0.x * x0.x + x0.y * x0.y) + (x1.x * x1.x + x1.y * x1.y); };
+      // Σ|X|^2 of each group is the fp32 sum over i2 = 0..15 in that order: h = 0 sums its own group's i2 = 0..7 and
+      // h = 1 the mirror group's (15 - i2 ascends as i2 descends); each keeps the other group's eight terms and adds
+      // them, i2 ascending, to the partial its lane + 8 hands over
+      float seq = 0.f, terms[8];
+#pragma unroll
+      for (int j = 0; j < 8; j++) {
+        const int i2 = h ? 15 - j : j, im = 15 - i2;
         const float4 q = *reinterpret_cast<const float4*>(base + i2 * R3);
-        float2 m0, m1;
+        const float4 r = ld_dsmem_f4(mbase + (uint32_t)(im * R3 * sizeof(float2)));
+        float2 m0, m1, mm0, mm1;  // the mirrors of q's and of r's two elements
         if (row != 0) {
-          const float4 m = ld_dsmem_f4(mbase + (uint32_t)((15 - i2) * R3 * sizeof(float2)));
-          m0 = make_float2(m.z, m.w);
-          m1 = make_float2(m.x, m.y);
+          m0 = make_float2(r.z, r.w);
+          m1 = make_float2(r.x, r.y);
+          mm0 = make_float2(q.z, q.w);
+          mm1 = make_float2(q.x, q.y);
         } else {  // row 0 pairs k2 with (L - k2) mod L, in this CTA
-          const int k0 = kb + 256 * i2;
+          const int k0 = kb + 256 * i2, km0 = kbm + 256 * im;
           m0 = *pos((L - k0) & (L - 1));
           m1 = *pos((L - k0 - 4096) & (L - 1));
+          mm0 = *pos((L - km0) & (L - 1));
+          mm1 = *pos((L - km0 - 4096) & (L - 1));
         }
         const float2 w0 = c_mul(wb, htw[i2]);
         const float2 w1 = c_mul(w0, make_float2(0.70710678118654752440f, -0.70710678118654752440f));  // k2 + L / 4
+        const float2 v0 = c_mul(wbm, htw[im]);
+        const float2 v1 = c_mul(v0, make_float2(0.70710678118654752440f, -0.70710678118654752440f));
         const float2 x0 = r2c_split_point(make_float2(q.x, q.y), m0, w0);
         const float2 x1 = r2c_split_point(make_float2(q.z, q.w), m1, w1);
-        const float2 mine = odd ? x0 : x1;
-        const float2 theirs = make_float2(__shfl_xor_sync(0xffffffffu, mine.x, 1), __shfl_xor_sync(0xffffffffu, mine.y, 1));
-        *reinterpret_cast<float4*>(o + (size_t)i2 * (32 * L)) =
-            odd ? make_float4(theirs.x, theirs.y, x1.x, x1.y) : make_float4(x0.x, x0.y, theirs.x, theirs.y);
-        ps += (x0.x * x0.x + x0.y * x0.y) + (x1.x * x1.x + x1.y * x1.y);
+        const float2 y0 = r2c_split_point(make_float2(r.x, r.y), mm0, v0);
+        const float2 y1 = r2c_split_point(make_float2(r.z, r.w), mm1, v1);
+        store_pair(o + (size_t)i2 * (32 * L), odd, x0, x1);
+        store_pair(om + (size_t)im * (32 * L), odd ^ 1, y0, y1);
+        const float tx = norm2(x0, x1), ty = norm2(y0, y1);
+        seq += h ? ty : tx;
+        terms[j] = h ? tx : ty;
       }
-      psum += (double)ps;
+      float gs = __shfl_xor_sync(0xffffffffu, seq, 8);
+#pragma unroll
+      for (int j = 7; j >= 0; j--) gs += terms[j];
+      // Σ over rows in row order, in double, of each group: h = 1 adds its own group's; h = 0 the mirror group's, which
+      // belongs to the partner from its first row on. Only cluster 0 has rows 0 and P / 2, at it = 0: there the mirror
+      // group is this CTA's own, so its partial goes to gsum here, and the partner thread continues that sum from it
+      if (h || !self_paired(row)) {
+        if (!h && it == (blockIdx.x < 2 ? 1u : 0u)) psum = ld_dsmem_f64(dsmem_addr(gsum_at() + mirror_slot(t), prank));
+        psum += (double)gs;
+      } else {
+        gsum_at()[mirror_slot(t)] = (double)gs;
+      }
     } else {
     // ---- pass 2: natural-order store. lane -> (d0, d1 bit 0): 32 consecutive output indices per instruction
       const int pd0 = lane & 15, pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3;
@@ -557,20 +636,41 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
         }
       }
     }
-    // the row's buffers are free (SRC = 2: once the partner has read them too): second half of the next row, first half
-    // of the one after
-    if constexpr (SRC == 2) cluster_sync_all();
-    else __syncthreads();
-    if (wid == 0) {
+    // the row's buffers are free: second half of the next row, first half of the one after
+    __syncthreads();
+    if constexpr (SRC == 2) {
+      // The split read buffer A only here and buffer B only in the CTA of the mirror row (here too for rows 0 and P / 2),
+      // so each is released on its own, and no cluster barrier waits for the split's stores. A, which takes the next
+      // row's second half (stage 0 needs it first), is free after the barrier above. B is free once the mirror row's
+      // CTA has arrived on bfree, which it does after its own barrier above: its remote reads of B have returned their
+      // values by then (they were consumed by the split), and the copy into B is issued only after the wait. Each CTA
+      // gets one arrive per row (from its partner, or from itself for rows 0 and P / 2), so bfree completes phase `it`
+      // in row `it`; the partner cannot arrive for row it + 1 before both CTAs pass the cluster barrier of row it + 1.
+      if (wid == 0) {
+        if (live(it + 1)) issue_half(row_of(it + 1), 1, hA);  // B of row it + 1 is A of row it
+        if (lane == 0) mbar_arrive_dsmem_relaxed(dsmem_addr(bfree_at(), mirror_rank(row)));
+        if (live(it + 2)) {
+          mbar_wait(bfree_at(), it & 1);
+          issue_half(row_of(it + 2), 0, hB);  // A of row it + 2 is B of row it
+        }
+      }
+    } else if (wid == 0) {
       if (live(it + 1)) issue_half(row_of(it + 1), 1, hA);  // B of row it + 1 is A of row it
       if (live(it + 2)) issue_half(row_of(it + 2), 0, hB);  // A of row it + 2 is B of row it
     }
   }
   if constexpr (SRC == 2) {
-    // Σ|X|^2: per-CTA partial, then the last CTA folds the partials in index order (as r2c_col0_fixup_kernel does)
+    // Σ|X|^2: the h = 1 threads store their own groups' sums, the h = 0 threads hand the mirror groups' sums to the
+    // partner (not after a CTA with only a self-paired row: its mirror group's sum is already in gsum); the cluster
+    // barrier makes those visible and keeps both CTAs' shared memory alive past the last remote access. Then thread t holds group t's sum, as a one-group-per-thread split would: per-CTA
+    // partial, then the last CTA folds the partials in index order (as r2c_col0_fixup_kernel does)
+    double* const gsum = gsum_at();
+    if ((tid >> 3) & 1) gsum[tid & ~8] = psum;
+    else if (blockIdx.x >= 2 || live(1)) st_dsmem_f64(dsmem_addr(gsum + mirror_slot(tid), crank ^ 1), psum);
+    cluster_sync_all();
     double* const redd = reinterpret_cast<double*>(red + 64);
     unsigned* const last = reinterpret_cast<unsigned*>(red + 96);
-    double v = psum;
+    double v = gsum[tid];
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     if (lane == 0) redd[wid] = v;

@@ -1090,13 +1090,13 @@ static int launch_r2c_rows(srtb_b200_ctx* ctx, const float2* s, float2* out, siz
   attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[1].val.programmaticStreamSerializationAllowed = 1;
   cfg.blockDim = dim3(C::NT);
-  cfg.dynamicSmemBytes = C::bytes;
+  cfg.dynamicSmemBytes = C::bytes_r2c;
   cfg.stream = ctx->lane.stream;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
   const void* key = reinterpret_cast<const void*>(kern);
   if (!ctx->configured.count(key)) {
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::bytes));
+    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::bytes_r2c));
     int clusters = 0;
     cfg.gridDim = dim3(2 * (unsigned)ctx->sm_count);
     CK(cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg));

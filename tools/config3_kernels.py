@@ -6,8 +6,9 @@ submitted device-resident through the ring API as bench.py does; kernel times co
 activities) in a run of its own after a warm-up.
 
 For each kernel: launches per stream per block, µs per launch, the bytes it must move per launch (HBM, from the
-shapes), GB/s and the share of the 3.35 TB/s data-sheet bandwidth. The card's name and power limit are read in the
-same run.  usage: config3_kernels.py [--steps K] [--warmup W] [--json PATH]"""
+shapes), GB/s and the share of the 3.35 TB/s data-sheet bandwidth. A control row times the row sweep's body without
+the split or the cluster: the forward C2C of the same [P][L] rows in place (values are not looked at). The card's name
+and power limit are read in the same run.  usage: config3_kernels.py [--steps K] [--warmup W] [--json PATH]"""
 import argparse
 import json
 import os
@@ -50,6 +51,40 @@ def bytes_per_launch(name, n):
     return None                       # zap ranges and the detector tail: no streaming traffic of their own
 
 
+def kernel_times(prof):
+    """kernel name -> [launches, total µs] of the CUDA activities of a profile"""
+    acc = defaultdict(lambda: [0, 0.0])
+    for e in prof.events():
+        if e.device_type != torch.autograd.DeviceType.CUDA or not e.device_time:
+            continue
+        name = e.name.split("(")[0].split("<")[0].replace("void ", "").replace("srtb_b200::", "").strip()
+        acc[name][0] += 1
+        acc[name][1] += e.device_time
+    return acc
+
+
+def control_c2c(n, steps, warmup):
+    """µs per launch of the row sweep's body without the split or the cluster: the forward C2C of the same [P][L]
+    rows (fft_bigrow_kernel<14, true, false, 0>, in place, 8 + 8 bytes per point), timed the same way"""
+    L = 1 << 14
+    P = n // 2 // L
+    x = torch.randn(P * L * 2, device="cuda", dtype=torch.float32)   # 16-byte aligned: the one-sweep route
+    ctx = srtb_b200.Context(torch.cuda.current_device(), torch.cuda.current_stream().cuda_stream)
+    try:
+        for _ in range(warmup):
+            ctx.fft_c2c(x, L, P, +1)
+        torch.cuda.synchronize()
+        from torch.profiler import ProfilerActivity, profile
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            for _ in range(steps):
+                ctx.fft_c2c(x, L, P, +1)
+            torch.cuda.synchronize()
+    finally:
+        ctx.close()
+    cnt, us = kernel_times(prof)["fft_bigrow_kernel"]
+    return us / cnt
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=20)
@@ -69,13 +104,9 @@ def main():
         H.drain()
         torch.cuda.synchronize()
     H.close()
-    acc = defaultdict(lambda: [0, 0.0])
-    for e in prof.events():
-        if e.device_type != torch.autograd.DeviceType.CUDA or not e.device_time:
-            continue
-        name = e.name.split("(")[0].split("<")[0].replace("void ", "").replace("srtb_b200::", "").strip()
-        acc[name][0] += 1
-        acc[name][1] += e.device_time
+    acc = kernel_times(prof)
+    total_us = sum(cnt * (us / cnt) for cnt, us in acc.values()) / args.steps
+    ctl = control_c2c(n, args.steps, args.warmup)
     name, power = card()
     launches = args.steps * streams
     rows = []
@@ -86,7 +117,9 @@ def main():
         if b:
             row.update(bytes=b, gbs=b / (per * 1e-6) / 1e9, share=b / (per * 1e-6) / DATASHEET_BPS)
         rows.append(row)
-    total_us = sum(cnt * (us / cnt) for cnt, us in acc.values()) / args.steps
+    b = bytes_per_launch("r2c_rows_split_kernel", n)
+    rows.append({"kernel": "control: same body, C2C, no split", "per_stream_block": 1.0, "us": ctl, "bytes": b,
+                 "gbs": b / (ctl * 1e-6) / 1e9, "share": b / (ctl * 1e-6) / DATASHEET_BPS})
     print(f"config #3, {streams} streams of 2^{n.bit_length() - 1} samples, one lane; {args.steps} blocks profiled")
     print(f"card: {name}, power limit {power}")
     print(f"{'kernel':34s} {'/stream':>7s} {'us':>9s} {'MB':>8s} {'GB/s':>8s} {'of 3.35 TB/s':>12s}")

@@ -197,5 +197,105 @@ def main_channel_blocked(logp=5, logq=8):
     return 0
 
 
+def paired_split(logp=3, seed=2):
+    """The row sweep's split at Q = L = 2^14, one read per mirror pair (r2c_rows_split_kernel). Rows k1 and P - k1 sit
+    in the two CTAs of a cluster, each row in the digit-reversed layout of the whole-row kernel: Z[k2] with
+    k2 = d0 + 16 d1 + 256 d2 + 4096 d3 at chunk d0 (half buffer A for d0 < 8, B for d0 >= 8), then (d1, d2, d3).
+    Thread u of a CTA: lane = u & 31, wid = u >> 5, pd0 = lane & 7, h = (lane >> 3) & 1,
+    pd1 = ((wid & 7) << 1) | (lane >> 4), sel = wid >> 3 (the parent's 32-bin group (pd0, pd1, sel), pd0 < 8 only).
+    For j = 0..7 and i2 = h ? 15 - j : j it reads its own 16-byte pair (pd0, pd1, i2, d3 = 2 sel, 2 sel + 1) from A and
+    the mirror pair (15 - pd0, 15 - pd1, 15 - i2, 1 - sel) from the mirror row's B (the partner's; its own for row P/2;
+    row 0 pairs k2 with (L - k2) mod L instead and reads both from its own row), and emits X of both pairs.
+    Checks: (a) every bin of every row emitted exactly once, equal to numpy.fft.rfft; (b) own reads in A, mirror reads
+    in B; (c) every store instruction (a warp, one j, own or mirror pair) writes whole 64-byte pieces of the
+    channel-blocked layout; (d) the fp32 partial of each 32-bin group is summed in the order i2 = 0..15 the one-group
+    threads used, and the groups map one to one onto the parent's threads."""
+    L = 1 << 14
+    P = 1 << logp
+    M = P * L
+    rng = np.random.default_rng(seed)
+    real = rng.standard_normal(2 * M)
+    H = np.fft.fft(real[0::2] + 1j * real[1::2])
+    Z = H[np.arange(P)[:, None] + P * np.arange(L)[None, :]]          # Z[k1][k2], as the row transform leaves it
+    ref = np.fft.rfft(real)[:M]
+
+    def pos(k2):  # (d0, d1, d2, d3) of natural-order k2
+        return k2 & 15, (k2 >> 4) & 15, (k2 >> 8) & 15, k2 >> 12
+
+    def split(zk, zm, k):
+        zm = np.conj(zm)
+        w = np.exp(-1j * np.pi * k / M)
+        return 0.5 * (zk + zm) - 0.5j * w * (zk - zm)
+
+    u = np.arange(512)
+    lane, wid = u & 31, u >> 5
+    pd0, h = lane & 7, (lane >> 3) & 1
+    pd1, sel = ((wid & 7) << 1) | (lane >> 4), wid >> 3
+    kb = pd0 + 16 * pd1 + 8192 * sel                 # own k2 of i2 = 0, d3 = 2 sel
+    kbm = (15 - pd0) + 16 * (15 - pd1) + 8192 * (1 - sel)
+    # the parent's thread of each group: one group per thread, bijective
+    parent = lambda d0, d1, s: 32 * ((d1 >> 1) + 8 * s) + (d0 + 16 * (d1 & 1))  # noqa: E731
+    assert len(set(parent(d0, d1, s) for d0 in range(16) for d1 in range(16) for s in range(2))) == 512
+    # h = 1 ends with its own group's partial, h = 0 with the mirror group's: each parent thread's group exactly once
+    fin = np.concatenate([parent(pd0, pd1, sel)[h == 1], parent(15 - pd0, 15 - pd1, 1 - sel)[h == 0]])
+    assert np.array_equal(np.sort(fin), np.arange(512))
+    # the kernel's closed forms of those two thread indices
+    assert np.array_equal(parent(pd0, pd1, sel), u & ~8) and np.array_equal(parent(15 - pd0, 15 - pd1, 1 - sel), 511 - (u & ~8))
+    X = np.full((P, L), np.nan + 0j)
+    for i in range(P // 2):
+        rows = (0, P // 2) if i == 0 else (i, P - i)
+        for row in rows:
+            prow = row if (row == 0 or 2 * row == P) else P - row
+            for j in range(8):
+                i2 = np.where(h == 1, 15 - j, j)
+                im = 15 - i2
+                for d3 in (0, 1):                     # the two elements of each 16-byte pair
+                    k = kb + 256 * i2 + 4096 * d3                      # own bin
+                    km = kbm + 256 * im + 4096 * d3                   # element d3 of the mirror pair
+                    assert (pos(k)[0] < 8).all() and (pos(km)[0] >= 8).all(), "own pairs in A, mirror pairs in B"
+                    if row != 0:
+                        # the mirror pair holds L - 1 - k in the opposite element: no other read
+                        assert np.array_equal(kbm + 256 * im + 4096 * (1 - d3), L - 1 - k)
+                        mk, mkm = Z[prow, L - 1 - k], Z[row, L - 1 - km]
+                    else:                             # row 0: k2 pairs with (L - k2) mod L of the same row
+                        mk, mkm = Z[0, (L - k) % L], Z[0, (L - km) % L]
+                    for r, kk, zk, zm in ((row, k, Z[row, k], mk), (prow, km, Z[prow, km], mkm)):
+                        assert np.isnan(X[r, kk]).all(), "bin emitted twice"
+                        X[r, kk] = split(zk, zm, r + P * kk)
+                # (c) the store instructions of each warp: lanes 2m, 2m + 1 trade halves (own pairs: the even lane stores
+                # d3 = 2 sel of k2, k2 + 1, the odd one d3 = 2 sel + 1; mirror pairs: pd0 even <-> odd swapped), so each
+                # lane stores one 16-byte pair of adjacent k2 of one row
+                for mine, r in ((True, row), (False, prow)):
+                    base = kb if mine else kbm
+                    ii = i2 if mine else im
+                    odd = (pd0 & 1) if mine else 1 - (pd0 & 1)
+                    ks = base - odd + 256 * ii + odd * 4096     # first k2 of the lane's 16-byte store
+                    assert (ks & 1 == 0).all()
+                    addr = channel_blocked_addr(r, ks, L) * 8                     # bytes
+                    for w in range(16):
+                        a = addr[32 * w:32 * w + 32]
+                        pieces = {}
+                        for x in a:
+                            pieces.setdefault(x // 64, set()).add(x % 64)
+                        assert all(v == {0, 16, 32, 48} for v in pieces.values()), "whole 64-byte pieces"
+    assert not np.isnan(X).any(), "every bin emitted"
+    err = np.abs(X.T.reshape(-1) - ref).max() / np.abs(ref).max()
+    assert err < 1e-12, err
+    # (d) order of the fp32 partials: h = 0 sums its own group's i2 = 0..7, h = 1 the mirror group's i2 = 0..7 (as
+    # 15 - i2 descends); each keeps the other group's eight terms and folds them after the lane-8 exchange, j = 7..0
+    i2_of = lambda hh, j: 15 - j if hh else j  # noqa: E731
+    own = [i2_of(0, j) for j in range(8)] + [i2_of(1, j) for j in range(7, -1, -1)]
+    mir = [15 - i2_of(1, j) for j in range(8)] + [15 - i2_of(0, j) for j in range(7, -1, -1)]
+    assert own == list(range(16)) and mir == list(range(16))
+    return err
+
+
+def main_paired_split(logp=3):
+    err = paired_split(logp)
+    print(f"P=2^{logp} L=2^14: one read per mirror pair, both rows emitted, 64-byte store pieces, partial order: "
+          f"max rel err {err:.2e}")
+    return 0
+
+
 if __name__ == "__main__":
     sys.exit(main(sys.argv))
