@@ -13,6 +13,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <set>
 #include <string>
 #include <vector>
@@ -33,28 +34,47 @@ static thread_local std::string g_last_error;
 // result headers per block: one per data stream (at most 4), then the total-intensity sum's (signal_detect_sum_streams)
 constexpr int RES_GROUP = 5, SUM_SLOT = 4;
 
+// an allocation the context owns, device memory or (PINNED) pinned host memory, freed with its owner. grow() sizes it;
+// move-only, so a lane_state holding some stays swappable (lane_swap)
+template <class T, bool PINNED = false>
+struct buffer {
+  T* p = nullptr;
+  size_t bytes = 0;
+  buffer() = default;
+  buffer(buffer&& o) noexcept : p(o.p), bytes(o.bytes) {
+    o.p = nullptr;
+    o.bytes = 0;
+  }
+  buffer& operator=(buffer&& o) noexcept {
+    std::swap(p, o.p);
+    std::swap(bytes, o.bytes);
+    return *this;
+  }
+  ~buffer() { release(); }
+  cudaError_t release() {
+    const cudaError_t e = !p ? cudaSuccess : PINNED ? cudaFreeHost(p) : cudaFree(p);
+    p = nullptr;
+    bytes = 0;
+    return e;
+  }
+};
+
 // what one chain of kernels writes through: the data streams of a block are independent until their result headers
 // are read back, so a context runs the odd-numbered ones on a second lane with its own CUDA stream and scratch (one
 // lane's kernel tails and small detector kernels overlap the other lane's FFT sweeps)
 struct lane_state {
   cudaStream_t stream = nullptr;
-  void* fft_scratch = nullptr;
-  size_t fft_scratch_bytes = 0;
+  buffer<float2> fft_scratch;
   // s1
   double* partial = nullptr;
   unsigned* ticket = nullptr;
   unsigned* detect_ticket = nullptr;  // last-CTA ticket of the detector's column-sum kernel
   float* mean = nullptr;
   // detect
-  float* colsum_partial = nullptr;
-  size_t colsum_partial_elems = 0;
-  float* acc = nullptr;
-  size_t acc_elems = 0;
+  buffer<float> colsum_partial, acc;
   // long waterfall rows: per-tile SK statistics of the last sweep, per-row zap flags
-  void* long_stats = nullptr;
-  size_t long_stats_bytes = 0;
-  void* long_zap = nullptr;
-  size_t long_zap_bytes = 0;
+  buffer<float2> long_stats;
+  buffer<unsigned char> long_zap;
 };
 
 struct srtb_b200_ctx {
@@ -75,27 +95,22 @@ struct srtb_b200_ctx {
   int lanes = 1;  // SRTB_B200_LANES (default 2): CUDA streams per context the data streams of a block are spread over
   cudaEvent_t lane_fork = nullptr, lane_join = nullptr;
   // FFT
-  float2* tw[13] = {nullptr};
-  std::map<int, float2*> bigtw;  // log2(n_i) -> [3 << q]
-  float2* bigrow_tab[2][2] = {{nullptr, nullptr}, {nullptr, nullptr}};  // [logl - 13][forward] whole-row kernel tables
+  buffer<float2> tw[13];
+  std::map<int, buffer<float2>> bigtw;  // log2(n_i) -> [3 << q]
+  buffer<float2> bigrow_tab[2][2];      // [logl - 13][forward] whole-row kernel tables
   // detect (slots = streams in flight, then SUM_SLOT)
-  float* series[RES_GROUP] = {};
-  size_t series_elems = 0;
+  buffer<float> series[RES_GROUP];
   detect_dev_result* d_res = nullptr;  // RES_GROUP slots
   detect_dev_result* h_res = nullptr;  // pinned, RES_GROUP slots for process_block, then RES_GROUP per ring slot
   size_t slot_time_count[RES_GROUP] = {};
   // total-intensity sum: the streams' raw column sums [1 + RING_SLOTS][4][L] (group 0: process_block, 1 + slot: the
   // ring; slot-owned, so a lane's next block cannot overwrite what the sum of this one still reads), and the mask
   // kernel's output (mask float2[C], mismatched channels uint2[C], their count)
-  float* sum_raw = nullptr;
-  size_t sum_raw_bytes = 0;
-  void* sum_mask = nullptr;
-  size_t sum_mask_bytes = 0;
-  float* raw_dst = nullptr;  // block path with the sum: this block's raw column sums [4][L] (else null)
+  buffer<float> sum_raw;
+  buffer<float2> sum_mask;
   // pipelined ingest ring
   cudaStream_t copy_stream = nullptr;
-  void* slot_baseband[SRTB_B200_RING_SLOTS] = {nullptr};
-  size_t slot_baseband_bytes[SRTB_B200_RING_SLOTS] = {0};
+  buffer<void> slot_baseband[SRTB_B200_RING_SLOTS];
   cudaEvent_t slot_h2d[SRTB_B200_RING_SLOTS] = {nullptr}, slot_done[SRTB_B200_RING_SLOTS] = {nullptr};
   int slot_streams[SRTB_B200_RING_SLOTS] = {0};
   bool slot_busy[SRTB_B200_RING_SLOTS] = {false};
@@ -104,52 +119,34 @@ struct srtb_b200_ctx {
   bool slot_sum[SRTB_B200_RING_SLOTS] = {false};  // the slot's block carries the total-intensity sum's header
   int slot_ticket[SRTB_B200_RING_SLOTS] = {0};
   // per-slot outputs: ctx-owned working buffers / pinned series unless the caller supplied its own (submit_block_ex)
-  float* slot_stream_buf[SRTB_B200_RING_SLOTS][4] = {};
-  size_t slot_stream_elems[SRTB_B200_RING_SLOTS] = {0};
-  float* slot_h_series[SRTB_B200_RING_SLOTS] = {nullptr};
-  size_t slot_h_series_elems[SRTB_B200_RING_SLOTS] = {0};
+  buffer<float> slot_stream_buf[SRTB_B200_RING_SLOTS][4];
+  buffer<float, true> slot_h_series[SRTB_B200_RING_SLOTS];
   float* slot_out_spectrum[SRTB_B200_RING_SLOTS][4] = {};
   float* slot_out_series[SRTB_B200_RING_SLOTS] = {nullptr};
   uint64_t submit_count = 0;
   // DM sweep working copy of the spectrum, per-trial result headers
-  void* sweep_buf = nullptr;
-  size_t sweep_buf_bytes = 0;
-  void* sweep_res = nullptr;
-  size_t sweep_res_bytes = 0;
+  buffer<float2> sweep_buf;
+  buffer<detect_dev_result> sweep_res;
   // optional per-stage timing (srtb_b200_stage_stats)
   bool stats_on = false;
   cudaEvent_t stat_ev[SRTB_B200_STAGE_COUNT][2] = {};
   double stat_bytes[SRTB_B200_STAGE_COUNT] = {};
   bool stat_have[SRTB_B200_STAGE_COUNT] = {};
-  // ring path: pinned host destination [streams][MAX_BOXCARS][L] of the current block's positive series (else null)
-  float* host_series_dst = nullptr;
-  // DM sweep with outputs: device record of the current (trial, stream) that the detector fills with its peaks (else null)
-  detect_dev_peak* peak_dst = nullptr;
-  bool pdl_auto = false;    // programmatic dependent launch for the current block (short kernels only)
-  bool res_zeroed = false;  // block path: the per-stream result headers were zeroed before the first kernel
+  bool pdl_auto = false;  // programmatic dependent launch for the current block (short kernels only)
   // process_block
-  void* d_baseband = nullptr;
-  size_t d_baseband_bytes = 0;
-  float* stream_buf[4] = {nullptr, nullptr, nullptr, nullptr};
-  size_t stream_buf_elems = 0;
+  buffer<void> d_baseband;
+  buffer<float> stream_buf[4];
   // K12 phase table of the current (block geometry, DM): see chirp_phase_table_kernel
-  float* chirp_tab = nullptr;
-  size_t chirp_tab_bytes = 0;
+  buffer<float> chirp_tab;
   double chirp_tab_key[7] = {0, 0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm, layout (logp)
   // simplify_spectrum: row-resampled intensities R[C][W] and the column stage's per-CTA partial sums
-  float* thumb_rows = nullptr;
-  size_t thumb_rows_bytes = 0;
-  float* thumb_partial = nullptr;
-  size_t thumb_partial_bytes = 0;
-  // correlate: the two inputs' in-place R2C buffers of real_count + 2 floats (entries 2 and 3 stay null)
-  float* corr_buf[4] = {};
-  size_t corr_buf_elems = 0;
+  buffer<float> thumb_rows, thumb_partial;
+  // correlate: the two inputs' in-place R2C buffers of real_count + 2 floats
+  buffer<float> corr_buf[2];
   // correlate_accumulate / _finish: the packed segment rows of both inputs (also finish's Ms-point C2C buffer), the
   // split's per-row-group partial sums and its per-bin-tile tickets (sm_count * 8, zero between launches)
-  void* corr_rows = nullptr;
-  size_t corr_rows_bytes = 0;
-  void* corr_partial = nullptr;
-  size_t corr_partial_bytes = 0;
+  buffer<float2> corr_rows;
+  buffer<double2> corr_partial;
   unsigned* corr_tickets = nullptr;
   // incoherent DM search: the shift tables of the last (geometry, dm, trial list), on the host and the device, and the
   // per-trial series [n_dm][nb][T], scans [n_dm][T], result headers, peaks and tickets
@@ -160,10 +157,7 @@ struct srtb_b200_ctx {
   std::vector<int2> inc_gspan, inc_groups;        // [groups][C] (min, max) of a group's offsets; [groups] (first, count)
   unsigned inc_spread = 0;                         // largest max - min of any group and channel
   bool inc_tab_uploaded = false;
-  void* inc_tab = nullptr;
-  size_t inc_tab_bytes = 0;
-  void* inc_work = nullptr;
-  size_t inc_work_bytes = 0;
+  buffer<char> inc_tab, inc_work;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -180,19 +174,6 @@ static cudaError_t lane_alloc(lane_state* l) {
   if (e == cudaSuccess) e = cudaMemset(l->detect_ticket, 0, sizeof(unsigned));
   if (e == cudaSuccess) e = cudaMalloc(&l->mean, sizeof(float));
   return e;
-}
-
-// every device buffer of a lane; not its stream
-static void lane_free(lane_state* l) {
-  cudaFree(l->fft_scratch);
-  cudaFree(l->partial);
-  cudaFree(l->ticket);
-  cudaFree(l->detect_ticket);
-  cudaFree(l->mean);
-  cudaFree(l->colsum_partial);
-  cudaFree(l->acc);
-  cudaFree(l->long_stats);
-  cudaFree(l->long_zap);
 }
 
 #define API_LOCK(c)                                         \
@@ -221,27 +202,24 @@ static int sync_lanes(srtb_b200_ctx* ctx) {
   return 0;
 }
 
-static int ensure(srtb_b200_ctx* ctx, void** p, size_t* have, size_t want_bytes) {
-  if (*have >= want_bytes && *p) return 0;
-  if (*p) {
+// b holds at least `bytes` afterwards: a larger allocation replaces a smaller one once both lanes are idle. A failed
+// allocation leaves b empty and clears the runtime's last error, which the next launch check would otherwise report.
+template <class T, bool PINNED>
+static int grow(srtb_b200_ctx* ctx, buffer<T, PINNED>& b, size_t bytes) {
+  if (b.bytes >= bytes && b.p) return 0;
+  if (b.p) {
     if (int rc = sync_lanes(ctx)) return rc;
-    CK(cudaFree(*p));
-    *p = nullptr;
-    *have = 0;
+    CK(b.release());
   }
-  cudaError_t e = cudaMalloc(p, want_bytes);
-  if (e != cudaSuccess)
-    return fail(ctx, SRTB_B200_E_NOMEM, std::string("cudaMalloc(") + std::to_string(want_bytes) +
+  void* q = nullptr;
+  const cudaError_t e = PINNED ? cudaMallocHost(&q, bytes) : cudaMalloc(&q, bytes);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(ctx, SRTB_B200_E_NOMEM, std::string(PINNED ? "cudaMallocHost(" : "cudaMalloc(") + std::to_string(bytes) +
                                             "): " + cudaGetErrorString(e));
-  *have = want_bytes;
-  return 0;
-}
-
-// the lane's partial column sums of the detector, grown to at least `elems` floats
-static int ensure_colsum_partial(srtb_b200_ctx* ctx, size_t elems) {
-  size_t have = ctx->lane.colsum_partial_elems * sizeof(float);
-  if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->lane.colsum_partial), &have, elems * sizeof(float))) return rc;
-  ctx->lane.colsum_partial_elems = have / sizeof(float);
+  }
+  b.p = static_cast<T*>(q);
+  b.bytes = bytes;
   return 0;
 }
 
@@ -323,46 +301,27 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
     cudaStreamSynchronize(ctx->alt.stream);
     cudaStreamDestroy(ctx->alt.stream);
   }
-  lane_free(&ctx->lane);
-  lane_free(&ctx->alt);
-  if (ctx->lane_fork) cudaEventDestroy(ctx->lane_fork);
-  if (ctx->lane_join) cudaEventDestroy(ctx->lane_join);
-  for (auto& p : ctx->tw)
-    if (p) cudaFree(p);
-  for (auto& kv : ctx->bigtw) cudaFree(kv.second);
-  for (auto& a : ctx->bigrow_tab)
-    for (auto& p : a) cudaFree(p);
-  for (auto& p : ctx->series) cudaFree(p);
+  for (lane_state* l : {&ctx->lane, &ctx->alt}) {
+    cudaFree(l->partial);
+    cudaFree(l->ticket);
+    cudaFree(l->detect_ticket);
+    cudaFree(l->mean);
+  }
   cudaFree(ctx->d_res);
   cudaFreeHost(ctx->h_res);
-  cudaFree(ctx->d_baseband);
-  cudaFree(ctx->sweep_buf);
-  cudaFree(ctx->sweep_res);
-  cudaFree(ctx->chirp_tab);
-  cudaFree(ctx->thumb_rows);
-  cudaFree(ctx->thumb_partial);
-  for (auto& p : ctx->corr_buf) cudaFree(p);
-  cudaFree(ctx->corr_rows);
-  cudaFree(ctx->corr_partial);
   cudaFree(ctx->corr_tickets);
-  cudaFree(ctx->inc_tab);
-  cudaFree(ctx->inc_work);
-  cudaFree(ctx->sum_raw);
-  cudaFree(ctx->sum_mask);
+  if (ctx->lane_fork) cudaEventDestroy(ctx->lane_fork);
+  if (ctx->lane_join) cudaEventDestroy(ctx->lane_join);
   for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
-    cudaFree(ctx->slot_baseband[i]);
-    for (auto& p : ctx->slot_stream_buf[i]) cudaFree(p);
-    if (ctx->slot_h_series[i]) cudaFreeHost(ctx->slot_h_series[i]);
     if (ctx->slot_h2d[i]) cudaEventDestroy(ctx->slot_h2d[i]);
     if (ctx->slot_done[i]) cudaEventDestroy(ctx->slot_done[i]);
     if (ctx->slot_done_alt[i]) cudaEventDestroy(ctx->slot_done_alt[i]);
   }
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
-  for (auto& p : ctx->stream_buf) cudaFree(p);
   for (auto& ev : ctx->stat_ev)
     for (auto& e2 : ev)
       if (e2) cudaEventDestroy(e2);
-  delete ctx;
+  delete ctx;  // the buffers free themselves
   return 0;
 }
 
@@ -531,26 +490,38 @@ extern "C" int srtb_b200_unpack(srtb_b200_ctx* ctx, const void* d_in, size_t in_
 // ------------------------------------------------------------------------------------
 // FFT planning + launches
 // ------------------------------------------------------------------------------------
+// a constant table on the device, uploaded synchronously so that both lanes and every later launch may read it; d is
+// set only once the upload has completed
+static int upload_table(srtb_b200_ctx* ctx, const std::vector<float2>& h, buffer<float2>* d) {
+  buffer<float2> t;
+  void* q = nullptr;
+  CK(cudaMalloc(&q, h.size() * sizeof(float2)));
+  t.p = static_cast<float2*>(q);
+  t.bytes = h.size() * sizeof(float2);
+  CK(cudaMemcpyAsync(t.p, h.data(), t.bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
+  CK(cudaStreamSynchronize(ctx->lane.stream));
+  *d = std::move(t);
+  return 0;
+}
+
 static int get_stage_twiddles(srtb_b200_ctx* ctx, int logl, const float2** out) {
-  if (!ctx->tw[logl]) {
+  if (!ctx->tw[logl].p) {
     const size_t L = (size_t)1 << logl;
     std::vector<float2> h(L);
     for (size_t j = 0; j < L; j++) {
       const double a = -2.0 * M_PI * (double)j / (double)L;
       h[j] = make_float2((float)std::cos(a), (float)std::sin(a));
     }
-    CK(cudaMalloc(&ctx->tw[logl], L * sizeof(float2)));
-    CK(cudaMemcpyAsync(ctx->tw[logl], h.data(), L * sizeof(float2), cudaMemcpyHostToDevice, ctx->lane.stream));
-    CK(cudaStreamSynchronize(ctx->lane.stream));
+    if (int rc = upload_table(ctx, h, &ctx->tw[logl])) return rc;
   }
-  *out = ctx->tw[logl];
+  *out = ctx->tw[logl].p;
   return 0;
 }
 
 static int get_big_twiddles(srtb_b200_ctx* ctx, int logn, big_twiddle* out) {
   const int q = (logn + 2) / 3;
-  auto it = ctx->bigtw.find(logn);
-  if (it == ctx->bigtw.end()) {
+  buffer<float2>& d = ctx->bigtw[logn];
+  if (!d.p) {
     const size_t n = (size_t)1 << logn, m = (size_t)1 << q;
     std::vector<float2> h(3 * m);
     for (int level = 0; level < 3; level++)
@@ -559,13 +530,9 @@ static int get_big_twiddles(srtb_b200_ctx* ctx, int logn, big_twiddle* out) {
         const double a = -2.0 * M_PI * (double)idx / (double)n;
         h[level * m + j] = make_float2((float)std::cos(a), (float)std::sin(a));
       }
-    float2* d = nullptr;
-    CK(cudaMalloc(&d, h.size() * sizeof(float2)));
-    CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->lane.stream));
-    CK(cudaStreamSynchronize(ctx->lane.stream));
-    it = ctx->bigtw.emplace(logn, d).first;
+    if (int rc = upload_table(ctx, h, &d)) return rc;
   }
-  out->tab = it->second;
+  out->tab = d.p;
   out->q = q;
   return 0;
 }
@@ -1000,8 +967,8 @@ static int dispatch_trans(srtb_b200_ctx* ctx, int logl, const float2* in, float2
 template <int LOGL>
 static int get_bigrow_tables(srtb_b200_ctx* ctx, bool fwd, const float2** out) {
   using C = bigrow<LOGL>;
-  float2*& d = ctx->bigrow_tab[LOGL - 13][fwd ? 1 : 0];
-  if (!d) {
+  buffer<float2>& d = ctx->bigrow_tab[LOGL - 13][fwd ? 1 : 0];
+  if (!d.p) {
     std::vector<float2> h(C::TABN);
     const double sgn = fwd ? -1.0 : 1.0;
     auto w = [&](size_t n, size_t e) {
@@ -1013,11 +980,9 @@ static int get_bigrow_tables(srtb_b200_ctx* ctx, bool fwd, const float2** out) {
       for (int j = 0; j < C::B2; j++) h[C::B1 + (i - 1) * C::B2 + j] = w(C::B1, (size_t)i * j);
     for (int i = 1; i < 16; i++)
       for (int j = 0; j < C::R3; j++) h[C::B1 + 15 * C::B2 + (i - 1) * C::R3 + j] = w(C::B2, (size_t)i * j);
-    CK(cudaMalloc(&d, h.size() * sizeof(float2)));
-    CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(float2), cudaMemcpyHostToDevice, ctx->lane.stream));
-    CK(cudaStreamSynchronize(ctx->lane.stream));
+    if (int rc = upload_table(ctx, h, &d)) return rc;
   }
-  *out = d;
+  *out = d.p;
   return 0;
 }
 
@@ -1036,8 +1001,8 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
     if (int rc = persistent_grid(ctx, kern, C::NT, smem, smem, nrows, &grid)) return rc;
     row_sk_params p{};
     if (with_sk) {
-      if (int rc = ensure_colsum_partial(ctx, (size_t)grid * sk->ts_count)) return rc;
-      sk->partial = ctx->lane.colsum_partial;
+      if (int rc = grow(ctx, ctx->lane.colsum_partial, (size_t)grid * sk->ts_count * sizeof(float))) return rc;
+      sk->partial = ctx->lane.colsum_partial.p;
       p = *sk;
     }
     CK(launch_pdl(ctx, kern, dim3(grid), dim3(C::NT), smem, in, out, (unsigned)nrows, tabs, p,
@@ -1152,8 +1117,8 @@ static int fft_c2c_impl(srtb_b200_ctx* ctx, float2* x, size_t n, size_t batch) {
                    : launch_bigrow<14, FWD>(ctx, x, x, batch, nullptr, nullptr, nullptr);
   }
   if (q > 30) return fail(ctx, SRTB_B200_E_SIZE, "fft: length above 2^30 not supported");
-  if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, batch * n * sizeof(float2))) return rc;
-  float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
+  if (int rc = grow(ctx, ctx->lane.fft_scratch, batch * n * sizeof(float2))) return rc;
+  float2* s = ctx->lane.fft_scratch.p;
   if (q <= 20) {
     const int l1 = (q + 1) / 2, l2 = q - l1;
     const size_t L1 = (size_t)1 << l1, L2 = (size_t)1 << l2;
@@ -1291,8 +1256,8 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
     if (four_sweeps(q, d_inout)) {
       int l[4];
       plan4(q, l);
-      if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, M * sizeof(float2))) return rc;
-      float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
+      if (int rc = grow(ctx, ctx->lane.fft_scratch, M * sizeof(float2))) return rc;
+      float2* s = ctx->lane.fft_scratch.p;
       const size_t L1 = (size_t)1 << l[0], L2 = (size_t)1 << l[1], L3 = (size_t)1 << l[2], L4 = (size_t)1 << l[3];
       bool first_done = false;
       if (raw && raw->base) {
@@ -1320,8 +1285,8 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
     }
     const int llast = l3 ? l3 : l2;
     if (llast >= 6 && llast <= 8 && get_encode_tiled()) {
-      if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, M * sizeof(float2))) return rc;
-      float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
+      if (int rc = grow(ctx, ctx->lane.fft_scratch, M * sizeof(float2))) return rc;
+      float2* s = ctx->lane.fft_scratch.p;
       const size_t L1 = (size_t)1 << l1, L2 = (size_t)1 << l2, L3 = (size_t)1 << l3;
       bool first_done = false;
       if (raw && raw->base) {
@@ -1556,27 +1521,35 @@ extern "C" int srtb_b200_rfi_s2_sk(srtb_b200_ctx* ctx, void* d_x, size_t time_co
 // ------------------------------------------------------------------------------------
 // signal detect
 // ------------------------------------------------------------------------------------
+// where one detector run writes: the series, result header d_res[slot] and sample count of the context's `slot`, and,
+// each already offset to this run by the caller (or null), the pinned host rows [MAX_BOXCARS][L] of its positive
+// series, its raw column sums [L] and its peak record. header_zeroed: the caller zeroed d_res[slot] before the first
+// kernel (a memset between two kernels would break their programmatic-dependent-launch chain).
+struct detect_out {
+  int slot = 0;
+  float* host_series = nullptr;
+  float* raw = nullptr;
+  detect_dev_peak* peak = nullptr;
+  bool header_zeroed = false;
+};
+
+// time samples of a row of time_count the detector searches: the reserved tail is left out unless it is the whole row
+static size_t detected_samples(size_t time_count, size_t reserved) {
+  return time_count <= reserved ? time_count : time_count - reserved;
+}
+
+// boxcar kernel CTAs for a series of ts samples: one per possible boxcar; those beyond n_boxcars (known only on the
+// device) exit at once
+static unsigned boxcar_ctas(size_t max_boxcar, size_t ts) {
+  unsigned n = 1;
+  for (size_t b = 2; b <= max_boxcar && b < ts && n < SRTB_B200_MAX_BOXCARS; b *= 2) n++;
+  return n;
+}
+
 static int detect_prepare(srtb_b200_ctx* ctx, int slot, size_t time_count, size_t need_partial_elems) {
-  const size_t series_need = (size_t)SRTB_B200_MAX_BOXCARS * time_count;
-  if (ctx->series_elems < series_need) {
-    if (int rc = sync_lanes(ctx)) return rc;
-    for (auto& p : ctx->series) {
-      if (p) CK(cudaFree(p));
-      p = nullptr;
-    }
-    ctx->series_elems = 0;
-  }
-  if (!ctx->series[slot]) {
-    cudaError_t e = cudaMalloc(&ctx->series[slot], series_need * sizeof(float));
-    if (e != cudaSuccess) return fail(ctx, SRTB_B200_E_NOMEM, "detect: series alloc failed");
-    ctx->series_elems = series_need;
-  }
-  {
-    size_t have = ctx->lane.acc_elems * sizeof(float);
-    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->lane.acc), &have, time_count * sizeof(float))) return rc;
-    ctx->lane.acc_elems = have / sizeof(float);
-  }
-  return ensure_colsum_partial(ctx, need_partial_elems);
+  if (int rc = grow(ctx, ctx->series[slot], (size_t)SRTB_B200_MAX_BOXCARS * time_count * sizeof(float))) return rc;
+  if (int rc = grow(ctx, ctx->lane.acc, time_count * sizeof(float))) return rc;
+  return grow(ctx, ctx->lane.colsum_partial, need_partial_elems * sizeof(float));
 }
 
 // channel rows in chunks for colsum_partial_kernel: about 8 CTAs per SM in all, at most 128 chunks
@@ -1592,50 +1565,53 @@ static colsum_chunks colsum_geometry(const srtb_b200_ctx* ctx, size_t samples_pe
 }
 
 // column-sum reduction over `chunks` partial rows, zero count, scan, boxcar ladder
+// partial: the `chunks` rows of partial column sums, or null when out.slot's series already holds the summed series
+// (the total-intensity sum, whose tail is not a stage of its own and so is not timed)
 // zero_stride / zero_count_n: where the detector looks for masked channels — the first time sample of every channel
-// of [C][L] (stride L, C of them; the default), or the first spectrum of [time][frequency] (stride 1; v1 detector)
-static int detect_tail(srtb_b200_ctx* ctx, int slot, const float2* x, size_t time_count, size_t chan_count,
-                       size_t ts_count, size_t chunks, float snr, float chan_thr, size_t max_boxcar,
-                       size_t zero_stride = 0) {
+// of [C][L] (stride L, C of them; the default), or the first spectrum of [time][frequency] (stride 1; v1 detector, and
+// the sum's channel mask)
+static int detect_tail(srtb_b200_ctx* ctx, const detect_out& out, const float* partial, const float2* x,
+                       size_t time_count, size_t chan_count, size_t ts_count, size_t chunks, float snr, float chan_thr,
+                       size_t max_boxcar, size_t zero_stride = 0) {
   if (zero_stride == 0) zero_stride = time_count;
-  float* const host_series = ctx->host_series_dst ? ctx->host_series_dst + (size_t)slot * SRTB_B200_MAX_BOXCARS * time_count : nullptr;
-  float* const raw = ctx->raw_dst ? ctx->raw_dst + (size_t)slot * time_count : nullptr;
-  stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_DETECT_TAIL, 4.0 * (double)chunks * (double)ts_count);
-  CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>((ts_count + 31) / 32, (size_t)ctx->sm_count)),
-                dim3(1024), 0, (const float*)ctx->lane.colsum_partial, ts_count, chunks, ctx->series[slot], ctx->lane.acc, x, zero_stride,
-                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0, raw));
+  const int slot = out.slot;
+  std::optional<stage_scope> stats_;
+  if (partial) stats_.emplace(ctx, SRTB_B200_STAGE_FUSED_DETECT_TAIL, 4.0 * (double)chunks * (double)ts_count);
+  const size_t scan_ctas = partial ? (ts_count + 31) / 32 : (chan_count + 1023) / 1024;
+  CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>(scan_ctas, (size_t)ctx->sm_count)),
+                dim3(1024), 0, partial, ts_count, chunks, ctx->series[slot].p, ctx->lane.acc.p, x, zero_stride,
+                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0, out.raw));
   ctx->launches++;
   CK(cudaGetLastError());
-  // one CTA per possible boxcar; CTAs beyond n_boxcars (known only on the device) exit at once
-  unsigned max_nb = 1;
-  for (size_t b = 2; b <= max_boxcar && b < ts_count && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2) max_nb++;
-  if (ctx->peak_dst)
-    CK(launch_pdl(ctx, detect_boxcar_kernel<true>, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count,
-                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, ctx->peak_dst, (size_t)0,
+  const unsigned max_nb = boxcar_ctas(max_boxcar, ts_count);
+  if (out.peak)
+    CK(launch_pdl(ctx, detect_boxcar_kernel<true>, dim3(max_nb), dim3(1024), 0, ctx->series[slot].p, time_count,
+                  (const float*)ctx->lane.acc.p, ts_count, snr, ctx->d_res + slot, out.host_series, out.peak, (size_t)0,
                   (size_t)0));
   else
-    CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, ctx->series[slot], time_count,
-                  (const float*)ctx->lane.acc, ts_count, snr, ctx->d_res + slot, host_series, (detect_dev_peak*)nullptr,
-                  (size_t)0, (size_t)0));
+    CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, ctx->series[slot].p, time_count,
+                  (const float*)ctx->lane.acc.p, ts_count, snr, ctx->d_res + slot, out.host_series,
+                  (detect_dev_peak*)nullptr, (size_t)0, (size_t)0));
   ctx->launches++;
   CK(cudaGetLastError());
   ctx->slot_time_count[slot] = time_count;
   return 0;
 }
 
-static int detect_enqueue(srtb_b200_ctx* ctx, int slot, const float2* x, size_t time_count,
+static int detect_enqueue(srtb_b200_ctx* ctx, const detect_out& out, const float2* x, size_t time_count,
                           size_t chan_count, size_t time_reserved_count, float snr, float chan_thr,
                           size_t max_boxcar) {
-  const size_t ts_count = (time_count <= time_reserved_count) ? time_count : time_count - time_reserved_count;
+  const size_t ts_count = detected_samples(time_count, time_reserved_count);
   const colsum_chunks cg = colsum_geometry(ctx, ts_count, chan_count);
-  if (int rc = detect_prepare(ctx, slot, time_count, cg.chunks * ts_count)) return rc;
-  CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  if (int rc = detect_prepare(ctx, out.slot, time_count, cg.chunks * ts_count)) return rc;
+  CK(cudaMemsetAsync(ctx->d_res + out.slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
   dim3 g((unsigned)cg.ctas_per_chunk, (unsigned)cg.chunks);
   colsum_partial_kernel<<<g, 256, 0, ctx->lane.stream>>>(const_cast<float2*>(x), time_count, chan_count, ts_count,
-                                                         cg.rows_per_chunk, ctx->lane.colsum_partial, nullptr);
+                                                         cg.rows_per_chunk, ctx->lane.colsum_partial.p, nullptr);
   ctx->launches++;
   CK(cudaGetLastError());
-  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr, max_boxcar);
+  return detect_tail(ctx, out, ctx->lane.colsum_partial.p, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr,
+                     max_boxcar);
 }
 
 // watfft (backward C2C of every channel row) with spectral kurtosis + the detector's partial column
@@ -1661,9 +1637,9 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
     constexpr size_t smem = row16_smem<LOGL, T16>::bytes;
     const size_t ntiles = (chan_count + T16 - 1) / T16;
     if (int rc = persistent_grid(ctx, kern, threads, smem, smem, ntiles, &grid)) return rc;
-    if (int rc = ensure_colsum_partial(ctx, (size_t)grid * ts_count)) return rc;
+    if (int rc = grow(ctx, ctx->lane.colsum_partial, (size_t)grid * ts_count * sizeof(float))) return rc;
     if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-    row_sk_params p{lo_, hi_, ctx->lane.colsum_partial, (unsigned)ts_count};
+    row_sk_params p{lo_, hi_, ctx->lane.colsum_partial.p, (unsigned)ts_count};
     CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem, src, x, chan_count, tw, p, chirp ? *chirp : row_chirp_params{}));
   } else {
     if (chirp || src != x) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: fused chirp needs the sixteen-point row kernel");
@@ -1672,9 +1648,9 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
     constexpr size_t smem = row_tma_smem<LOGL, T>::bytes;
     const size_t ntiles = (chan_count + T - 1) / T;
     if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
-    if (int rc = ensure_colsum_partial(ctx, (size_t)grid * ts_count)) return rc;
+    if (int rc = grow(ctx, ctx->lane.colsum_partial, (size_t)grid * ts_count * sizeof(float))) return rc;
     if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-    row_sk_params p{lo_, hi_, ctx->lane.colsum_partial, (unsigned)ts_count};
+    row_sk_params p{lo_, hi_, ctx->lane.colsum_partial.p, (unsigned)ts_count};
     kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(x, x, chan_count, tw, p);
   }
   ctx->launches++;
@@ -1683,15 +1659,13 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
   return 0;
 }
 
-static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_t time_count, size_t chan_count,
+static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, const detect_out& out, float2* x, size_t time_count, size_t chan_count,
                                   size_t time_reserved_count, float sk_threshold, float snr, float chan_thr,
                                   size_t max_boxcar, const row_chirp_params* chirp = nullptr,
                                   const float2* src = nullptr, bool sweep_order = false) {
-  const size_t ts_count = (time_count <= time_reserved_count) ? time_count : time_count - time_reserved_count;
-  if (int rc = detect_prepare(ctx, slot, time_count, 1)) return rc;
-  // the result header is zeroed here unless the block path did it for every stream up front (a memset between two
-  // kernels would break their programmatic-dependent-launch chain)
-  if (!ctx->res_zeroed) CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  const size_t ts_count = detected_samples(time_count, time_reserved_count);
+  if (int rc = detect_prepare(ctx, out.slot, time_count, 1)) return rc;
+  if (!out.header_zeroed) CK(cudaMemsetAsync(ctx->d_res + out.slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
   const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
   size_t chunks = 0;
   int rc = 0;
@@ -1725,7 +1699,8 @@ static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_
                                                          sweep_order);
     if (rc) return rc;
     stats_.reset();
-    return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, chunks, snr, chan_thr, max_boxcar);
+    return detect_tail(ctx, out, ctx->lane.colsum_partial.p, x, time_count, chan_count, ts_count, chunks, snr, chan_thr,
+                       max_boxcar);
   }
   switch (ilog2(time_count)) {
     case 9: rc = watfft_sk_launch<9>(ctx, x, chan_count, lo_, hi_, ts_count, &chunks, chirp, src); break;
@@ -1735,7 +1710,8 @@ static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, int slot, float2* x, size_
   }
   if (rc) return rc;
   stats_.reset();
-  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, chunks, snr, chan_thr, max_boxcar);
+  return detect_tail(ctx, out, ctx->lane.colsum_partial.p, x, time_count, chan_count, ts_count, chunks, snr, chan_thr,
+                     max_boxcar);
 }
 
 // Rows longer than one CTA's shared memory (2^15 .. 2^20 time samples; the shipped configurations have 2^18):
@@ -1750,21 +1726,21 @@ static bool long_fusable(size_t time_count) {
   return is_pow2(time_count) && q >= 15 && q <= 18 && get_encode_tiled();
 }
 
-static int watfft_long_fused(srtb_b200_ctx* ctx, int slot, float2* x, const float2* src, size_t time_count,
+static int watfft_long_fused(srtb_b200_ctx* ctx, const detect_out& out, float2* x, const float2* src, size_t time_count,
                              size_t chan_count, size_t time_reserved_count, float sk_threshold, float snr,
                              float chan_thr, size_t max_boxcar, const row_chirp_params& chirp) {
-  const size_t ts_count = (time_count <= time_reserved_count) ? time_count : time_count - time_reserved_count;
+  const size_t ts_count = detected_samples(time_count, time_reserved_count);
   const int q = ilog2(time_count);
   const int l1 = (q + 1) / 2, l2 = q - l1;
   const size_t L1 = (size_t)1 << l1, L2 = (size_t)1 << l2;
-  if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, chan_count * time_count * sizeof(float2))) return rc;
-  float2* s = static_cast<float2*>(ctx->lane.fft_scratch);
+  if (int rc = grow(ctx, ctx->lane.fft_scratch, chan_count * time_count * sizeof(float2))) return rc;
+  float2* s = ctx->lane.fft_scratch.p;
   const size_t T_last = (l2 <= 8) ? 16 : 8;  // rows per tile of the last sweep (col_t)
   const size_t tiles_per_row = L1 / T_last;
-  if (int rc = ensure(ctx, &ctx->lane.long_stats, &ctx->lane.long_stats_bytes, chan_count * tiles_per_row * sizeof(float2))) return rc;
-  if (int rc = ensure(ctx, &ctx->lane.long_zap, &ctx->lane.long_zap_bytes, chan_count)) return rc;
-  float2* stats = static_cast<float2*>(ctx->lane.long_stats);
-  unsigned char* zap = static_cast<unsigned char*>(ctx->lane.long_zap);
+  if (int rc = grow(ctx, ctx->lane.long_stats, chan_count * tiles_per_row * sizeof(float2))) return rc;
+  if (int rc = grow(ctx, ctx->lane.long_zap, chan_count)) return rc;
+  float2* stats = ctx->lane.long_stats.p;
+  unsigned char* zap = ctx->lane.long_zap.p;
   row_chirp_params cp = chirp;
   {
     // Newton steps for 1/f between a thread's consecutive points, U * B = (L1 / 16) * L2 bins apart
@@ -1800,15 +1776,16 @@ static int watfft_long_fused(srtb_b200_ctx* ctx, int slot, float2* x, const floa
   CK(cudaGetLastError());
   // partial column sums (all time samples are visited so that flagged rows are zeroed completely)
   const colsum_chunks cg = colsum_geometry(ctx, time_count, chan_count);
-  if (int rc2 = detect_prepare(ctx, slot, time_count, cg.chunks * ts_count)) return rc2;
-  if (!ctx->res_zeroed) CK(cudaMemsetAsync(ctx->d_res + slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
+  if (int rc2 = detect_prepare(ctx, out.slot, time_count, cg.chunks * ts_count)) return rc2;
+  if (!out.header_zeroed) CK(cudaMemsetAsync(ctx->d_res + out.slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
   dim3 g((unsigned)cg.ctas_per_chunk, (unsigned)cg.chunks);
   colsum_partial_kernel<<<g, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, cg.rows_per_chunk,
-                                                         ctx->lane.colsum_partial, zap);
+                                                         ctx->lane.colsum_partial.p, zap);
   ctx->launches++;
   CK(cudaGetLastError());
   stats_.reset();
-  return detect_tail(ctx, slot, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr, max_boxcar);
+  return detect_tail(ctx, out, ctx->lane.colsum_partial.p, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr,
+                     max_boxcar);
 }
 
 static int detect_collect(srtb_b200_ctx* ctx, int slot, srtb_b200_detect_result* h_result, float* h_series,
@@ -1820,7 +1797,7 @@ static int detect_collect(srtb_b200_ctx* ctx, int slot, srtb_b200_detect_result*
     bool any = false;
     for (int b = 0; b < h_result->n_boxcars; b++) {
       if (copy_all || h_result->signal_count[b] > 0) {
-        CK(cudaMemcpyAsync(h_series + (size_t)b * stride, ctx->series[slot] + (size_t)b * stride,
+        CK(cudaMemcpyAsync(h_series + (size_t)b * stride, ctx->series[slot].p + (size_t)b * stride,
                            h_result->series_length[b] * sizeof(float), cudaMemcpyDeviceToHost, ctx->lane.stream));
         any = true;
       }
@@ -1828,7 +1805,7 @@ static int detect_collect(srtb_b200_ctx* ctx, int slot, srtb_b200_detect_result*
     if (any) CK(cudaStreamSynchronize(ctx->lane.stream));
   } else if (h_series && copy_all) {
     // detection disabled: still hand back the mean-removed time series
-    CK(cudaMemcpyAsync(h_series, ctx->series[slot], h_result->time_series_count * sizeof(float),
+    CK(cudaMemcpyAsync(h_series, ctx->series[slot].p, h_result->time_series_count * sizeof(float),
                        cudaMemcpyDeviceToHost, ctx->lane.stream));
     CK(cudaStreamSynchronize(ctx->lane.stream));
   }
@@ -1845,7 +1822,7 @@ extern "C" int srtb_b200_signal_detect(srtb_b200_ctx* ctx, const void* d_x, size
   if (time_count == 0 || chan_count == 0) return fail(ctx, SRTB_B200_E_INVALID, "signal_detect: zero size");
   CK(cudaSetDevice(ctx->device));
   stage_scope stats_(ctx, SRTB_B200_STAGE_SIGNAL_DETECT, 8.0 * (double)time_count * (double)chan_count);
-  if (int rc = detect_enqueue(ctx, 0, static_cast<const float2*>(d_x), time_count, chan_count,
+  if (int rc = detect_enqueue(ctx, detect_out{}, static_cast<const float2*>(d_x), time_count, chan_count,
                               time_reserved_count, snr_threshold, channel_threshold, max_boxcar_length))
     return rc;
   CK(cudaMemcpyAsync(ctx->h_res, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
@@ -1856,8 +1833,8 @@ extern "C" int srtb_b200_signal_detect(srtb_b200_ctx* ctx, const void* d_x, size
 // ---- alternates of the refft path: spectra laid out [time][frequency] ------------------------------------------
 static int sk_v1_enqueue(srtb_b200_ctx* ctx, float2* x, size_t fft_bins, size_t time_counts, float sk_threshold,
                          float* d_sk_out) {
-  if (int rc = ensure(ctx, &ctx->lane.long_zap, &ctx->lane.long_zap_bytes, fft_bins)) return rc;
-  unsigned char* zap = static_cast<unsigned char*>(ctx->lane.long_zap);
+  if (int rc = grow(ctx, ctx->lane.long_zap, fft_bins)) return rc;
+  unsigned char* zap = ctx->lane.long_zap.p;
   const auto [lo_, hi_] = sk_bounds(sk_threshold, time_counts);
   sk_v1_stats_kernel<<<(unsigned)((fft_bins + 31) / 32), 256, 0, ctx->lane.stream>>>(x, fft_bins, time_counts, lo_, hi_, zap, d_sk_out);
   ctx->launches++;
@@ -1894,11 +1871,11 @@ extern "C" int srtb_b200_signal_detect_v1(srtb_b200_ctx* ctx, void* d_x, size_t 
   // batch_size values, masked channels counted over the first spectrum
   if (int rc = detect_prepare(ctx, 0, batch_size, batch_size)) return rc;
   CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result), ctx->lane.stream));
-  rowsum_norm_kernel<<<(unsigned)((batch_size + 7) / 8), 256, 0, ctx->lane.stream>>>(x, count_per_batch, batch_size, ctx->lane.colsum_partial);
+  rowsum_norm_kernel<<<(unsigned)((batch_size + 7) / 8), 256, 0, ctx->lane.stream>>>(x, count_per_batch, batch_size, ctx->lane.colsum_partial.p);
   ctx->launches++;
   CK(cudaGetLastError());
-  if (int rc = detect_tail(ctx, 0, x, batch_size, count_per_batch, batch_size, 1, snr_threshold, channel_threshold,
-                           max_boxcar_length, /*zero_stride=*/1))
+  if (int rc = detect_tail(ctx, detect_out{}, ctx->lane.colsum_partial.p, x, batch_size, count_per_batch, batch_size, 1,
+                           snr_threshold, channel_threshold, max_boxcar_length, /*zero_stride=*/1))
     return rc;
   CK(cudaMemcpyAsync(ctx->h_res, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
   CK(cudaStreamSynchronize(ctx->lane.stream));
@@ -1960,26 +1937,6 @@ static bool raw_sources_for(const srtb_b200_block_config* cfg, const void* d_bas
   return true;
 }
 
-// (re)allocate one set of per-stream working buffers of N + 2 floats (the in-place buffer of the reference's works,
-// unpack_pipe.hpp:65-67) owned by the ctx
-static int ensure_stream_bufs(srtb_b200_ctx* ctx, float* (&bufs)[4], size_t* elems, size_t N, int streams) {
-  if (*elems < N + 2) {
-    if (int rc = sync_lanes(ctx)) return rc;
-    for (auto& p : bufs) {
-      if (p) CK(cudaFree(p));
-      p = nullptr;
-    }
-    *elems = 0;
-  }
-  for (int s = 0; s < streams; s++)
-    if (!bufs[s]) {
-      cudaError_t e = cudaMalloc(&bufs[s], (N + 2) * sizeof(float));
-      if (e != cudaSuccess) return fail(ctx, SRTB_B200_E_NOMEM, "process_block: stream buffer alloc failed");
-    }
-  *elems = N + 2;
-  return 0;
-}
-
 // K12 phase table for the whole-row waterfall kernel (block path; the DM sweep, and tables above 4 GiB, evaluate every
 // phase on the fly). Rebuilt when the geometry or the DM changes; built synchronously, so both lanes and any later
 // launch may read it.
@@ -1989,18 +1946,18 @@ static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params&
   *out = nullptr;
   if (n * sizeof(float) > ((size_t)4 << 30)) return 0;
   const double key[7] = {(double)n, cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm, (double)logp};
-  if (ctx->chirp_tab && std::memcmp(key, ctx->chirp_tab_key, sizeof(key)) == 0) {
-    *out = ctx->chirp_tab;
+  if (ctx->chirp_tab.p && std::memcmp(key, ctx->chirp_tab_key, sizeof(key)) == 0) {
+    *out = ctx->chirp_tab.p;
     return 0;
   }
-  if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->chirp_tab), &ctx->chirp_tab_bytes, n * sizeof(float))) return rc;
+  if (int rc = grow(ctx, ctx->chirp_tab, n * sizeof(float))) return rc;
   if (int rc = sync_lanes(ctx)) return rc;  // a block still in flight may be reading the previous table
-  chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(ctx->chirp_tab, n, cp.f_min, cp.df, cp.inv_fc,
+  chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(ctx->chirp_tab.p, n, cp.f_min, cp.df, cp.inv_fc,
                                                                            cp.f_c, cp.ddm, logp);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(ctx->lane.stream));
   std::memcpy(ctx->chirp_tab_key, key, sizeof(key));
-  *out = ctx->chirp_tab;
+  *out = ctx->chirp_tab.p;
   return 0;
 }
 
@@ -2118,8 +2075,8 @@ static bool r2c_sweep_order(const block_params& p, const block_input& in) {
 static int r2c_sweep_order_stream(srtb_b200_ctx* ctx, const block_params& p, const block_input& in, int s,
                                   float2* spectrum) {
   const size_t P = (size_t)1 << SWEEP_LOGP, Q = (size_t)1 << SWEEP_LOGQ;
-  if (int rc = ensure(ctx, &ctx->lane.fft_scratch, &ctx->lane.fft_scratch_bytes, P * Q * sizeof(float2))) return rc;
-  float2* const z = static_cast<float2*>(ctx->lane.fft_scratch);
+  if (int rc = grow(ctx, ctx->lane.fft_scratch, P * Q * sizeof(float2))) return rc;
+  float2* const z = ctx->lane.fft_scratch.p;
   bool done = false;
   if (int rc = dispatch_col_raw(ctx, (int)SWEEP_LOGP, in.raw[s], z, Q, &done)) return rc;
   if (!done) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "r2c: the raw 2^11-point column sweep refused the block");
@@ -2149,12 +2106,11 @@ static int r2c_stream(srtb_b200_ctx* ctx, const block_params& p, block_input* in
 // spectrum beforehand (0 stays 0 through s1 and the chirp)
 static bool chirp_on_load(size_t L) { return chirp_fusable(L) || long_fusable(L); }
 
-// one stream's chain after its R2C, at one DM: s1 + chirp, waterfall FFT, SK and detector, result header in
-// d_res[slot]. src holds the spectrum, dst receives the dynamic spectrum: the same buffer on the block path, while the
+// one stream's chain after its R2C, at one DM: s1 + chirp, waterfall FFT, SK and detector writing to `out`. src holds the spectrum, dst receives the dynamic spectrum: the same buffer on the block path, while the
 // DM sweep keeps src for the next trial. phase_table: the whole-row kernel may read a tabulated chirp (built for the
 // block's DM; the DM sweep changes DM every trial). Both buffers are 16-byte aligned: the ctx allocates them, or
 // submit_block_ex checked the caller's.
-static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, float2* dst, const float2* src, float dm,
+static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, const detect_out& out, float2* dst, const float2* src, float dm,
                        bool phase_table, unsigned sweep_logp = 0) {
   const srtb_b200_block_config* cfg = p.cfg;
   const size_t reserved = p.reserved(dm);
@@ -2163,7 +2119,7 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
     row_chirp_params cp = p.chirp(dm, ctx->lane.mean);
     if (phase_table)
       if (int rc = get_chirp_table(ctx, p.Nc, cp, &cp.phase, sweep_logp)) return rc;
-    return watfft_sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
+    return watfft_sk_detect_fused(ctx, out, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
                                   cfg->signal_detect_max_boxcar_length, &cp, src, sweep_logp != 0);
   }
@@ -2171,7 +2127,7 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
     // long rows: chirp-on-load column sweep, last sweep with SK statistics, decision, column sums (20 bytes per
     // sample). No phase table here: the long-row column sweep is DRAM-bound, and the 4 extra bytes per bin a table
     // costs outweigh the fp64 evaluation it would replace.
-    const int rc = watfft_long_fused(ctx, slot, dst, src, p.L, p.batch, reserved,
+    const int rc = watfft_long_fused(ctx, out, dst, src, p.L, p.batch, reserved,
                                      cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                      cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
                                      cfg->signal_detect_max_boxcar_length, p.chirp(dm, ctx->lane.mean));
@@ -2183,14 +2139,14 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
   if (p.L == 512) {
     // waterfall FFT + SK + partial column sums in one kernel (the eight-point row kernel has no chirp on load), then
     // the small detector tail
-    return watfft_sk_detect_fused(ctx, slot, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
+    return watfft_sk_detect_fused(ctx, out, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
                                   cfg->signal_detect_max_boxcar_length);
   }
   if (int rc = srtb_b200_watfft_c2c_backward(ctx, dst, p.L, p.batch)) return rc;
   if (int rc = srtb_b200_rfi_s2_sk(ctx, dst, p.L, p.batch, cfg->mitigate_rfi_spectral_kurtosis_threshold, nullptr))
     return rc;
-  return detect_enqueue(ctx, slot, dst, p.L, p.batch, reserved, cfg->signal_detect_signal_noise_threshold,
+  return detect_enqueue(ctx, out, dst, p.L, p.batch, reserved, cfg->signal_detect_signal_noise_threshold,
                         cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length);
 }
 
@@ -2201,12 +2157,11 @@ static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, int slot, floa
 static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* bufs, const float* raw,
                     float* host_series) {
   const srtb_b200_block_config* cfg = p.cfg;
-  const size_t L = p.L, C = p.batch, reserved = p.reserved(cfg->dm);
-  const size_t ts = (L <= reserved) ? L : L - reserved;
+  const size_t L = p.L, C = p.batch;
+  const size_t ts = detected_samples(L, p.reserved(cfg->dm));
   if (int rc = detect_prepare(ctx, SUM_SLOT, L, 1)) return rc;
-  if (int rc = ensure(ctx, &ctx->sum_mask, &ctx->sum_mask_bytes, C * (sizeof(float2) + sizeof(uint2)) + sizeof(unsigned)))
-    return rc;
-  float2* const mask = static_cast<float2*>(ctx->sum_mask);
+  if (int rc = grow(ctx, ctx->sum_mask, C * (sizeof(float2) + sizeof(uint2)) + sizeof(unsigned))) return rc;
+  float2* const mask = ctx->sum_mask.p;
   uint2* const mis = reinterpret_cast<uint2*>(mask + C);
   unsigned* const n_mis = reinterpret_cast<unsigned*>(mis + C);
   stream_sum_inputs in{};
@@ -2218,30 +2173,16 @@ static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* buf
   stream_sum_mask_kernel<<<1, 1024, 0, ctx->lane.stream>>>(in, p.streams, L, C, mask, mis, n_mis);
   ctx->launches++;
   CK(cudaGetLastError());
-  float* const v = ctx->series[SUM_SLOT];
   CK(launch_pdl(ctx, stream_sum_kernel, dim3(grid_for(ctx, ts, 256)), dim3(256), 0, in, p.streams, L, ts,
-                (const uint2*)mis, (const unsigned*)n_mis, v));
+                (const uint2*)mis, (const unsigned*)n_mis, ctx->series[SUM_SLOT].p));
   ctx->launches++;
   CK(cudaGetLastError());
   // the tail counts the mask's zeros (stride 1): the union count. The first lane's ticket and scan buffer are free here:
   // its own stream's tail has finished in stream order.
-  CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>((C + 1023) / 1024, (size_t)ctx->sm_count)),
-                dim3(1024), 0, (const float*)nullptr, ts, (size_t)0, v, ctx->lane.acc, (const float2*)mask, (size_t)1, C,
-                cfg->signal_detect_channel_threshold, (size_t)cfg->signal_detect_max_boxcar_length,
-                ctx->lane.detect_ticket, ctx->d_res + SUM_SLOT, (size_t)0, (size_t)0, (float*)nullptr));
-  ctx->launches++;
-  CK(cudaGetLastError());
-  unsigned max_nb = 1;
-  for (size_t b = 2; b <= cfg->signal_detect_max_boxcar_length && b < ts && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2)
-    max_nb++;
-  float* const host_out = host_series ? host_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * L : nullptr;
-  CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, v, L, (const float*)ctx->lane.acc, ts,
-                cfg->signal_detect_signal_noise_threshold, ctx->d_res + SUM_SLOT, host_out, (detect_dev_peak*)nullptr,
-                (size_t)0, (size_t)0));
-  ctx->launches++;
-  CK(cudaGetLastError());
-  ctx->slot_time_count[SUM_SLOT] = L;
-  return 0;
+  const detect_out out{SUM_SLOT, host_series ? host_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * L : nullptr,
+                       nullptr, nullptr, /*header_zeroed=*/true};
+  return detect_tail(ctx, out, nullptr, mask, L, C, ts, 0, cfg->signal_detect_signal_noise_threshold,
+                     cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length, /*zero_stride=*/1);
 }
 
 // enqueue every stage of one block (no host sync); results land in ctx->h_res[res_base .. res_base + streams) once the
@@ -2254,24 +2195,17 @@ static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* buf
 static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* d_baseband, size_t baseband_bytes,
                          int res_base, float* const* bufs, float* host_series, bool join_lanes = true,
                          bool* alt_used = nullptr) {
-  struct series_dst_scope {  // detect_tail reads ctx->host_series_dst; it is only meaningful inside this call
+  struct pdl_scope {  // launch_pdl reads ctx->pdl_auto; it is only meaningful inside this call
     srtb_b200_ctx* c;
-    ~series_dst_scope() {
-      c->host_series_dst = nullptr;
-      c->raw_dst = nullptr;
-      c->res_zeroed = false;
-      c->pdl_auto = false;
-    }
-  } series_scope_{ctx};
-  ctx->host_series_dst = host_series;
+    ~pdl_scope() { c->pdl_auto = false; }
+  } pdl_scope_{ctx};
   ctx->pdl_auto = p.N <= ((size_t)1 << 25);
   const bool sum = p.cfg->signal_detect_sum_streams != 0;
+  float* raw = nullptr;  // this block's raw column sums [4][L]
   if (sum) {
     const size_t group = (size_t)(res_base / RES_GROUP);
-    if (int rc = ensure(ctx, reinterpret_cast<void**>(&ctx->sum_raw), &ctx->sum_raw_bytes,
-                        (1 + SRTB_B200_RING_SLOTS) * 4 * p.L * sizeof(float)))
-      return rc;
-    ctx->raw_dst = ctx->sum_raw + group * 4 * p.L;
+    if (int rc = grow(ctx, ctx->sum_raw, (1 + SRTB_B200_RING_SLOTS) * 4 * p.L * sizeof(float))) return rc;
+    raw = ctx->sum_raw.p + group * 4 * p.L;
   }
   // the data streams of a block are independent: odd ones go to the context's second lane (per-stage timing wants the
   // kernels alone, so it keeps one lane)
@@ -2284,7 +2218,6 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     // with two lanes every stream zeroes its own header at the head of its chain, on its lane
     CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result) * p.streams, ctx->lane.stream));
   }
-  ctx->res_zeroed = true;
   block_input in{d_baseband, baseband_bytes, bufs};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
   if (two_lanes)
@@ -2293,6 +2226,8 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
   auto enqueue_stream = [&](int s) -> int {
     float2* buf = reinterpret_cast<float2*>(bufs[s]);
     if (two_lanes) CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
+    const detect_out out{s, host_series ? host_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
+                         raw ? raw + (size_t)s * p.L : nullptr, nullptr, /*header_zeroed=*/true};
     if (sweep_order) {
       {
         stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
@@ -2300,7 +2235,7 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
         if (int rc = r2c_sweep_order_stream(ctx, p, in, s, buf)) return rc;
       }
       if (int rc = zero_bin_ranges(ctx, buf, p.bins, SWEEP_LOGP, SWEEP_LOGQ)) return rc;
-      return stream_tail(ctx, p, s, buf, buf, p.cfg->dm, /*phase_table=*/true, SWEEP_LOGP);
+      return stream_tail(ctx, p, out, buf, buf, p.cfg->dm, /*phase_table=*/true, SWEEP_LOGP);
     }
     {
       stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
@@ -2310,7 +2245,7 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     }
     if (chirp_on_load(p.L))
       if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
-    return stream_tail(ctx, p, s, buf, buf, p.cfg->dm, /*phase_table=*/true);
+    return stream_tail(ctx, p, out, buf, buf, p.cfg->dm, /*phase_table=*/true);
   };
   for (int s = 0; s < p.streams; s++) {
     const bool alt = two_lanes && (s & 1);
@@ -2332,7 +2267,7 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     CK(cudaMemcpyAsync(ctx->h_res + res_base, ctx->d_res, sizeof(detect_dev_result) * p.streams, cudaMemcpyDeviceToHost,
                        ctx->lane.stream));
   if (sum) {
-    if (int rc = sum_tail(ctx, p, bufs, ctx->raw_dst, host_series)) return rc;
+    if (int rc = sum_tail(ctx, p, bufs, raw, host_series)) return rc;
     CK(cudaMemcpyAsync(ctx->h_res + res_base + SUM_SLOT, ctx->d_res + SUM_SLOT, sizeof(detect_dev_result),
                        cudaMemcpyDeviceToHost, ctx->lane.stream));
   }
@@ -2348,8 +2283,12 @@ extern "C" int srtb_b200_process_block_device(srtb_b200_ctx* ctx, const srtb_b20
   CK(cudaSetDevice(ctx->device));
   block_params p;
   if (int rc = block_params_for(ctx, cfg, "process_block", &p)) return rc;
-  if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, p.N, p.streams)) return rc;
-  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, 0, ctx->stream_buf, nullptr)) return rc;
+  float* bufs[4] = {};
+  for (int s = 0; s < p.streams; s++) {
+    if (int rc = grow(ctx, ctx->stream_buf[s], (p.N + 2) * sizeof(float))) return rc;
+    bufs[s] = ctx->stream_buf[s].p;
+  }
+  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, 0, bufs, nullptr)) return rc;
   CK(cudaStreamSynchronize(ctx->lane.stream));
   for (int s = 0; s < p.streams; s++)
     if (int rc = detect_collect(ctx, s, h_results + s, h_series ? h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
@@ -2368,9 +2307,9 @@ extern "C" int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block
   API_LOCK(ctx);
   if (!ctx || !cfg || !h_baseband) return fail(ctx, SRTB_B200_E_INVALID, "process_block: null argument");
   CK(cudaSetDevice(ctx->device));
-  if (int rc = ensure(ctx, &ctx->d_baseband, &ctx->d_baseband_bytes, baseband_bytes)) return rc;
-  CK(cudaMemcpyAsync(ctx->d_baseband, h_baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
-  return srtb_b200_process_block_device(ctx, cfg, ctx->d_baseband, baseband_bytes, h_results, h_series, copy_all);
+  if (int rc = grow(ctx, ctx->d_baseband, baseband_bytes)) return rc;
+  CK(cudaMemcpyAsync(ctx->d_baseband.p, h_baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
+  return srtb_b200_process_block_device(ctx, cfg, ctx->d_baseband.p, baseband_bytes, h_results, h_series, copy_all);
 }
 
 // ---- DM sweep on one block (BASELINE config #4): unpack + R2C + mean once per stream, then for every
@@ -2436,52 +2375,48 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
         return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum[" + std::to_string(s) + "] is not 16-byte aligned");
     }
   }
-  struct sweep_scope {  // detect_tail reads these; they are only meaningful inside this call
-    srtb_b200_ctx* c;
-    ~sweep_scope() {
-      c->peak_dst = nullptr;
-      c->host_series_dst = nullptr;
-    }
-  } sweep_scope_{ctx};
   const void* d_baseband = baseband;
   if (!on_device) {
-    if (int rc = ensure(ctx, &ctx->d_baseband, &ctx->d_baseband_bytes, baseband_bytes)) return rc;
-    CK(cudaMemcpyAsync(ctx->d_baseband, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
-    d_baseband = ctx->d_baseband;
+    if (int rc = grow(ctx, ctx->d_baseband, baseband_bytes)) return rc;
+    CK(cudaMemcpyAsync(ctx->d_baseband.p, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
+    d_baseband = ctx->d_baseband.p;
   }
-  if (int rc = ensure_stream_bufs(ctx, ctx->stream_buf, &ctx->stream_buf_elems, p.N, p.streams)) return rc;
-  if (int rc = ensure(ctx, &ctx->sweep_buf, &ctx->sweep_buf_bytes, (p.Nc + 1) * sizeof(float2))) return rc;
-  float2* W = static_cast<float2*>(ctx->sweep_buf);
+  float* bufs[4] = {};
+  for (int s = 0; s < p.streams; s++) {
+    if (int rc = grow(ctx, ctx->stream_buf[s], (p.N + 2) * sizeof(float))) return rc;
+    bufs[s] = ctx->stream_buf[s].p;
+  }
+  if (int rc = grow(ctx, ctx->sweep_buf, (p.Nc + 1) * sizeof(float2))) return rc;
+  float2* W = ctx->sweep_buf.p;
   // every trial's result header is parked on the device and fetched once at the end: no host sync per trial. With
   // outputs, the trials' peak records [n_dm][streams] follow the headers in the same allocation, then each stream's
   // mean(|X|^2), which s1 reads from the lane and the next stream's R2C overwrites
   const size_t n_rec = n_dm * p.streams;
-  if (int rc = ensure(ctx, &ctx->sweep_res, &ctx->sweep_res_bytes,
-                      n_rec * (sizeof(detect_dev_result) + (outputs ? sizeof(detect_dev_peak) : 0)) +
-                          (outputs ? 4 * sizeof(float) : 0)))
+  if (int rc = grow(ctx, ctx->sweep_res,
+                    n_rec * (sizeof(detect_dev_result) + (outputs ? sizeof(detect_dev_peak) : 0)) +
+                        (outputs ? 4 * sizeof(float) : 0)))
     return rc;
-  detect_dev_result* d_sweep = static_cast<detect_dev_result*>(ctx->sweep_res);
+  detect_dev_result* d_sweep = ctx->sweep_res.p;
   detect_dev_peak* const d_peaks = outputs ? reinterpret_cast<detect_dev_peak*>(d_sweep + n_rec) : nullptr;
   float* const d_means = outputs ? reinterpret_cast<float*>(d_peaks + n_rec) : nullptr;
   // zeroed once before the first kernel: a memset between kernels would break the dependent-launch chain
   if (outputs) CK(cudaMemsetAsync(d_peaks, 0, n_rec * sizeof(detect_dev_peak), ctx->lane.stream));
-  block_input in{d_baseband, baseband_bytes, ctx->stream_buf};
+  block_input in{d_baseband, baseband_bytes, bufs};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
   for (int s = 0; s < p.streams; s++) {
     if (int rc = r2c_stream(ctx, p, &in, s, /*fork=*/false)) return rc;
     if (d_means)
       CK(cudaMemcpyAsync(d_means + s, ctx->lane.mean, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
-    float2* buf = reinterpret_cast<float2*>(ctx->stream_buf[s]);
+    float2* buf = reinterpret_cast<float2*>(bufs[s]);
     if (chirp_on_load(p.L))  // the manual zap does not depend on the DM: once, on the kept spectrum
       if (int rc = zero_bin_ranges(ctx, buf, p.bins)) return rc;
     for (size_t j = 0; j < n_dm; j++) {
-      if (d_peaks) ctx->peak_dst = d_peaks + j * p.streams + s;
-      if (int rc = stream_tail(ctx, p, 0, W, buf, h_dms[j], /*phase_table=*/false)) return rc;
+      const detect_out out{0, nullptr, nullptr, d_peaks ? d_peaks + j * p.streams + s : nullptr};
+      if (int rc = stream_tail(ctx, p, out, W, buf, h_dms[j], /*phase_table=*/false)) return rc;
       CK(cudaMemcpyAsync(d_sweep + j * p.streams + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToDevice,
                          ctx->lane.stream));
     }
   }
-  ctx->peak_dst = nullptr;
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
   static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
   CK(cudaMemcpyAsync(h_results, d_sweep, n_rec * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
@@ -2502,15 +2437,13 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
   // the best trial once more per stream, from the kept spectrum: its spectrum to d_spectrum[s], its positive series
   // straight from the detector kernel to h_series' row of the stream, its header to h_res[s]
   for (int s = 0; s < p.streams; s++) {
-    ctx->host_series_dst = outputs->h_series ? outputs->h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr;
+    const detect_out out{0, outputs->h_series ? outputs->h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr};
     float2* dst = user_spec ? reinterpret_cast<float2*>(outputs->d_spectrum[s]) : W;
     CK(cudaMemcpyAsync(ctx->lane.mean, d_means + s, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
-    if (int rc = stream_tail(ctx, p, 0, dst, reinterpret_cast<float2*>(ctx->stream_buf[s]), h_dms[best[s]],
-                             /*phase_table=*/false))
+    if (int rc = stream_tail(ctx, p, out, dst, reinterpret_cast<float2*>(bufs[s]), h_dms[best[s]], /*phase_table=*/false))
       return rc;
     CK(cudaMemcpyAsync(ctx->h_res + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
   }
-  ctx->host_series_dst = nullptr;
   CK(cudaStreamSynchronize(ctx->lane.stream));
   // same kernels on the same input: the re-run must reproduce the loop's header of that trial bit for bit
   for (int s = 0; s < p.streams; s++)
@@ -2644,15 +2577,14 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
     return fail(ctx, SRTB_B200_E_SIZE, "incoherent_dm_search: T = ts - S+ - S- = " +
                                            std::to_string((long long)ts - (long long)span) + " < 2");
   const size_t T = ts - span;
-  unsigned max_nb = 1;
-  for (size_t b = 2; b <= max_boxcar_length && b < T && max_nb < SRTB_B200_MAX_BOXCARS; b *= 2) max_nb++;
+  const unsigned max_nb = boxcar_ctas(max_boxcar_length, T);
   const size_t n_groups = ctx->inc_groups.size();
   // device tables: off [C][n_dm] int, order [n_dm] int, gspan [groups][C] int2, groups [groups] int2
   const size_t off_b = chan_count * n_dm * sizeof(int), order_b = n_dm * sizeof(int);
   const size_t gspan_o = (off_b + order_b + 15) & ~(size_t)15, gspan_b = n_groups * chan_count * sizeof(int2);
   const size_t groups_o = gspan_o + gspan_b, tab_b = groups_o + n_groups * sizeof(int2);
-  if (ctx->inc_tab_bytes < tab_b) ctx->inc_tab_uploaded = false;
-  if (int rc = ensure(ctx, &ctx->inc_tab, &ctx->inc_tab_bytes, tab_b)) return rc;
+  if (ctx->inc_tab.bytes < tab_b) ctx->inc_tab_uploaded = false;
+  if (int rc = grow(ctx, ctx->inc_tab, tab_b)) return rc;
   // work: series [n_dm][max_nb][T], scans [n_dm][T], headers [n_dm], peaks [n_dm], tickets [n_dm]
   const size_t series_stride = (size_t)max_nb * T;
   const size_t series_b = n_dm * series_stride * sizeof(float), acc_b = n_dm * T * sizeof(float);
@@ -2660,9 +2592,9 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   const size_t peak_o = res_o + n_dm * sizeof(detect_dev_result);
   const size_t ticket_o = peak_o + n_dm * sizeof(detect_dev_peak);
   const size_t work_b = ticket_o + n_dm * sizeof(unsigned);
-  if (int rc = ensure(ctx, &ctx->inc_work, &ctx->inc_work_bytes, work_b)) return rc;
-  char* tab = static_cast<char*>(ctx->inc_tab);
-  char* work = static_cast<char*>(ctx->inc_work);
+  if (int rc = grow(ctx, ctx->inc_work, work_b)) return rc;
+  char* tab = ctx->inc_tab.p;
+  char* work = ctx->inc_work.p;
   float* d_series = reinterpret_cast<float*>(work);
   float* d_acc = reinterpret_cast<float*>(work + series_b);
   detect_dev_result* d_res = reinterpret_cast<detect_dev_result*>(work + res_o);
@@ -2766,23 +2698,16 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
       bufs[s] = outputs->d_spectrum[s];
     }
   } else {
-    if (int rc = ensure_stream_bufs(ctx, ctx->slot_stream_buf[slot], &ctx->slot_stream_elems[slot], p.N, p.streams))
-      return rc;
-    for (int s = 0; s < p.streams; s++) bufs[s] = ctx->slot_stream_buf[slot][s];
+    for (int s = 0; s < p.streams; s++) {
+      if (int rc = grow(ctx, ctx->slot_stream_buf[slot][s], (p.N + 2) * sizeof(float))) return rc;
+      bufs[s] = ctx->slot_stream_buf[slot][s].p;
+    }
   }
   float* h_series = outputs ? outputs->h_series : nullptr;
   if (!h_series) {
     const size_t need = (size_t)(p.streams + (cfg->signal_detect_sum_streams ? 1 : 0)) * SRTB_B200_MAX_BOXCARS * p.L;
-    if (ctx->slot_h_series_elems[slot] < need) {
-      if (int rc = sync_lanes(ctx)) return rc;
-      if (ctx->slot_h_series[slot]) CK(cudaFreeHost(ctx->slot_h_series[slot]));
-      ctx->slot_h_series[slot] = nullptr;
-      ctx->slot_h_series_elems[slot] = 0;
-      if (cudaMallocHost(&ctx->slot_h_series[slot], need * sizeof(float)) != cudaSuccess)
-        return fail(ctx, SRTB_B200_E_NOMEM, "submit_block: pinned series buffer alloc failed");
-      ctx->slot_h_series_elems[slot] = need;
-    }
-    h_series = ctx->slot_h_series[slot];
+    if (int rc = grow(ctx, ctx->slot_h_series[slot], need * sizeof(float))) return rc;
+    h_series = ctx->slot_h_series[slot].p;
   }
   const void* d_baseband = baseband;
   if (!on_device) {
@@ -2790,11 +2715,11 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
       CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
       for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) CK(cudaEventCreateWithFlags(&ctx->slot_h2d[i], cudaEventDisableTiming));
     }
-    if (int rc = ensure(ctx, &ctx->slot_baseband[slot], &ctx->slot_baseband_bytes[slot], baseband_bytes)) return rc;
-    CK(cudaMemcpyAsync(ctx->slot_baseband[slot], baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
+    if (int rc = grow(ctx, ctx->slot_baseband[slot], baseband_bytes)) return rc;
+    CK(cudaMemcpyAsync(ctx->slot_baseband[slot].p, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
     CK(cudaEventRecord(ctx->slot_h2d[slot], ctx->copy_stream));
     CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->slot_h2d[slot], 0));
-    d_baseband = ctx->slot_baseband[slot];
+    d_baseband = ctx->slot_baseband[slot].p;
   }
   bool alt_used = false;
   if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, RES_GROUP * (1 + slot), bufs, h_series, /*join_lanes=*/false,
@@ -2860,13 +2785,13 @@ extern "C" int srtb_b200_collect_block(srtb_b200_ctx* ctx, int ticket, srtb_b200
 
 extern "C" const void* srtb_b200_block_spectrum(const srtb_b200_ctx* ctx, int stream) {
   if (!ctx || stream < 0 || stream >= 4) return nullptr;
-  return ctx->stream_buf[stream];
+  return ctx->stream_buf[stream].p;
 }
 
 // every trial of a DM sweep writes its dynamic spectrum into sweep_buf; the last one written stays there
 extern "C" const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx) {
   if (!ctx) return nullptr;
-  return ctx->sweep_buf;
+  return ctx->sweep_buf.p;
 }
 
 // ------------------------------------------------------------------------------------
@@ -2892,29 +2817,25 @@ extern "C" int srtb_b200_simplify_spectrum(srtb_b200_ctx* ctx, const void* d_spe
   if (tiles > 65535) return fail(ctx, SRTB_B200_E_INVALID, "simplify_spectrum: out_width too large for this in_width");
   const size_t n = out_width * out_height;
   const unsigned col_grid = (unsigned)std::min<size_t>(1024, (n + THUMB_THREADS - 1) / THUMB_THREADS);
-  void* rows = ctx->thumb_rows;
-  if (int rc = ensure(ctx, &rows, &ctx->thumb_rows_bytes, sizeof(float) * in_height * out_width)) return rc;
-  ctx->thumb_rows = static_cast<float*>(rows);
-  void* part = ctx->thumb_partial;
-  if (int rc = ensure(ctx, &part, &ctx->thumb_partial_bytes, sizeof(float) * col_grid)) return rc;
-  ctx->thumb_partial = static_cast<float*>(part);
+  if (int rc = grow(ctx, ctx->thumb_rows, sizeof(float) * in_height * out_width)) return rc;
+  if (int rc = grow(ctx, ctx->thumb_partial, sizeof(float) * col_grid)) return rc;
 
   const float2* spec = static_cast<const float2*>(d_spectrum);
   const dim3 row_grid((unsigned)in_height, (unsigned)tiles);
   if (in_width % 2 == 0 && (reinterpret_cast<uintptr_t>(d_spectrum) & 15u) == 0)
     thumb_row_kernel<true><<<row_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(spec, in_width, out_width, G,
-                                                                           ctx->thumb_rows);
+                                                                           ctx->thumb_rows.p);
   else
     thumb_row_kernel<false><<<row_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(spec, in_width, out_width, G,
-                                                                            ctx->thumb_rows);
+                                                                            ctx->thumb_rows.p);
   ctx->launches++;
   CK(cudaGetLastError());
-  thumb_col_kernel<<<col_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(ctx->thumb_rows, in_height, out_width, out_height,
-                                                                     d_intensity, ctx->thumb_partial);
+  thumb_col_kernel<<<col_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(ctx->thumb_rows.p, in_height, out_width, out_height,
+                                                                     d_intensity, ctx->thumb_partial.p);
   ctx->launches++;
   CK(cudaGetLastError());
   thumb_norm_kernel<<<grid_for(ctx, n, THUMB_THREADS, 4), THUMB_THREADS, 0, ctx->lane.stream>>>(
-      d_intensity, n, ctx->thumb_partial, (int)col_grid, argb_0, argb_1, argb_overflow, d_pixmap, d_average);
+      d_intensity, n, ctx->thumb_partial.p, (int)col_grid, argb_0, argb_1, argb_overflow, d_pixmap, d_average);
   ctx->launches++;
   CK(cudaGetLastError());
   return 0;
@@ -2982,7 +2903,8 @@ extern "C" int srtb_b200_correlate(srtb_b200_ctx* ctx, const void* d_in_1, const
   if (N > ((size_t)1 << 31))
     return fail(ctx, SRTB_B200_E_SIZE, "correlate: real_count " + std::to_string(N) + " above 2^31 samples not supported");
   CK(cudaSetDevice(ctx->device));
-  if (int rc = ensure_stream_bufs(ctx, ctx->corr_buf, &ctx->corr_buf_elems, N, 2)) return rc;
+  for (auto& b : ctx->corr_buf)
+    if (int rc = grow(ctx, b, (N + 2) * sizeof(float))) return rc;
   // std::pow(input_size, -1.5) in double, stored as float (correlator.cpp:59): an odd input_size counts (q13)
   const float norm = static_cast<float>(std::pow(static_cast<double>(input_size), -1.5));
   // each input is one SIMPLE stream of unsigned 8-bit samples without a window: the block path's R2C, with the unpack
@@ -2998,14 +2920,14 @@ extern "C" int srtb_b200_correlate(srtb_b200_ctx* ctx, const void* d_in_1, const
   p.N = N;
   const void* inputs[2] = {d_in_1, d_in_2};
   for (int s = 0; s < 2; s++) {
-    float* const bufs[4] = {ctx->corr_buf[s], nullptr, nullptr, nullptr};
+    float* const bufs[4] = {ctx->corr_buf[s].p, nullptr, nullptr, nullptr};
     block_input in{inputs[s], N, bufs};
     if (int rc = block_input_init(ctx, p, &in)) return rc;
     if (int rc = r2c_stream(ctx, p, &in, 0, /*fork=*/false)) return rc;
   }
   // (1) cross spectrum over X1 (the Nyquist bin is dropped), (2) unnormalised backward C2C of M points, (3) |y|
-  float2* x1 = reinterpret_cast<float2*>(ctx->corr_buf[0]);
-  if (int rc = launch_cross_spectrum(ctx, x1, reinterpret_cast<const float2*>(ctx->corr_buf[1]), M, norm, x1)) return rc;
+  float2* x1 = reinterpret_cast<float2*>(ctx->corr_buf[0].p);
+  if (int rc = launch_cross_spectrum(ctx, x1, reinterpret_cast<const float2*>(ctx->corr_buf[1].p), M, norm, x1)) return rc;
   if (int rc = fft_c2c_impl<false>(ctx, x1, M, 1)) return rc;
   return launch_magnitude(ctx, x1, M, d_out);
 }
@@ -3052,13 +2974,13 @@ extern "C" int srtb_b200_correlate_accumulate(srtb_b200_ctx* ctx, const void* d_
   CK(cudaSetDevice(ctx->device));
   const size_t Ls = segment_size, Ms = Ls / 2, rows = (n_segments + 1) / 2;  // rows per input
   const int log_ls = ilog2(Ls);
-  if (int rc = ensure(ctx, &ctx->corr_rows, &ctx->corr_rows_bytes, 2 * rows * Ls * sizeof(float2))) return rc;
+  if (int rc = grow(ctx, ctx->corr_rows, 2 * rows * Ls * sizeof(float2))) return rc;
   const unsigned target = (unsigned)ctx->sm_count * 8;  // resident 256-thread CTAs of the whole GPU
   if (!ctx->corr_tickets) {
     CK(cudaMalloc(&ctx->corr_tickets, target * sizeof(unsigned)));
     CK(cudaMemsetAsync(ctx->corr_tickets, 0, target * sizeof(unsigned), ctx->lane.stream));
   }
-  float2* z = static_cast<float2*>(ctx->corr_rows);
+  float2* z = ctx->corr_rows.p;
   int rc = 0;
   switch (bits) {
     case 1: rc = launch_corr_pack<1>(ctx, d_in_1, d_in_2, log_ls, n_segments, rows, z); break;
@@ -3079,8 +3001,8 @@ extern "C" int srtb_b200_correlate_accumulate(srtb_b200_ctx* ctx, const void* d_
   groups = (rows + rows_per_group - 1) / rows_per_group;
   double2* partial = nullptr;
   if (groups > 1) {
-    if (int rc2 = ensure(ctx, &ctx->corr_partial, &ctx->corr_partial_bytes, groups * Ms * sizeof(double2))) return rc2;
-    partial = static_cast<double2*>(ctx->corr_partial);
+    if (int rc2 = grow(ctx, ctx->corr_partial, groups * Ms * sizeof(double2))) return rc2;
+    partial = ctx->corr_partial.p;
   }
   corr_split_accumulate_kernel<<<dim3((unsigned)tiles, (unsigned)groups), 256, 0, ctx->lane.stream>>>(
       z, log_ls, log_bt, rows, n_segments, rows_per_group, partial, ctx->corr_tickets, static_cast<double2*>(d_acc),
@@ -3102,11 +3024,11 @@ extern "C" int srtb_b200_correlate_finish(srtb_b200_ctx* ctx, const void* d_acc,
   if (int rc = check_segment_size(ctx, "correlate_finish", segment_size)) return rc;
   CK(cudaSetDevice(ctx->device));
   const size_t Ms = segment_size / 2;
-  if (int rc = ensure(ctx, &ctx->corr_rows, &ctx->corr_rows_bytes, Ms * sizeof(float2))) return rc;
+  if (int rc = grow(ctx, ctx->corr_rows, Ms * sizeof(float2))) return rc;
   // the reference's norm with Ls in place of input_size, rounded to float, then over the segment count in float64
   const float norm = static_cast<float>(std::pow(static_cast<double>(segment_size), -1.5));
   const double scale = static_cast<double>(norm) / static_cast<double>(total_segments);
-  float2* y = static_cast<float2*>(ctx->corr_rows);
+  float2* y = ctx->corr_rows.p;
   corr_scale_kernel<<<grid_for(ctx, Ms, 256), 256, 0, ctx->lane.stream>>>(static_cast<const double2*>(d_acc), Ms,
                                                                            scale, y);
   ctx->launches++;
