@@ -50,6 +50,14 @@ struct configs {
   // the channels no stream masks: sqrt(2) the S/N of either polarisation for an unpolarised pulse. Needs a format of
   // two or more streams; not with dm_list or incoherent_dm_list
   bool signal_detect_sum_polarizations = false;
+  // fold every block of a recording at a known pulsar period (seconds; 0 = off) with derivative fold_period_derivative
+  // (s/s) into fold_bin_count phase bins and fold_subband_count subbands of consecutive channels; subintegrations of
+  // fold_subintegration_blocks blocks (0 = one for the whole run). Phase and time reference: include/srtb_b200.h
+  double fold_period = 0;
+  double fold_period_derivative = 0;
+  size_t fold_bin_count = 256;
+  size_t fold_subband_count = 1;
+  size_t fold_subintegration_blocks = 0;
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

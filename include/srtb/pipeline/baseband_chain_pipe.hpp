@@ -21,6 +21,7 @@
 #include "srtb/cuda_queue.hpp"
 #include "srtb/log.hpp"
 #include "srtb/memory.hpp"
+#include "srtb/pipeline/fold_pipe.hpp"            // fold_block_step
 #include "srtb/pipeline/rfi_mitigation_pipe.hpp"  // srtb::spectrum::eval_rfi_ranges
 #include "srtb/pipeline/unpack_pipe.hpp"          // resolve_format_alias
 #include "srtb/program_options.hpp"               // parse_dm_list
@@ -170,6 +171,9 @@ class baseband_chain_pipe {
     srtb_b200_detect_result res[5];
     const int n = srtb_b200_collect_block_ex(q.ctx(), p.ticket, res, nullptr, nullptr);
     q.check(n);
+    // fold_period: the block's fold, for the sink's accumulator (blocks not read from a file are not folded)
+    std::shared_ptr<const srtb::work::fold_block> fold;
+    if (srtb::config.fold_period != 0 && p.work.first_sample != p.work.no_first_sample) fold = fold_front(p);
     bool sum_positive = false;
     if (p.sum)
       for (int b = 0; b < res[n].n_boxcars; b++) sum_positive = sum_positive || res[n].signal_count[b] > 0;
@@ -187,6 +191,7 @@ class baseband_chain_pipe {
       w.zero_count = res[s].zero_count;
       w.ptr = p.d_spectrum[s];
       w.sum_positive = sum_positive;
+      if (s == 0) w.fold = fold;
       if (p.sum && s == 0) {
         w.carries_sum = true;
         w.sum_zero_count = res[n].zero_count;
@@ -199,6 +204,31 @@ class baseband_chain_pipe {
         incoherent_search(w, p, s, res[s], inc_dms, h_inc);
       out.push_back(std::move(w));
     }
+  }
+
+  /** folds the block's streams at fold_period: the first min(block step, samples read) / (2C) spectrum samples */
+  std::shared_ptr<const srtb::work::fold_block> fold_front(const pending_block& p) {
+    const auto& c = srtb::config;
+    const uint64_t two_c = 2 * (uint64_t)p.C, step = fold_block_step();
+    auto f = std::make_shared<srtb::work::fold_block>();
+    f->block_index = p.work.first_sample / step;
+    f->first_sample = p.work.first_sample;
+    f->streams = (size_t)p.streams;
+    f->subbands = c.fold_subband_count;
+    f->bins = c.fold_bin_count;
+    f->profile.assign(f->streams * f->subbands * f->bins, 0.0);
+    f->hits.assign(f->bins, 0);
+    f->kept.assign(f->streams * f->subbands, 0);
+    const size_t fold_count = (size_t)std::min<uint64_t>(std::min(step, p.work.valid_samples) / two_c, p.L);
+    if (fold_count == 0) return f;  // nothing read past the previous block's share: an empty fold keeps the order
+    double phi0 = 0, a = 0, b = 0;
+    q.check(srtb_b200_fold_phase(c.fold_period, c.fold_period_derivative, c.baseband_sample_rate, two_c,
+                                 p.work.first_sample, &phi0, &a, &b));
+    const void* spectra[4] = {};
+    for (int s = 0; s < p.streams; s++) spectra[s] = p.d_spectrum[s].get();
+    q.check(srtb_b200_fold(q.ctx(), spectra, p.streams, p.L, p.C, fold_count, phi0, a, b, f->bins, f->subbands,
+                           f->profile.data(), f->hits.data(), f->kept.data()));
+    return f;
   }
 
   /** the incoherent search of stream s's spectrum: fills w's DM-search fields as dm_sweep_chain_pipe does (best trial's

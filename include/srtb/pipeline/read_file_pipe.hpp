@@ -60,7 +60,13 @@ class read_file_pipe {
                                      srtb::BITS_PER_BYTE * streams;
     auto h_in = srtb::host_allocator.allocate_shared<std::byte>(time_sample_bytes);
     std::memset(h_in.get(), 0, time_sample_bytes);
+    // the block's place in the recording, in samples per stream: bytes * 8 / (|bits| * streams)
+    const uint64_t bits_per_sample = static_cast<uint64_t>(std::abs(srtb::config.baseband_input_bits)) * streams;
+    const uint64_t first_sample =
+        (uint64_t)(logical_file_pos - (std::streamoff)srtb::config.input_file_offset_bytes) * srtb::BITS_PER_BYTE /
+        bits_per_sample;
     input_file_stream.read(reinterpret_cast<char*>(h_in.get()), (std::streamsize)time_sample_bytes);
+    const uint64_t valid_samples = (uint64_t)input_file_stream.gcount() * srtb::BITS_PER_BYTE / bits_per_sample;
     const bool hit_eof = input_file_stream.eof();
     logical_file_pos += (std::streamoff)time_sample_bytes;
 
@@ -87,6 +93,8 @@ class read_file_pipe {
                       .count();
     w.udp_packet_counter = w.no_udp_packet_counter;
     w.data_stream_id = 0;
+    w.first_sample = first_sample;
+    w.valid_samples = valid_samples;
     block_counter++;
     return w;
   }

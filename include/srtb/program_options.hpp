@@ -238,7 +238,8 @@ inline const std::vector<std::string>& known_options() {
       "dedisperse_measurement", "fft_fftw_wisdom_path", "mitigate_rfi_average_method_threshold",
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length",
-      "signal_detect_sum_polarizations"};
+      "signal_detect_sum_polarizations", "fold_period", "fold_period_derivative", "fold_bin_count",
+      "fold_subband_count", "fold_subintegration_blocks"};
   return names;
 }
 
@@ -372,6 +373,11 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(signal_detect_channel_threshold)
   SRTB_PARSE(signal_detect_max_boxcar_length)
   SRTB_PARSE(signal_detect_sum_polarizations)
+  SRTB_PARSE(fold_period)
+  SRTB_PARSE(fold_period_derivative)
+  SRTB_PARSE(fold_bin_count)
+  SRTB_PARSE(fold_subband_count)
+  SRTB_PARSE(fold_subintegration_blocks)
   SRTB_PARSE(thread_query_work_wait_time)
   SRTB_PARSE(gui_enable)
   SRTB_PARSE(gui_pixmap_width)
@@ -410,6 +416,35 @@ inline void check_sum_polarizations(const srtb::configs& config, size_t streams)
   if (!trim(config.incoherent_dm_list).empty())
     throw std::invalid_argument("[program_options] signal_detect_sum_polarizations and incoherent_dm_list are both set: "
                                 "the incoherent search has no total-intensity detector");
+}
+
+/** folding (fold_period != 0) at start-up: a finite, positive period of at least two spectrum samples (2 dt, dt =
+ *  2C / baseband_sample_rate with C = min(spectrum_channel_count, baseband_input_count / 2)), 1 to 4096 bins, a subband
+ *  count that divides C, no dm_list (the sweep gives each stream another DM) and a recording to fold (input_file_path) */
+inline void check_fold(const srtb::configs& config) {
+  if (config.fold_period == 0) return;
+  const double P = config.fold_period;
+  if (!std::isfinite(P) || P < 0 || !std::isfinite(config.fold_period_derivative))
+    throw std::invalid_argument("[program_options] fold_period = " + std::to_string(P) + ", fold_period_derivative = " +
+                                std::to_string(config.fold_period_derivative) +
+                                ": the period must be finite and positive, its derivative finite");
+  const size_t C = std::min<size_t>(config.spectrum_channel_count, config.baseband_input_count / 2);
+  const double dt = 2.0 * (double)C / (double)config.baseband_sample_rate;
+  if (!(P >= 2 * dt))
+    throw std::invalid_argument("[program_options] fold_period = " + std::to_string(P) +
+                                " s is shorter than two spectrum samples (2 dt = " + std::to_string(2 * dt) +
+                                " s; dt = 2 spectrum_channel_count / baseband_sample_rate)");
+  if (config.fold_bin_count < 1 || config.fold_bin_count > 4096)
+    throw std::invalid_argument("[program_options] fold_bin_count = " + std::to_string(config.fold_bin_count) +
+                                " is outside 1..4096");
+  if (config.fold_subband_count == 0 || C % config.fold_subband_count)
+    throw std::invalid_argument("[program_options] fold_subband_count = " + std::to_string(config.fold_subband_count) +
+                                " does not divide the " + std::to_string(C) + " channels (spectrum_channel_count)");
+  if (!trim(config.dm_list).empty())
+    throw std::invalid_argument("[program_options] fold_period and dm_list are both set: the DM sweep hands out a "
+                                "different DM per stream, fold at one dm instead");
+  if (trim(config.input_file_path).empty())
+    throw std::invalid_argument("[program_options] fold_period needs input_file_path: only recordings are folded");
 }
 
 inline void apply_changed_configs(const std::map<std::string, std::string>& changed, srtb::configs& config) {

@@ -139,6 +139,12 @@ struct work {
   uint64_t udp_packet_counter = static_cast<uint64_t>(-1);
   uint32_t data_stream_id = 0;
   static constexpr uint64_t no_udp_packet_counter = static_cast<uint64_t>(-1);
+  // the block's place in a recording, in baseband samples per stream (read_file_pipe): its first sample, counted from
+  // input_file_offset_bytes, and the samples actually read (the rest of the block is zero fill). Blocks from other
+  // sources keep no_first_sample and are never folded
+  static constexpr uint64_t no_first_sample = static_cast<uint64_t>(-1);
+  uint64_t first_sample = no_first_sample;
+  uint64_t valid_samples = 0;
   baseband_data_holder baseband_data;
 
   template <typename U>
@@ -146,6 +152,8 @@ struct work {
     timestamp = other.timestamp;
     udp_packet_counter = other.udp_packet_counter;
     data_stream_id = other.data_stream_id;
+    first_sample = other.first_sample;
+    valid_samples = other.valid_samples;
     baseband_data = std::move(other.baseband_data);
   }
   template <typename U>
@@ -153,6 +161,8 @@ struct work {
     timestamp = other.timestamp;
     udp_packet_counter = other.udp_packet_counter;
     data_stream_id = other.data_stream_id;
+    first_sample = other.first_sample;
+    valid_samples = other.valid_samples;
     baseband_data = other.baseband_data;
   }
 };
@@ -195,6 +205,16 @@ struct dm_trial_summary {
   std::vector<boxcar> boxcars;
 };
 
+/** one block folded at fold_period: where it lies in the recording and what srtb_b200_fold returned for it */
+struct fold_block {
+  uint64_t block_index = 0;   // first_sample / (N - R): blocks tile the recording in steps of N - R samples
+  uint64_t first_sample = 0;
+  size_t streams = 0, subbands = 0, bins = 0;
+  std::vector<double> profile;  // [streams][subbands][bins]
+  std::vector<uint64_t> hits;   // [bins]
+  std::vector<uint32_t> kept;   // [streams][subbands]
+};
+
 struct write_signal_work : public write_file_work {
   std::vector<time_series_holder> time_series;  // non-empty <=> has_signal
   size_t zero_count = 0;
@@ -208,6 +228,8 @@ struct write_signal_work : public write_file_work {
   // DM search only (dm_sweep_chain_pipe): the best trial's DM, which ptr and time_series belong to, and every trial
   srtb::real dm = 0;
   std::vector<dm_trial_summary> dm_trials;
+  // fold_period: the block's fold (srtb_b200_fold), carried by the block's first stream
+  std::shared_ptr<const fold_block> fold;
 };
 
 /** a [batch_size][count] complex dynamic spectrum on the device, to be turned into a waterfall thumbnail

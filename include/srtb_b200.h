@@ -356,6 +356,47 @@ int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, s
                                    srtb_b200_peak* h_peaks /* [n_dm] or NULL */, int32_t* h_best_trial /* or NULL */,
                                    float* h_series /* [SRTB_B200_MAX_BOXCARS][T] or NULL */);
 
+/* ---- folding at a known pulsar period --------------------------------------------------------------------------
+ * Time of a spectrum sample. A block whose first baseband sample (per stream) is first_sample holds the spectrum
+ * samples j < L at t_j = (first_sample + 2C j) / sample_rate; t = 0 is the first sample after input_file_offset_bytes.
+ * Times are topocentric, and an arrival is referred to the chirp's f_c (the band edge coherent dedispersion aligns to).
+ * Phase model. Constant period P with derivative Pdot: phi(t) = t/P - 1/2 (Pdot/P^2) t^2. Around a block it is exactly
+ *   phi_j = phi0 + a j + b j^2,  phi0 = frac(phi(t_0)),  a = (1/P - Pdot t_0/P^2) D,  b = -1/2 (Pdot/P^2) D^2,
+ * with D = 2C / sample_rate. srtb_b200_fold_phase computes them in float64, in exactly this order (q = Pdot / (P P)):
+ *   t0 = first_sample / sample_rate; phi = t0 / P - (0.5 q) (t0 t0); phi0 = phi - floor(phi);
+ *   a = (1 / P - q t0) (2C / sample_rate); b = (-0.5 q) (D D).
+ * A period or sample_rate that is not finite and positive, a non-finite Pdot, a zero 2C or a null output returns
+ * SRTB_B200_E_INVALID. */
+int srtb_b200_fold_phase(double period, double period_derivative, double sample_rate,
+                         uint64_t samples_per_spectrum_sample /* 2C */, uint64_t first_sample, double* phi0, double* a,
+                         double* b);
+/* Bin of a sample, with every float64 operation rounded on its own (no FMA contraction):
+ *   p = (phi0 + a j) + b (j j);  f = p - floor(p);  bin = min(floor(f nbin), nbin - 1).
+ * The samples j < fold_count of each stream's d_spectra[s] ([chan_count][time_count] complex64, time contiguous) are
+ * folded; with nsub subbands of chan_count / nsub consecutive channels the call returns
+ *   h_profile[s][k][bin] = sum over the channels of subband k and the j in bin of |x_s[c][j]|^2   (float64),
+ *   h_hits[bin]          = the number of j < fold_count in bin,
+ *   h_kept[s][k]         = the channels of subband k with |x_s[c][0]|^2 != 0 (the detector's zero_count rule: a masked
+ *                          channel adds zeros to the profile and nothing to kept).
+ * The block path folds fold_count = min((N - R) / (2C), valid_samples / (2C)) samples: the first N - R baseband samples,
+ * which the overlap-save leaves uncorrupted and consecutive blocks tile without overlap (R = the reader's rewind).
+ * |x|^2 is formed in fp32 and summed in float64 in a fixed order: two calls agree bit for bit. The spectra are only read
+ * (S C fold_count 8 bytes), in at most three kernel launches whatever streams, nsub and nbin. Stream-ordered on the
+ * ctx's stream; synchronises it once before it returns.
+ * Before any launch: a null ctx, d_spectra, spectrum or output, a zero time_count or chan_count, streams outside 1..4,
+ * a spectrum that is not 8-byte aligned or a non-finite phi0, a or b returns SRTB_B200_E_INVALID; fold_count of 0 or
+ * above time_count, nbin outside 1..SRTB_B200_FOLD_MAX_BINS, nsub not dividing chan_count, chan_count above 2^24 or
+ * fold_count above 2^40 returns SRTB_B200_E_SIZE.
+ * Scratch the ctx grows on demand and keeps, with G = the largest divisor of chan_count / nsub up to 64,
+ * K = streams chan_count / G CTAs and R = min(ceil(fold_count / 2048), max(1, floor(4 SMs / K))) tile ranges each:
+ * 4 ceil(fold_count / 2048) 2048 + 8 nbin + 8 streams nsub nbin + 4 streams nsub bytes, plus 8 K R nbin + 4 K bytes
+ * when (chan_count / nsub / G) R > 1 (each part rounded up to 256 bytes). */
+#define SRTB_B200_FOLD_MAX_BINS 4096
+int srtb_b200_fold(srtb_b200_ctx* ctx, const void* const* d_spectra /* [streams] */, int streams, size_t time_count,
+                   size_t chan_count, size_t fold_count, double phi0, double a, double b, size_t nbin, size_t nsub,
+                   double* h_profile /* [streams][nsub][nbin] */, uint64_t* h_hits /* [nbin] */,
+                   uint32_t* h_kept /* [streams][nsub] */);
+
 /* simplify_spectrum_pipe_2 (pipeline/spectrum_pipe.hpp:82-143): resample_spectrum_3 with norm(),
  * normalize_with_average_value, generate_pixmap. d_spectrum is [in_height][in_width] complex64
  * (time contiguous, as a block leaves it); d_intensity [out_height][out_width] floats receives the

@@ -26,6 +26,7 @@
 #include "correlator.cuh"
 #include "incoherent.cuh"
 #include "stream_sum.cuh"
+#include "fold.cuh"
 
 using namespace srtb_b200;
 
@@ -158,6 +159,8 @@ struct srtb_b200_ctx {
   unsigned inc_spread = 0;                         // largest max - min of any group and channel
   bool inc_tab_uploaded = false;
   buffer<char> inc_tab, inc_work;
+  // fold: the sorted bin plan, hits, profile and kept, and the per-CTA rows fold_finish_kernel adds (srtb_b200_fold)
+  buffer<char> fold_work;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -2656,6 +2659,107 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
     any = true;
   }
   if (any) CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// ---- fold at a pulsar period (fold.cuh): the bin plan of each time tile, one read of the spectra into per-CTA bin
+// rows, and the rows' sum in a fixed order.
+
+extern "C" int srtb_b200_fold_phase(double period, double period_derivative, double sample_rate,
+                                    uint64_t samples_per_spectrum_sample, uint64_t first_sample, double* phi0,
+                                    double* a, double* b) {
+  if (!phi0 || !a || !b || samples_per_spectrum_sample == 0)
+    return fail(nullptr, SRTB_B200_E_INVALID, "fold_phase: bad argument");
+  if (!std::isfinite(period) || !(period > 0) || !std::isfinite(period_derivative) || !std::isfinite(sample_rate) ||
+      !(sample_rate > 0))
+    return fail(nullptr, SRTB_B200_E_INVALID, "fold_phase: period and sample_rate must be finite and positive, "
+                                              "period_derivative finite");
+  // the order of every operation is part of the definition (include/srtb_b200.h)
+  const double t0 = (double)first_sample / sample_rate;
+  const double q = period_derivative / (period * period);
+  const double phi = t0 / period - (0.5 * q) * (t0 * t0);
+  const double delta = (double)samples_per_spectrum_sample / sample_rate;
+  *phi0 = phi - std::floor(phi);
+  *a = (1.0 / period - q * t0) * delta;
+  *b = (-0.5 * q) * (delta * delta);
+  return 0;
+}
+
+extern "C" int srtb_b200_fold(srtb_b200_ctx* ctx, const void* const* d_spectra, int streams, size_t time_count,
+                              size_t chan_count, size_t fold_count, double phi0, double a, double b, size_t nbin,
+                              size_t nsub, double* h_profile, uint64_t* h_hits, uint32_t* h_kept) {
+  API_LOCK(ctx);
+  if (!ctx || !d_spectra || !h_profile || !h_hits || !h_kept || time_count == 0 || chan_count == 0)
+    return fail(ctx, SRTB_B200_E_INVALID, "fold: bad argument");
+  if (streams < 1 || streams > 4) return fail(ctx, SRTB_B200_E_INVALID, "fold: streams must be 1 to 4");
+  fold_spectra sp{};
+  for (int s = 0; s < streams; s++) {
+    if (!d_spectra[s]) return fail(ctx, SRTB_B200_E_INVALID, "fold: spectrum " + std::to_string(s) + " is null");
+    if (!aligned8(d_spectra[s]))
+      return fail(ctx, SRTB_B200_E_INVALID, "fold: spectrum " + std::to_string(s) + " is not 8-byte aligned");
+    sp.x[s] = static_cast<const float2*>(d_spectra[s]);
+  }
+  if (fold_count == 0 || fold_count > time_count)
+    return fail(ctx, SRTB_B200_E_SIZE, "fold: fold_count must be 1 to time_count");
+  if (nbin < 1 || nbin > (size_t)FOLD_MAX_BINS) return fail(ctx, SRTB_B200_E_SIZE, "fold: nbin must be 1 to 4096");
+  if (nsub == 0 || chan_count % nsub) return fail(ctx, SRTB_B200_E_SIZE, "fold: nsub must divide chan_count");
+  if (chan_count > ((size_t)1 << 24) || fold_count > ((size_t)1 << 40))
+    return fail(ctx, SRTB_B200_E_SIZE, "fold: chan_count above 2^24 or fold_count above 2^40");
+  if (!std::isfinite(phi0) || !std::isfinite(a) || !std::isfinite(b))
+    return fail(ctx, SRTB_B200_E_INVALID, "fold: a phase coefficient is not finite");
+  CK(cudaSetDevice(ctx->device));
+  const size_t C = chan_count, S = (size_t)streams, csub = C / nsub;
+  size_t G = std::min<size_t>(csub, FOLD_MAX_GROUP);
+  while (csub % G) G--;  // channels per CTA: the largest divisor of the subband width up to FOLD_MAX_GROUP
+  const size_t ntiles = (fold_count + FOLD_TILE - 1) / FOLD_TILE, ctas = S * (C / G);
+  // tile ranges per channel group: up to one wave of four CTAs per SM (nsub = 1 then still spreads over the SMs)
+  const size_t target = (size_t)ctx->sm_count * 4;
+  const size_t R = std::max<size_t>(1, std::min<size_t>(ntiles, target / ctas));
+  const size_t gps = csub / G, rows_per_output = gps * R, outputs = S * nsub * nbin;
+  // scratch: plan u32 [ntiles][FOLD_TILE], hits u64 [nbin], profile f64 [outputs], kept u32 [S nsub]; with more than
+  // one CTA row per output also rows f64 [ctas R nbin] and kept rows u32 [ctas]
+  const auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
+  const size_t hits_o = up(ntiles * FOLD_TILE * sizeof(uint32_t));
+  const size_t prof_o = hits_o + up(nbin * sizeof(uint64_t));
+  const size_t kept_o = prof_o + up(outputs * sizeof(double));
+  const size_t rows_o = kept_o + up(S * nsub * sizeof(uint32_t));
+  const bool finish = rows_per_output > 1;
+  const size_t krow_o = rows_o + (finish ? up(ctas * R * nbin * sizeof(double)) : 0);
+  const size_t work_b = krow_o + (finish ? ctas * sizeof(uint32_t) : 0);
+  if (int rc = grow(ctx, ctx->fold_work, work_b)) return rc;
+  char* w = ctx->fold_work.p;
+  uint32_t* d_plan = reinterpret_cast<uint32_t*>(w);
+  unsigned long long* d_hits = reinterpret_cast<unsigned long long*>(w + hits_o);
+  double* d_prof = reinterpret_cast<double*>(w + prof_o);
+  unsigned* d_kept = reinterpret_cast<unsigned*>(w + kept_o);
+  double* d_rows = finish ? reinterpret_cast<double*>(w + rows_o) : d_prof;
+  unsigned* d_krows = finish ? reinterpret_cast<unsigned*>(w + krow_o) : d_kept;
+  cudaStream_t st = ctx->lane.stream;
+  const void* key = reinterpret_cast<const void*>(fold_kernel);
+  if (!ctx->configured.count(key)) {
+    CK(cudaFuncSetAttribute(fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)fold_smem_bytes(FOLD_MAX_BINS)));
+    ctx->configured.insert(key);
+  }
+  CK(cudaMemsetAsync(d_hits, 0, nbin * sizeof(uint64_t), st));
+  fold_plan_kernel<<<(unsigned)ntiles, FOLD_PLAN_THREADS, 0, st>>>(phi0, a, b, (int)nbin, (long long)fold_count,
+                                                                    d_plan, d_hits);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  fold_kernel<<<dim3((unsigned)ctas, (unsigned)R), FOLD_THREADS, fold_smem_bytes((int)nbin), st>>>(
+      sp, time_count, (int)C, (int)G, (int)nbin, (long long)fold_count, (int)ntiles, d_plan, d_rows, d_krows);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  if (finish) {
+    fold_finish_kernel<<<(unsigned)((outputs + 255) / 256), 256, 0, st>>>(d_rows, d_krows, (int)rows_per_output,
+                                                                          (int)gps, (int)nbin, outputs, d_prof, d_kept);
+    ctx->launches++;
+    CK(cudaGetLastError());
+  }
+  CK(cudaMemcpyAsync(h_profile, d_prof, outputs * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_hits, d_hits, nbin * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_kept, d_kept, S * nsub * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
   return 0;
 }
 

@@ -146,8 +146,13 @@ SYMBOLS = {
                                          C.POINTER(C.c_uint64)]),
     "srtb_b200_incoherent_dm_search": (_I, [_P, _P, _SZ, _SZ, _SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _F, _F, _SZ,
                                             C.POINTER(DetectResult), _P, _P, _P]),
+    "srtb_b200_fold_phase": (_I, [C.c_double, C.c_double, C.c_double, C.c_uint64, C.c_uint64,
+                                  C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "srtb_b200_fold": (_I, [_P, C.POINTER(_P), _I, _SZ, _SZ, _SZ, C.c_double, C.c_double, C.c_double, _SZ, _SZ,
+                            _P, _P, _P]),
 }
 INCOHERENT_MAX_DMS = 4096
+FOLD_MAX_BINS = 4096
 
 _lib = None
 
@@ -365,6 +370,21 @@ class Context:
         self._sum_tickets[ticket] = bool(cfg.signal_detect_sum_streams)
         return ticket
 
+    def fold(self, d_spectra, time_count: int, chan_count: int, fold_count: int, phase, nbin: int, nsub: int = 1):
+        """fold the first fold_count samples of each [chan_count][time_count] complex64 spectrum in d_spectra (1 to 4
+        streams) into nbin phase bins, phase = (phi0, a, b) as fold_phase returns it. Returns numpy arrays (profile
+        float64 [streams][nsub][nbin], hits uint64 [nbin], kept uint32 [streams][nsub])"""
+        import numpy as np
+        streams = len(d_spectra)
+        arr = (C.c_void_p * max(streams, 1))(*[_ptr(d) for d in d_spectra])
+        profile = np.zeros((streams, nsub, nbin), np.float64)
+        hits = np.zeros(nbin, np.uint64)
+        kept = np.zeros((streams, nsub), np.uint32)
+        phi0, a, b = phase
+        self._ck(self.lib.srtb_b200_fold(self.h, arr, streams, time_count, chan_count, fold_count, phi0, a, b, nbin,
+                                         nsub, profile.ctypes.data, hits.ctypes.data, kept.ctypes.data))
+        return profile, hits, kept
+
     def submit_block(self, cfg: BlockConfig, h_baseband, nbytes: int) -> int:
         """pipelined ingest: H2D on the copy stream overlaps the previous block's compute"""
         return self._submitted(cfg, self._ck(self.lib.srtb_b200_submit_block(self.h, C.byref(cfg), _ptr(h_baseband),
@@ -487,3 +507,16 @@ def incoherent_shifts(chan_count: int, freq_low: float, bandwidth: float, sample
     if rc < 0:
         raise SrtbError(rc, lib.srtb_b200_last_error(None).decode())
     return out, int(sp.value), int(sm.value)
+
+
+def fold_phase(period: float, period_derivative: float, sample_rate: float, samples_per_spectrum_sample: int,
+               first_sample: int):
+    """(phi0, a, b) of the fold's phase model for a block starting at baseband sample first_sample, exactly as
+    srtb_b200_fold_phase computes them: phi_j = phi0 + a j + b j^2 at spectrum sample j"""
+    lib = load_library()
+    phi0, a, b = C.c_double(), C.c_double(), C.c_double()
+    rc = lib.srtb_b200_fold_phase(period, period_derivative, sample_rate, samples_per_spectrum_sample, first_sample,
+                                  C.byref(phi0), C.byref(a), C.byref(b))
+    if rc < 0:
+        raise SrtbError(rc, lib.srtb_b200_last_error(None).decode())
+    return phi0.value, a.value, b.value

@@ -24,6 +24,8 @@
 // With incoherent_dm_list set instead (--incoherent_dm_list, same syntax), baseband_chain_pipe dedisperses coherently at
 // `dm` and then searches those trial DMs incoherently on each stream's dynamic spectrum; the ring is kept and the sink
 // writes the same files for the best incoherent trial.
+// With fold_period set (a recording only), every block is also folded at that period on the device after its
+// detector, and the sink adds the folds into subintegrations: <prefix>fold.npy, fold.weights.npy and fold.json.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -41,6 +43,7 @@
 #include "srtb/memory.hpp"
 #include "srtb/pipeline/baseband_chain_pipe.hpp"
 #include "srtb/pipeline/dm_sweep_chain_pipe.hpp"
+#include "srtb/pipeline/fold_pipe.hpp"
 #include "srtb/pipeline/framework/pipe.hpp"
 #include "srtb/pipeline/framework/pipe_io.hpp"
 #include "srtb/pipeline/read_file_pipe.hpp"
@@ -98,12 +101,19 @@ void log_sum(const srtb::work::write_signal_work& w) {
             << ", masked channels " << w.sum_zero_count << ", signal counts per boxcar [" << counts << "]";
 }
 
+// fold_period: the block's fold goes to the accumulator (null when folding is off)
+void add_fold(const std::shared_ptr<srtb::pipeline::fold_accumulator>& folds, const srtb::work::write_signal_work& w) {
+  if (folds && w.fold) folds->add(w.fold);
+}
+
 template <typename Sink>
 struct counting_sink {
   std::shared_ptr<Sink> sink;
   std::shared_ptr<std::atomic<uint64_t>> done;
+  std::shared_ptr<srtb::pipeline::fold_accumulator> folds;
   std::optional<srtb::work::dummy_work> operator()(std::stop_token st, srtb::work::write_signal_work w) {
     log_sum(w);
+    add_fold(folds, w);
     (*sink)(st, std::move(w));
     (*done)++;
     return srtb::work::dummy_work{};
@@ -129,8 +139,10 @@ std::string take_option(std::vector<std::string>& args, const std::string& name,
 /** results counted, nothing written (throughput runs) */
 struct discard_sink {
   std::shared_ptr<std::atomic<uint64_t>> done, positives;
+  std::shared_ptr<srtb::pipeline::fold_accumulator> folds;
   std::optional<srtb::work::dummy_work> operator()(std::stop_token, srtb::work::write_signal_work w) {
     log_sum(w);
+    add_fold(folds, w);
     if (!w.time_series.empty()) (*positives)++;
     (*done)++;
     return srtb::work::dummy_work{};
@@ -217,6 +229,7 @@ int main(int argc, char** argv) {
   try {
     srtb::program_options::check_sum_polarizations(
         cfg, srtb::io::backend_registry::get_data_stream_count(cfg.baseband_format_type));
+    srtb::program_options::check_fold(cfg);
   } catch (const std::exception& e) {
     std::fprintf(stderr, "srtb_b200: %s\n", e.what());
     return 2;
@@ -267,6 +280,18 @@ int main(int argc, char** argv) {
               << *std::max_element(inc_trials.begin(), inc_trials.end()) << ", S+ = " << s_plus << ", S- = " << s_minus
               << " spectrum samples, block overlap " << overlap << " samples";
   }
+  std::shared_ptr<fold_accumulator> folds;
+  if (cfg.fold_period != 0) {
+    const fold_parameters fp = fold_parameters::from_config(
+        srtb::io::backend_registry::get_data_stream_count(cfg.baseband_format_type), fold_block_step());
+    folds = std::make_shared<fold_accumulator>(fp);
+    SRTB_LOGI << " [main] " << "folding at P = " << fp.period << " s, Pdot = " << fp.period_derivative << ": "
+              << fp.bins << " bin(s), " << fp.subbands << " subband(s) of " << fp.channels / fp.subbands
+              << " channel(s), dt = " << fp.dt() << " s, " << fp.block_step / (2 * fp.channels)
+              << " spectrum samples per block, " << (fp.subintegration_blocks ? std::to_string(fp.subintegration_blocks)
+                                                                              : std::string{"all"})
+              << " block(s) per subintegration";
+  }
   // the device chain between source and sink: one DM, or the trial DMs of dm_list
   auto start_chain = [&](auto in, auto out, int dev) {
     if (dm_sweep) return start_pipe<dm_sweep_chain_pipe>(in, out, srtb::cuda_queue{dev});
@@ -315,14 +340,14 @@ int main(int argc, char** argv) {
   srtb::cuda_queue q0{devices.front()};
   auto positives = std::make_shared<std::atomic<uint64_t>>(0);
   if (discard) {
-    threads.push_back(start_pipe<discard_sink>(queue_in_functor{out_q}, dummy_out_functor<>{}, done, positives));
+    threads.push_back(start_pipe<discard_sink>(queue_in_functor{out_q}, dummy_out_functor<>{}, done, positives, folds));
   } else if (cfg.baseband_write_all) {
     SRTB_LOGW << " [main] " << "Writing all baseband data, take care of disk space!";
     threads.push_back(start_pipe<counting_sink<write_file_pipe>>(
-        queue_in_functor{out_q}, dummy_out_functor<>{}, std::make_shared<write_file_pipe>(q0), done));
+        queue_in_functor{out_q}, dummy_out_functor<>{}, std::make_shared<write_file_pipe>(q0), done, folds));
   } else {
     threads.push_back(start_pipe<counting_sink<write_signal_pipe>>(
-        queue_in_functor{out_q}, dummy_out_functor<>{}, std::make_shared<write_signal_pipe>(q0), done));
+        queue_in_functor{out_q}, dummy_out_functor<>{}, std::make_shared<write_signal_pipe>(q0), done, folds));
   }
   // source (main.cpp:125-168)
   std::signal(SIGINT, on_signal);
@@ -414,6 +439,11 @@ int main(int argc, char** argv) {
                  (unsigned long long)thumbnails_dropped->load());
   for (auto& t : threads) t.request_stop();
   threads.clear();
+  if (folds) {
+    folds->finish();
+    SRTB_LOGI << " [main] " << "folded " << folds->blocks() << " block(s) into " << folds->subintegrations()
+              << " subintegration(s): " << cfg.baseband_output_file_prefix << "fold.npy";
+  }
   srtb::device_allocator.deallocate_all_free_ptrs();
   srtb::host_allocator.deallocate_all_free_ptrs();
   return 0;
