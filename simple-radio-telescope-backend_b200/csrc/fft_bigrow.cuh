@@ -163,7 +163,8 @@ __device__ __forceinline__ void bigrow_stage_table(float2* __restrict__ p, const
 
 // CHIRP: 0 = plain transform; otherwise s1 + chirp on load, 1/f of successive bins by Newton steps from the neighbour:
 //   1 = one step along a butterfly's inputs (B1 bins apart) and one to the adjacent bin, 3 = two and one,
-//   4 = two and two, 2 = a correctly rounded reciprocal for every bin (widely spaced bins of short test blocks)
+//   4 = two and two, 2 = a correctly rounded reciprocal for every bin (widely spaced bins of short test blocks, and the
+//   sweep-order load, SRC = 1), 5 = the phase table's angles (natural-order rows only)
 // SRC: where the rows come from and what is stored.
 //   0 = rows of `in` (natural order), natural-order rows to `out`;
 //   1 = channel `row` of a spectrum left channel-blocked by SRC = 2 (bin k = k1 + P k2 at (k2 >> 3) L + 8 k1 + (k2 & 7),
@@ -183,7 +184,7 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
                                             const float2* __restrict__ tabs, const row_sk_params& skp,
                                             const row_chirp_params& cp, const tensor_map_blob* tmap,
                                             const r2c_rows_params& rr) {
-  static_assert(SRC == 0 || (LOGL == 14 && ((SRC == 1 && !FWD && SK && CHIRP == 5) || (SRC == 2 && FWD && !SK && CHIRP == 0))),
+  static_assert(SRC == 0 || (LOGL == 14 && ((SRC == 1 && !FWD && SK && CHIRP == 2) || (SRC == 2 && FWD && !SK && CHIRP == 0))),
                 "sweep-order routes: rows of 2^14");
   using C = bigrow<LOGL>;
   constexpr int L = C::L, R3 = C::R3, B1 = C::B1, B2 = C::B2, S1 = C::S1, S2 = C::S2, NT = C::NT, NW = C::NW;
@@ -200,11 +201,11 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
   uint64_t* const mbar = reinterpret_cast<uint64_t*>(sm + off_mbar);  // [3 buffers][8 chunks]
   float* const red = reinterpret_cast<float*>(sm + off_red);  // [2 slots][s2 | s4][32]
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
-  // SRC = 2: the per-row addresses of stage 2, of the last stage and of the split come from a thread index read afresh
-  // (volatile), so they cost a few integer operations per row instead of registers kept live through the butterflies
-  // (a spill)
+  // SRC = 1, 2: the per-row addresses of stages 1 and 2, of the last stage and of the split come from a thread index
+  // read afresh (volatile), so they cost a few integer operations per row instead of registers kept live through the
+  // butterflies and, in SRC = 1, the chirp angles (a spill)
   auto tid_row = [&]() -> int {
-    if constexpr (SRC == 2) {
+    if constexpr (SRC != 0) {
       unsigned t;
       asm volatile("mov.u32 %0, %%tid.x;" : "=r"(t));
       return (int)t;
@@ -331,21 +332,33 @@ __device__ __forceinline__ void bigrow_body(const float2* __restrict__ in, float
       if constexpr (SRC == 1) {
         // rows j, j + 1 of each half are line tid, 128 contiguous bytes: eight 16-byte pieces (columns 2 (p & 3),
         // 2 (p & 3) + 1 of row j + (p >> 2)). The swizzled load left piece p at p ^ (tid & 7), so a quarter warp reading
-        // piece p touches eight distinct bank groups; the phases of piece p are the p-th pair of the row pair's 16
-        // table entries
+        // piece p touches eight distinct bank groups. Piece p of half h holds k1 = (P / 2) h + j + (p >> 2) at columns
+        // k2' = 2 (p & 3) + e, e = 0, 1: bin k1 + P (8 row + k2') = row L + k1 + P k2'. Its phase is evaluated exactly
+        // (chirp_angle, the phase table's expression) rather than read from a table (2 bytes per sample). The angles
+        // do not depend on the data, so each half's sixteen are formed before its wait: half B of this row was issued
+        // only at the end of the previous row, and its wait is where the fp64 work can hide.
         const int rot = tid & 7, box = tid >> 7;
-        const float2* const ph = reinterpret_cast<const float2*>(cp.phase + (size_t)row * L + 8 * j);
+        const double bin0 = (double)((size_t)row * L + j);  // below 2^25: every bin below is an exact double
 #pragma unroll
         for (int h = 0; h < 2; h++) {
+          float ang[16];
+#pragma unroll
+          for (int p = 0; p < 8; p++)
+#pragma unroll
+            for (int e = 0; e < 2; e++)
+              ang[2 * p + e] = chirp_angle(bin0 + (double)((L / 16) * h + (p >> 2) + (L / 8) * (2 * (p & 3) + e)),
+                                           cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm);
+          // the angles are formed before the wait, not sunk past it by the compiler
+#pragma unroll
+          for (int i = 0; i < 16; i++) asm volatile("" : "+f"(ang[i]));
           mbar_wait(&mbar[(h ? hB : hA) * 8 + box], h ? parB : parA);
           const float4* const src = reinterpret_cast<const float4*>((h ? bufB : bufA) + 8 * j);
 #pragma unroll
           for (int p = 0; p < 8; p++) {
-            const float2 g = __ldg(ph + (size_t)h * (L / 16) * 4 + p);
             const float4 x = src[p ^ rot];
             const int c = 2 * (p & 3);  // columns c, c + 1 -> d0 = 2 c + h, 2 c + 2 + h
-            const float2 y0 = chirp_point_tab(make_float2(x.x, x.y), g.x, limit, cp.coef);
-            const float2 y1 = chirp_point_tab(make_float2(x.z, x.w), g.y, limit, cp.coef);
+            const float2 y0 = chirp_point_tab(make_float2(x.x, x.y), ang[2 * p], limit, cp.coef);
+            const float2 y1 = chirp_point_tab(make_float2(x.z, x.w), ang[2 * p + 1], limit, cp.coef);
             if (p < 4) {
               a[2 * c + h] = y0;
               a[2 * c + 2 + h] = y1;
@@ -717,7 +730,7 @@ __global__ void __launch_bounds__(bigrow<14>::NT, 1)
     waterfall_sweep_order_kernel(const float2* __restrict__ in, float2* __restrict__ out, unsigned nrows,
                                  const float2* __restrict__ tabs, row_sk_params skp, row_chirp_params cp,
                                  const __grid_constant__ tensor_map_blob tmap) {
-  bigrow_body<14, false, true, 5, 1>(in, out, nrows, tabs, skp, cp, &tmap, r2c_rows_params{});
+  bigrow_body<14, false, true, 2, 1>(in, out, nrows, tabs, skp, cp, &tmap, r2c_rows_params{});
 }
 
 }  // namespace srtb_b200

@@ -746,25 +746,23 @@ __device__ __forceinline__ float2 chirp_point_tab(float2 v, float ang, float lim
   return make_float2(v.x * wr - v.y * wi, v.x * wi + v.y * wr);
 }
 
-// K12 phase of every bin of a block, once per (block geometry, DM): k exactly as chirp_factor evaluates it (fp64,
-// correctly rounded reciprocal), reduced to [-1/2, 1/2] cycles and stored as the fp32 angle -2 pi frac(k) — the very
-// value chirp_point hands to the SFU, so both routes agree to the last bit of the argument. DM and band are constants
-// of a run, so the table is part of the plan like the twiddles.
-// logp != 0: the order in which the whole-row kernel reads a sweep-order spectrum (fft_bigrow_kernel, SRC = 1), channel
-// by channel: entry ch L + 8 k1 + c (L = 2^(logp + 3)) holds bin k1 + 2^logp (8 ch + c), so one channel's phases stay
-// one contiguous range
+// K12 phase of bin `bin` (an integer, exact in fp64): k exactly as chirp_factor evaluates it (fp64, correctly rounded
+// reciprocal), reduced to [-1/2, 1/2] cycles, as the fp32 angle -2 pi frac(k) — the very value chirp_point hands to
+// the SFU, so every route that takes its angle from here agrees with it to the last bit of the argument
+__device__ __forceinline__ float chirp_angle(double bin, double f_min, double df, double inv_fc, double f_c, double ddm) {
+  const double f = fma(df, bin, f_min);
+  const double q = (f - f_c) * inv_fc;
+  const double k = (ddm * __drcp_rn(f)) * (q * q);
+  const float fr = (float)(k - rint(k));  // the difference is exact, in [-1/2, 1/2]
+  return -6.283185307179586f * fr;
+}
+
+// chirp_angle of every bin of a block, once per (block geometry, DM). DM and band are constants of a run, so the table
+// is part of the plan like the twiddles.
 __global__ void __launch_bounds__(256) chirp_phase_table_kernel(float* __restrict__ out, size_t n, double f_min,
-                                                                double df, double inv_fc, double f_c, double ddm,
-                                                                unsigned logp) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-    const size_t ch = i >> (logp + 3), r = i & ((((size_t)8) << logp) - 1);
-    const size_t bin = logp ? (r >> 3) + ((8 * ch + (r & 7)) << logp) : i;
-    const double f = fma(df, (double)bin, f_min);
-    const double q = (f - f_c) * inv_fc;
-    const double k = (ddm * __drcp_rn(f)) * (q * q);
-    const float fr = (float)(k - rint(k));  // the difference is exact, in [-1/2, 1/2]
-    out[i] = -6.283185307179586f * fr;
-  }
+                                                                double df, double inv_fc, double f_c, double ddm) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    out[i] = chirp_angle((double)i, f_min, df, inv_fc, f_c, ddm);
 }
 
 // ---------------------------------------------------------------------------------

@@ -139,7 +139,7 @@ struct srtb_b200_ctx {
   buffer<float> stream_buf[4];
   // K12 phase table of the current (block geometry, DM): see chirp_phase_table_kernel
   buffer<float> chirp_tab;
-  double chirp_tab_key[7] = {0, 0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm, layout (logp)
+  double chirp_tab_key[6] = {0, 0, 0, 0, 0, 0};  // n, f_min, df, inv_fc, f_c, ddm
   // simplify_spectrum: row-resampled intensities R[C][W] and the column stage's per-CTA partial sums
   buffer<float> thumb_rows, thumb_partial;
   // correlate: the two inputs' in-place R2C buffers of real_count + 2 floats
@@ -1017,8 +1017,8 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
   };
   if constexpr (!FWD && LOGL == 14) {
     if (sweep_order) {
-      if (!(sk && chirp && chirp->newton == 5) || nrows * 8 != (size_t)C::L)
-        return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: the sweep-order load needs the phase table and P = L / 8");
+      if (!(sk && chirp && chirp->newton == 2) || nrows * 8 != (size_t)C::L)
+        return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: the sweep-order load needs the exact chirp and P = L / 8");
       // the spectrum as lines of 16 elements (128 bytes); a box is a quarter of a half channel, 128 lines, swizzled so
       // that stage 0's gather is conflict free without moving registers around
       const cuuint64_t dims[2] = {16u, (cuuint64_t)nrows * C::L / 16};
@@ -1695,6 +1695,7 @@ static int watfft_sk_detect_fused(srtb_b200_ctx* ctx, const detect_out& out, flo
       cpv.newton = (far_steps == 0 || near_steps == 0) ? 2
                    : (far_steps == 1 ? 1 : (near_steps == 1 ? 3 : 4));
       if (cpv.phase) cpv.newton = 5;  // tabulated phases (block path): no reciprocal at all
+      if (sweep_order) cpv.newton = 2;  // every bin's phase evaluated exactly as the table would hold it
     }
     const float2* s_ = src ? src : x;
     rc = (time_count == 8192) ? launch_bigrow<13, false>(ctx, s_, x, chan_count, &p, chirp ? &cpv : nullptr, &chunks)
@@ -1940,15 +1941,13 @@ static bool raw_sources_for(const srtb_b200_block_config* cfg, const void* d_bas
   return true;
 }
 
-// K12 phase table for the whole-row waterfall kernel (block path; the DM sweep, and tables above 4 GiB, evaluate every
-// phase on the fly). Rebuilt when the geometry or the DM changes; built synchronously, so both lanes and any later
-// launch may read it.
-// logp != 0: the sweep-order layout of r2c_sweep_order, channel by channel (chirp_phase_table_kernel)
-static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params& cp, const float** out,
-                           unsigned logp = 0) {
+// K12 phase table for the whole-row waterfall kernel (natural-order block path; the sweep-order route, the DM sweep,
+// and tables above 4 GiB, evaluate every phase on the fly). Rebuilt when the geometry or the DM changes; built
+// synchronously, so both lanes and any later launch may read it.
+static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params& cp, const float** out) {
   *out = nullptr;
   if (n * sizeof(float) > ((size_t)4 << 30)) return 0;
-  const double key[7] = {(double)n, cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm, (double)logp};
+  const double key[6] = {(double)n, cp.f_min, cp.df, cp.inv_fc, cp.f_c, cp.ddm};
   if (ctx->chirp_tab.p && std::memcmp(key, ctx->chirp_tab_key, sizeof(key)) == 0) {
     *out = ctx->chirp_tab.p;
     return 0;
@@ -1956,7 +1955,7 @@ static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params&
   if (int rc = grow(ctx, ctx->chirp_tab, n * sizeof(float))) return rc;
   if (int rc = sync_lanes(ctx)) return rc;  // a block still in flight may be reading the previous table
   chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(ctx->chirp_tab.p, n, cp.f_min, cp.df, cp.inv_fc,
-                                                                           cp.f_c, cp.ddm, logp);
+                                                                           cp.f_c, cp.ddm);
   CK(cudaGetLastError());
   CK(cudaStreamSynchronize(ctx->lane.stream));
   std::memcpy(ctx->chirp_tab_key, key, sizeof(key));
@@ -2111,20 +2110,21 @@ static bool chirp_on_load(size_t L) { return chirp_fusable(L) || long_fusable(L)
 
 // one stream's chain after its R2C, at one DM: s1 + chirp, waterfall FFT, SK and detector writing to `out`. src holds the spectrum, dst receives the dynamic spectrum: the same buffer on the block path, while the
 // DM sweep keeps src for the next trial. phase_table: the whole-row kernel may read a tabulated chirp (built for the
-// block's DM; the DM sweep changes DM every trial). Both buffers are 16-byte aligned: the ctx allocates them, or
+// block's DM; the DM sweep changes DM every trial). sweep_order: src is the channel-blocked spectrum of r2c_sweep_order,
+// whose waterfall kernel evaluates every phase itself. Both buffers are 16-byte aligned: the ctx allocates them, or
 // submit_block_ex checked the caller's.
 static int stream_tail(srtb_b200_ctx* ctx, const block_params& p, const detect_out& out, float2* dst, const float2* src, float dm,
-                       bool phase_table, unsigned sweep_logp = 0) {
+                       bool phase_table, bool sweep_order = false) {
   const srtb_b200_block_config* cfg = p.cfg;
   const size_t reserved = p.reserved(dm);
   if (chirp_fusable(p.L)) {
-    // ONE kernel: s1 + chirp on load, waterfall FFT, SK, partial column sums. sweep_logp: src is in sweep order
+    // ONE kernel: s1 + chirp on load, waterfall FFT, SK, partial column sums
     row_chirp_params cp = p.chirp(dm, ctx->lane.mean);
     if (phase_table)
-      if (int rc = get_chirp_table(ctx, p.Nc, cp, &cp.phase, sweep_logp)) return rc;
+      if (int rc = get_chirp_table(ctx, p.Nc, cp, &cp.phase)) return rc;
     return watfft_sk_detect_fused(ctx, out, dst, p.L, p.batch, reserved, cfg->mitigate_rfi_spectral_kurtosis_threshold,
                                   cfg->signal_detect_signal_noise_threshold, cfg->signal_detect_channel_threshold,
-                                  cfg->signal_detect_max_boxcar_length, &cp, src, sweep_logp != 0);
+                                  cfg->signal_detect_max_boxcar_length, &cp, src, sweep_order);
   }
   if (long_fusable(p.L)) {
     // long rows: chirp-on-load column sweep, last sweep with SK statistics, decision, column sums (20 bytes per
@@ -2238,7 +2238,7 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
         if (int rc = r2c_sweep_order_stream(ctx, p, in, s, buf)) return rc;
       }
       if (int rc = zero_bin_ranges(ctx, buf, p.bins, SWEEP_LOGP, SWEEP_LOGQ)) return rc;
-      return stream_tail(ctx, p, out, buf, buf, p.cfg->dm, /*phase_table=*/true, SWEEP_LOGP);
+      return stream_tail(ctx, p, out, buf, buf, p.cfg->dm, /*phase_table=*/false, /*sweep_order=*/true);
     }
     {
       stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,

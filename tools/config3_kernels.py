@@ -47,7 +47,7 @@ def bytes_per_launch(name, n):
     if name.startswith("r2c_rows_split_kernel"):
         return 4 * n + 4 * n          # scratch in, spectrum out
     if name.startswith("waterfall_sweep_order_kernel"):
-        return 4 * n + 4 * n + 2 * n  # spectrum in, dynamic spectrum out, fp32 phase table in
+        return 4 * n + 4 * n          # spectrum in, dynamic spectrum out (the chirp phase is computed, not read)
     return None                       # zap ranges and the detector tail: no streaming traffic of their own
 
 
