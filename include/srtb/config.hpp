@@ -58,6 +58,9 @@ struct configs {
   size_t fold_bin_count = 256;
   size_t fold_subband_count = 1;
   size_t fold_subintegration_blocks = 0;
+  // with fold_period: also fold the coherence products AA, BB, CR, CI of streams 0 and 1 (the two feeds of a
+  // dual-polarisation format) over the channels kept in both; needs a two-stream format (not gznupsr_a1_4)
+  bool fold_coherence = false;
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

@@ -220,6 +220,10 @@ class baseband_chain_pipe {
     f->hits.assign(f->bins, 0);
     f->kept.assign(f->streams * f->subbands, 0);
     const size_t fold_count = (size_t)std::min<uint64_t>(std::min(step, p.work.valid_samples) / two_c, p.L);
+    if (c.fold_coherence) {
+      f->coherence.assign(4 * f->subbands * f->bins, 0.0);
+      f->coherence_kept.assign(f->subbands, 0);
+    }
     if (fold_count == 0) return f;  // nothing read past the previous block's share: an empty fold keeps the order
     double phi0 = 0, a = 0, b = 0;
     q.check(srtb_b200_fold_phase(c.fold_period, c.fold_period_derivative, c.baseband_sample_rate, two_c,
@@ -228,6 +232,9 @@ class baseband_chain_pipe {
     for (int s = 0; s < p.streams; s++) spectra[s] = p.d_spectrum[s].get();
     q.check(srtb_b200_fold(q.ctx(), spectra, p.streams, p.L, p.C, fold_count, phi0, a, b, f->bins, f->subbands,
                            f->profile.data(), f->hits.data(), f->kept.data()));
+    if (c.fold_coherence)  // streams 0 and 1 are the two feeds (check_fold); the same samples, bins and hits
+      q.check(srtb_b200_fold_coherence(q.ctx(), spectra[0], spectra[1], p.L, p.C, fold_count, phi0, a, b, f->bins,
+                                       f->subbands, f->coherence.data(), f->hits.data(), f->coherence_kept.data()));
     return f;
   }
 

@@ -9,6 +9,11 @@
 //                                                  fold / weights is the mean power per channel-sample
 //   <baseband_output_file_prefix>fold.json         the parameters, each subintegration's start time and the reference;
 //                                                  no wall-clock time, so two runs over one recording write the same bytes
+// and with fold_coherence also
+//   <baseband_output_file_prefix>fold.coherence.npy          float64 [subint][4][subband][bin]: AA, BB, CR, CI of
+//                                                            X = stream 0 and Y = stream 1 (srtb_b200_fold_coherence)
+//   <baseband_output_file_prefix>fold.coherence.weights.npy  float64 [subint][subband][bin]: sum over blocks of
+//                                                            kept[k] hits[bin], kept counting the channels kept in both
 #pragma once
 #include <cmath>
 #include <cstdint>
@@ -43,6 +48,7 @@ struct fold_parameters {
   size_t streams = 1, channels = 0, subbands = 1, bins = 1;
   uint64_t block_step = 0;           // N - R: baseband samples per stream between consecutive blocks
   size_t subintegration_blocks = 0;  // 0 = one subintegration for the whole run
+  bool coherence = false;            // fold_coherence: also the coherence products of streams 0 and 1
   std::string prefix;
 
   static fold_parameters from_config(size_t streams, uint64_t block_step) {
@@ -60,6 +66,7 @@ struct fold_parameters {
     p.bins = c.fold_bin_count;
     p.block_step = block_step;
     p.subintegration_blocks = c.fold_subintegration_blocks;
+    p.coherence = c.fold_coherence;
     p.prefix = c.baseband_output_file_prefix;
     return p;
   }
@@ -75,6 +82,9 @@ class fold_accumulator {
     std::lock_guard<std::mutex> g{m};
     if (b->streams != par.streams || b->subbands != par.subbands || b->bins != par.bins)
       throw std::runtime_error("[fold] a block's fold shape does not match the run's");
+    if (par.coherence && (b->coherence.size() != 4 * par.subbands * par.bins ||
+                          b->coherence_kept.size() != par.subbands))
+      throw std::runtime_error("[fold] a block carries no coherence products of the run's shape");
     waiting[b->block_index] = std::move(b);
     bool completed = false;
     while (!waiting.empty() && waiting.begin()->first == next_block) {
@@ -109,6 +119,8 @@ class fold_accumulator {
   uint64_t next_block = 0;
   uint64_t blocks_folded = 0;
   std::vector<double> profile, weights;  // [subint][stream][subband][bin]
+  std::vector<double> coherence;         // [subint][4][subband][bin] (fold_coherence)
+  std::vector<double> coherence_weights;  // [subint][subband][bin] (fold_coherence)
   std::vector<uint64_t> subint_first;    // first_sample of each subintegration's first block
   std::vector<uint64_t> subint_blocks;   // blocks added to each subintegration
 
@@ -122,6 +134,10 @@ class fold_accumulator {
       subint_blocks.resize(si + 1, 0);
       profile.resize((si + 1) * row(), 0.0);
       weights.resize((si + 1) * row(), 0.0);
+      if (par.coherence) {
+        coherence.resize((si + 1) * 4 * par.subbands * par.bins, 0.0);
+        coherence_weights.resize((si + 1) * par.subbands * par.bins, 0.0);
+      }
     }
     if (subint_blocks[si] == 0) subint_first[si] = b.first_sample;  // blocks come in index order
     subint_blocks[si]++;
@@ -132,6 +148,15 @@ class fold_accumulator {
         p[sk * par.bins + bin] += b.profile[sk * par.bins + bin];
         w[sk * par.bins + bin] += (double)b.kept[sk] * (double)b.hits[bin];
       }
+    if (par.coherence) {
+      const size_t kb = par.subbands * par.bins;
+      double* cp = coherence.data() + si * 4 * kb;
+      double* cw = coherence_weights.data() + si * kb;
+      for (size_t i = 0; i < 4 * kb; i++) cp[i] += b.coherence[i];
+      for (size_t k = 0; k < par.subbands; k++)
+        for (size_t bin = 0; bin < par.bins; bin++)
+          cw[k * par.bins + bin] += (double)b.coherence_kept[k] * (double)b.hits[bin];
+    }
     blocks_folded++;
     return par.subintegration_blocks && (b.block_index + 1) % par.subintegration_blocks == 0;
   }
@@ -152,6 +177,14 @@ class fold_accumulator {
     };
     replace(base + ".npy", [&](const std::string& f) { srtb::io::npy_save(f, profile.data(), shape); });
     replace(base + ".weights.npy", [&](const std::string& f) { srtb::io::npy_save(f, weights.data(), shape); });
+    if (par.coherence) {
+      const size_t n = subint_first.size();
+      const std::vector<size_t> cshape = {n, 4, par.subbands, par.bins}, wshape = {n, par.subbands, par.bins};
+      replace(base + ".coherence.npy",
+              [&](const std::string& f) { srtb::io::npy_save(f, coherence.data(), cshape); });
+      replace(base + ".coherence.weights.npy",
+              [&](const std::string& f) { srtb::io::npy_save(f, coherence_weights.data(), wshape); });
+    }
     std::string starts, counts;
     for (size_t i = 0; i < subint_first.size(); i++) {
       starts += (i ? ", " : "") + num((double)subint_first[i] / par.sample_rate);
@@ -174,7 +207,12 @@ class fold_accumulator {
         "  \"blocks_per_subintegration\": " + std::to_string(par.subintegration_blocks) + ",\n"
         "  \"blocks_folded\": " + std::to_string(blocks_folded) + ",\n"
         "  \"subintegration_blocks_folded\": [" + counts + "],\n"
-        "  \"subintegration_start_s\": [" + starts + "],\n"
+        "  \"subintegration_start_s\": [" + starts + "],\n" +
+        (par.coherence ? "  \"coherence\": [\"AA\", \"BB\", \"CR\", \"CI\"],\n"
+                         "  \"coherence_definition\": \"X = stream 0, Y = stream 1; AA = |X|^2, BB = |Y|^2, "
+                         "CR = Re(X conj Y), CI = Im(X conj Y), summed over the channels kept in both streams; "
+                         "no calibration is applied\",\n"
+                       : "") +
         "  \"reference\": \"t = 0 at the first sample after input_file_offset_bytes; topocentric, not barycentred; "
         "arrival times referred to freq_low + bandwidth, the frequency coherent dedispersion aligns the channels to; "
         "phase = t/P - (Pdot/P^2) t^2 / 2 with no timing-model predictor; bin 0 starts at phase 0\"\n"

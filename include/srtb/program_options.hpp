@@ -239,7 +239,7 @@ inline const std::vector<std::string>& known_options() {
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length",
       "signal_detect_sum_polarizations", "fold_period", "fold_period_derivative", "fold_bin_count",
-      "fold_subband_count", "fold_subintegration_blocks"};
+      "fold_subband_count", "fold_subintegration_blocks", "fold_coherence"};
   return names;
 }
 
@@ -378,6 +378,7 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(fold_bin_count)
   SRTB_PARSE(fold_subband_count)
   SRTB_PARSE(fold_subintegration_blocks)
+  SRTB_PARSE(fold_coherence)
   SRTB_PARSE(thread_query_work_wait_time)
   SRTB_PARSE(gui_enable)
   SRTB_PARSE(gui_pixmap_width)
@@ -420,8 +421,20 @@ inline void check_sum_polarizations(const srtb::configs& config, size_t streams)
 
 /** folding (fold_period != 0) at start-up: a finite, positive period of at least two spectrum samples (2 dt, dt =
  *  2C / baseband_sample_rate with C = min(spectrum_channel_count, baseband_input_count / 2)), 1 to 4096 bins, a subband
- *  count that divides C, no dm_list (the sweep gives each stream another DM) and a recording to fold (input_file_path) */
+ *  count that divides C, no dm_list (the sweep gives each stream another DM) and a recording to fold (input_file_path);
+ *  fold_coherence needs fold_period and a two-stream format: naocpsr_snap1, interleaved_samples_2 or gznupsr_a1 */
 inline void check_fold(const srtb::configs& config) {
+  if (config.fold_coherence) {  // the coherence products pair the two feeds of a dual-polarisation format
+    if (config.fold_period == 0)
+      throw std::invalid_argument("[program_options] fold_coherence needs fold_period: it folds at the fold's period");
+    const std::string& f = config.baseband_format_type;
+    if (f == "gznupsr_a1_4")
+      throw std::invalid_argument("[program_options] fold_coherence with baseband_format_type = gznupsr_a1_4: its four "
+                                  "streams are not documented as two feed pairs");
+    if (f != "naocpsr_snap1" && f != "interleaved_samples_2" && f != "gznupsr_a1")
+      throw std::invalid_argument("[program_options] fold_coherence with baseband_format_type = " + f +
+                                  ": a single-stream format has no second polarisation to pair");
+  }
   if (config.fold_period == 0) return;
   const double P = config.fold_period;
   if (!std::isfinite(P) || P < 0 || !std::isfinite(config.fold_period_derivative))

@@ -205,7 +205,8 @@ struct dm_trial_summary {
   std::vector<boxcar> boxcars;
 };
 
-/** one block folded at fold_period: where it lies in the recording and what srtb_b200_fold returned for it */
+/** one block folded at fold_period: where it lies in the recording and what srtb_b200_fold (and, with fold_coherence,
+ *  srtb_b200_fold_coherence) returned for it */
 struct fold_block {
   uint64_t block_index = 0;   // first_sample / (N - R): blocks tile the recording in steps of N - R samples
   uint64_t first_sample = 0;
@@ -213,6 +214,10 @@ struct fold_block {
   std::vector<double> profile;  // [streams][subbands][bins]
   std::vector<uint64_t> hits;   // [bins]
   std::vector<uint32_t> kept;   // [streams][subbands]
+  // fold_coherence only (srtb_b200_fold_coherence of streams 0 and 1; empty otherwise): AA, BB, CR, CI and the
+  // channels kept in both streams
+  std::vector<double> coherence;         // [4][subbands][bins]
+  std::vector<uint32_t> coherence_kept;  // [subbands]
 };
 
 struct write_signal_work : public write_file_work {

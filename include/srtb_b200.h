@@ -396,6 +396,32 @@ int srtb_b200_fold(srtb_b200_ctx* ctx, const void* const* d_spectra /* [streams]
                    size_t chan_count, size_t fold_count, double phi0, double a, double b, size_t nbin, size_t nsub,
                    double* h_profile /* [streams][nsub][nbin] */, uint64_t* h_hits /* [nbin] */,
                    uint32_t* h_kept /* [streams][nsub] */);
+/* The coherence products of a stream pair, folded as srtb_b200_fold folds (the same samples j < fold_count, bins and
+ * hits): with X = d_x and Y = d_y ([chan_count][time_count] complex64 each, the two feeds of one receiver) and K(k) the
+ * channels c of subband k kept in both, |X[c][0]|^2 != 0 and |Y[c][0]|^2 != 0 (formed in fp32, the detector's rule),
+ *   h_coherence[0][k][bin] = AA = sum over c in K(k) and the j in bin of |X[c][j]|^2,
+ *   h_coherence[1][k][bin] = BB = ... |Y[c][j]|^2,
+ *   h_coherence[2][k][bin] = CR = ... Re(X[c][j] conj(Y[c][j])),
+ *   h_coherence[3][k][bin] = CI = ... Im(X[c][j] conj(Y[c][j])),
+ *   h_hits[bin]            = the number of j < fold_count in bin (srtb_b200_fold's hits),
+ *   h_kept[k]              = |K(k)|.
+ * A channel masked in either stream adds nothing to any of the four (PSRCHIVE's Coherence state: AA, BB, CR, CI; no
+ * calibration). Each product of two fp32 components is formed exactly in float64 and the sums run in float64 in a fixed
+ * order: two calls agree bit for bit. Both spectra are read once (2 chan_count fold_count 8 bytes, less the masked
+ * channels), in at most three kernel launches whatever nsub and nbin. Stream-ordered on the ctx's stream; synchronises
+ * it once before it returns.
+ * Before any launch: a null ctx, spectrum or output, a zero time_count or chan_count, a spectrum that is not 8-byte
+ * aligned, d_x == d_y or a non-finite phi0, a or b returns SRTB_B200_E_INVALID; fold_count of 0 or above time_count,
+ * nbin outside 1..SRTB_B200_FOLD_MAX_BINS, nsub not dividing chan_count, chan_count above 2^24 or fold_count above 2^40
+ * returns SRTB_B200_E_SIZE.
+ * Scratch the ctx grows on demand and keeps (shared with srtb_b200_fold), with G = the largest divisor of
+ * chan_count / nsub up to 64, K = chan_count / G CTAs and R = min(ceil(fold_count / 2048), max(1, floor(2 SMs / K)))
+ * tile ranges each: 4 ceil(fold_count / 2048) 2048 + 8 nbin + 32 nsub nbin + 16 nsub bytes, plus 32 K R nbin + 16 K
+ * bytes when (chan_count / nsub / G) R > 1 (each part rounded up to 256 bytes). */
+int srtb_b200_fold_coherence(srtb_b200_ctx* ctx, const void* d_x, const void* d_y, size_t time_count,
+                             size_t chan_count, size_t fold_count, double phi0, double a, double b, size_t nbin,
+                             size_t nsub, double* h_coherence /* [4][nsub][nbin]: AA, BB, CR, CI */,
+                             uint64_t* h_hits /* [nbin] */, uint32_t* h_kept /* [nsub]: kept in both */);
 
 /* simplify_spectrum_pipe_2 (pipeline/spectrum_pipe.hpp:82-143): resample_spectrum_3 with norm(),
  * normalize_with_average_value, generate_pixmap. d_spectrum is [in_height][in_width] complex64

@@ -22,6 +22,9 @@
 //                        stored once: one float64 row of nbin per CTA.
 //   fold_finish_kernel   adds each output's CTA rows (channel groups, then tile ranges, in index order) and the groups'
 //                        kept counts. Not launched when every subband has one CTA: fold_kernel then stores the output.
+//
+// fold_coherence_kernel (srtb_b200_fold_coherence) takes fold_kernel's place for a stream pair: the coherence products
+// AA, BB, CR, CI of X = x_0 and Y = x_1 over the channels kept in both, between the same plan and finish kernels.
 #pragma once
 #include <cuda_runtime.h>
 
@@ -170,6 +173,138 @@ __global__ void __launch_bounds__(FOLD_THREADS, 4) fold_kernel(fold_spectra sp, 
   double* o = out + (size_t)(blockIdx.x * (size_t)R + r) * nbin;
   for (int i = t; i < nbin; i += FOLD_THREADS) o[i] = acc[i];
   if (r == 0 && t == 0) kept_out[blockIdx.x] = kept;
+}
+
+// ---- coherence products of a stream pair (srtb_b200_fold_coherence): X = x_0, Y = x_1 and, for the channels c kept in
+// both (|X[c][0]|^2 != 0 and |Y[c][0]|^2 != 0, in fp32 as fold_kernel's rule), the four sums
+//   AA = |X|^2, BB = |Y|^2, CR = Re(X conj Y), CI = Im(X conj Y)
+// over the channels of subband k and the j in bin. The bin plan is fold_plan_kernel's and the CTA rows are added by
+// fold_finish_kernel, with the four products in the place of the streams. Every product of two fp32 components is exact
+// in float64, so CR and CI, which cancel heavily on unpolarised noise, carry only the float64 rounding of their sums.
+constexpr int FOLD_COH_THREADS = 256;  // fold_coherence_kernel
+constexpr int FOLD_COH_PER_THREAD = FOLD_TILE / FOLD_COH_THREADS;
+
+// dynamic shared memory of fold_coherence_kernel: acc [nbin + 1][4], pw [FOLD_TILE][4], carry [threads][4], has_start
+__host__ __device__ constexpr size_t fold_coherence_smem_bytes(int nbin) {
+  return (size_t)(nbin + 1) * 4 * sizeof(double) + FOLD_TILE * 4 * sizeof(double) +
+         FOLD_COH_THREADS * (4 * sizeof(double) + sizeof(int));
+}
+
+// grid.x = C / G channel groups, grid.y = tile ranges. out row of CTA (product p, group g, range r):
+// ((p * C / G + g) * gridDim.y + r) * nbin; kept_out[p * C / G + g] (the same count for each p, from the CTAs of range
+// 0), so fold_finish_kernel adds rows and counts for 4 "streams". A channel masked in either stream is skipped: its
+// samples are not loaded and it adds nothing to any product
+__global__ void __launch_bounds__(FOLD_COH_THREADS, 2) fold_coherence_kernel(
+    const float2* __restrict__ xs, const float2* __restrict__ ys, size_t L, int C, int G, int nbin, long long F,
+    int ntiles, const uint32_t* __restrict__ plan, double* __restrict__ out, unsigned* __restrict__ kept_out) {
+  extern __shared__ double smem[];
+  double* acc = smem;                                     // [nbin + 1][4]: the last bin takes the padding samples
+  double* pw = acc + (size_t)(nbin + 1) * 4;              // [FOLD_TILE][4]: the summed products by local j
+  double* carry = pw + FOLD_TILE * 4;                     // [threads][4]: a chunk's sums before its first run start
+  int* has_start = reinterpret_cast<int*>(carry + FOLD_COH_THREADS * 4);
+  __shared__ uint32_t keep_bits[FOLD_MAX_GROUP / 32];
+  const int groups = C / G, g = blockIdx.x;
+  const float2* x = xs + (size_t)g * G * L;
+  const float2* y = ys + (size_t)g * G * L;
+  const int t = threadIdx.x;
+  for (int i = t; i < (nbin + 1) * 4; i += FOLD_COH_THREADS) acc[i] = 0.0;
+  if (t < FOLD_MAX_GROUP) {  // the pair's mask of the group's channels, one bit each
+    bool keep = false;
+    if (t < G) {
+      const float2 a = x[(size_t)t * L], b = y[(size_t)t * L];
+      keep = __fadd_rn(__fmul_rn(a.x, a.x), __fmul_rn(a.y, a.y)) != 0.f &&
+             __fadd_rn(__fmul_rn(b.x, b.x), __fmul_rn(b.y, b.y)) != 0.f;
+    }
+    const uint32_t bits = __ballot_sync(0xffffffffu, keep);
+    if ((t & 31) == 0) keep_bits[t >> 5] = bits;
+  }
+  __syncthreads();
+  const int r = blockIdx.y, R = gridDim.y;
+  const int tile_lo = (int)((long long)ntiles * r / R), tile_hi = (int)((long long)ntiles * (r + 1) / R);
+  for (int tile = tile_lo; tile < tile_hi; tile++) {
+    const long long j0 = (long long)tile * FOLD_TILE;
+    double aa[FOLD_COH_PER_THREAD], bb[FOLD_COH_PER_THREAD], cr[FOLD_COH_PER_THREAD], ci[FOLD_COH_PER_THREAD];
+#pragma unroll
+    for (int e = 0; e < FOLD_COH_PER_THREAD; e++) aa[e] = bb[e] = cr[e] = ci[e] = 0.0;
+    for (int c = 0; c < G; c++) {
+      if (!((keep_bits[c >> 5] >> (c & 31)) & 1u)) continue;  // masked in X or Y: in no product
+      const float2* xrow = x + (size_t)c * L;
+      const float2* yrow = y + (size_t)c * L;
+      float2 p[FOLD_COH_PER_THREAD], q[FOLD_COH_PER_THREAD];
+#pragma unroll
+      for (int e = 0; e < FOLD_COH_PER_THREAD; e++) {
+        const long long j = j0 + t + e * FOLD_COH_THREADS;
+        p[e] = j < F ? __ldcs(xrow + j) : make_float2(0.f, 0.f);
+        q[e] = j < F ? __ldcs(yrow + j) : make_float2(0.f, 0.f);
+      }
+#pragma unroll
+      for (int e = 0; e < FOLD_COH_PER_THREAD; e++) {  // each product exact in float64; one rounding per add
+        const double xr = p[e].x, xi = p[e].y, yr = q[e].x, yi = q[e].y;
+        aa[e] = __dadd_rn(aa[e], __dadd_rn(__dmul_rn(xr, xr), __dmul_rn(xi, xi)));
+        bb[e] = __dadd_rn(bb[e], __dadd_rn(__dmul_rn(yr, yr), __dmul_rn(yi, yi)));
+        cr[e] = __dadd_rn(cr[e], __dadd_rn(__dmul_rn(xr, yr), __dmul_rn(xi, yi)));
+        ci[e] = __dadd_rn(ci[e], __dsub_rn(__dmul_rn(xi, yr), __dmul_rn(xr, yi)));
+      }
+    }
+#pragma unroll
+    for (int e = 0; e < FOLD_COH_PER_THREAD; e++) {
+      double2* o = reinterpret_cast<double2*>(pw + (size_t)(t + e * FOLD_COH_THREADS) * 4);
+      o[0] = make_double2(aa[e], bb[e]);
+      o[1] = make_double2(cr[e], ci[e]);
+    }
+    __syncthreads();
+    // this thread's chunk of the sorted order, as in fold_kernel, with four sums per run
+    const uint32_t* pl = plan + (size_t)tile * FOLD_TILE + t * FOLD_COH_PER_THREAD;
+    uint32_t prev_bin = t > 0 ? (pl[-1] >> 16) : 0xffffffffu;
+    bool started = false;
+    double2 c0 = make_double2(0.0, 0.0), c1 = c0;
+    uint32_t cur_bin = 0;
+#pragma unroll
+    for (int e = 0; e < FOLD_COH_PER_THREAD; e++) {
+      const uint32_t k = pl[e], bin = k >> 16;
+      if (bin != prev_bin) {
+        double2* dst = reinterpret_cast<double2*>(started ? acc + (size_t)cur_bin * 4 : carry + t * 4);
+        if (started) {
+          c0 = make_double2(__dadd_rn(dst[0].x, c0.x), __dadd_rn(dst[0].y, c0.y));
+          c1 = make_double2(__dadd_rn(dst[1].x, c1.x), __dadd_rn(dst[1].y, c1.y));
+        }
+        dst[0] = c0;
+        dst[1] = c1;
+        started = true;
+        c0 = c1 = make_double2(0.0, 0.0);
+        cur_bin = bin;
+        prev_bin = bin;
+      }
+      const double2* src = reinterpret_cast<const double2*>(pw + (size_t)(k & 0xffffu) * 4);
+      const double2 s0 = src[0], s1 = src[1];
+      c0 = make_double2(__dadd_rn(c0.x, s0.x), __dadd_rn(c0.y, s0.y));
+      c1 = make_double2(__dadd_rn(c1.x, s1.x), __dadd_rn(c1.y, s1.y));
+    }
+    if (!started) {
+      double2* dst = reinterpret_cast<double2*>(carry + t * 4);
+      dst[0] = c0;
+      dst[1] = c1;
+    }
+    has_start[t] = started ? 1 : 0;
+    __syncthreads();
+    if (started) {  // the last run started here: add the following chunks' carries up to the next run start
+      for (int u = t + 1; u < FOLD_COH_THREADS; u++) {
+        const double2* cu = reinterpret_cast<const double2*>(carry + u * 4);
+        c0 = make_double2(__dadd_rn(c0.x, cu[0].x), __dadd_rn(c0.y, cu[0].y));
+        c1 = make_double2(__dadd_rn(c1.x, cu[1].x), __dadd_rn(c1.y, cu[1].y));
+        if (has_start[u]) break;
+      }
+      double2* dst = reinterpret_cast<double2*>(acc + (size_t)cur_bin * 4);
+      dst[0] = make_double2(__dadd_rn(dst[0].x, c0.x), __dadd_rn(dst[0].y, c0.y));
+      dst[1] = make_double2(__dadd_rn(dst[1].x, c1.x), __dadd_rn(dst[1].y, c1.y));
+    }
+    __syncthreads();
+  }
+  for (int p = 0; p < 4; p++) {
+    double* o = out + ((size_t)(p * groups + g) * R + r) * nbin;
+    for (int i = t; i < nbin; i += FOLD_COH_THREADS) o[i] = acc[(size_t)i * 4 + p];
+  }
+  if (r == 0 && t < 4) kept_out[t * groups + g] = __popc(keep_bits[0]) + __popc(keep_bits[1]);
 }
 
 // one thread per output (s, k, bin): adds the rows of its subband's groups and tile ranges in index order; the bin-0

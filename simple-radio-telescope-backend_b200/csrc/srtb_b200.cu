@@ -2763,6 +2763,86 @@ extern "C" int srtb_b200_fold(srtb_b200_ctx* ctx, const void* const* d_spectra, 
   return 0;
 }
 
+// the coherence products of a stream pair: srtb_b200_fold's plan and finish around fold_coherence_kernel, whose CTA
+// rows stand for four streams (AA, BB, CR, CI)
+extern "C" int srtb_b200_fold_coherence(srtb_b200_ctx* ctx, const void* d_x, const void* d_y, size_t time_count,
+                                        size_t chan_count, size_t fold_count, double phi0, double a, double b,
+                                        size_t nbin, size_t nsub, double* h_coherence, uint64_t* h_hits,
+                                        uint32_t* h_kept) {
+  API_LOCK(ctx);
+  if (!ctx || !d_x || !d_y || !h_coherence || !h_hits || !h_kept || time_count == 0 || chan_count == 0)
+    return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: bad argument");
+  if (!aligned8(d_x) || !aligned8(d_y))
+    return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: a spectrum is not 8-byte aligned");
+  if (d_x == d_y) return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: d_x and d_y are the same spectrum");
+  if (fold_count == 0 || fold_count > time_count)
+    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: fold_count must be 1 to time_count");
+  if (nbin < 1 || nbin > (size_t)FOLD_MAX_BINS)
+    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: nbin must be 1 to 4096");
+  if (nsub == 0 || chan_count % nsub)
+    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: nsub must divide chan_count");
+  if (chan_count > ((size_t)1 << 24) || fold_count > ((size_t)1 << 40))
+    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: chan_count above 2^24 or fold_count above 2^40");
+  if (!std::isfinite(phi0) || !std::isfinite(a) || !std::isfinite(b))
+    return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: a phase coefficient is not finite");
+  CK(cudaSetDevice(ctx->device));
+  const size_t C = chan_count, P = 4, csub = C / nsub;
+  size_t G = std::min<size_t>(csub, FOLD_MAX_GROUP);
+  while (csub % G) G--;  // channels per CTA, as srtb_b200_fold
+  const size_t ntiles = (fold_count + FOLD_TILE - 1) / FOLD_TILE, ctas = C / G;
+  // tile ranges per channel group: up to one wave of two CTAs per SM (the shared memory of nbin <= 1024 allows two)
+  const size_t target = (size_t)ctx->sm_count * 2;
+  const size_t R = std::max<size_t>(1, std::min<size_t>(ntiles, target / ctas));
+  const size_t gps = csub / G, rows_per_output = gps * R, outputs = P * nsub * nbin;
+  // scratch: plan u32 [ntiles][FOLD_TILE], hits u64 [nbin], coherence f64 [4][nsub][nbin], kept u32 [4][nsub] (the
+  // same count four times: fold_finish_kernel's layout); with more than one CTA row per output also rows
+  // f64 [4 ctas R nbin] and kept rows u32 [4 ctas]
+  const auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
+  const size_t hits_o = up(ntiles * FOLD_TILE * sizeof(uint32_t));
+  const size_t prof_o = hits_o + up(nbin * sizeof(uint64_t));
+  const size_t kept_o = prof_o + up(outputs * sizeof(double));
+  const size_t rows_o = kept_o + up(P * nsub * sizeof(uint32_t));
+  const bool finish = rows_per_output > 1;
+  const size_t krow_o = rows_o + (finish ? up(P * ctas * R * nbin * sizeof(double)) : 0);
+  const size_t work_b = krow_o + (finish ? P * ctas * sizeof(uint32_t) : 0);
+  if (int rc = grow(ctx, ctx->fold_work, work_b)) return rc;
+  char* w = ctx->fold_work.p;
+  uint32_t* d_plan = reinterpret_cast<uint32_t*>(w);
+  unsigned long long* d_hits = reinterpret_cast<unsigned long long*>(w + hits_o);
+  double* d_prof = reinterpret_cast<double*>(w + prof_o);
+  unsigned* d_kept = reinterpret_cast<unsigned*>(w + kept_o);
+  double* d_rows = finish ? reinterpret_cast<double*>(w + rows_o) : d_prof;
+  unsigned* d_krows = finish ? reinterpret_cast<unsigned*>(w + krow_o) : d_kept;
+  cudaStream_t st = ctx->lane.stream;
+  const void* key = reinterpret_cast<const void*>(fold_coherence_kernel);
+  if (!ctx->configured.count(key)) {
+    CK(cudaFuncSetAttribute(fold_coherence_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                            (int)fold_coherence_smem_bytes(FOLD_MAX_BINS)));
+    ctx->configured.insert(key);
+  }
+  CK(cudaMemsetAsync(d_hits, 0, nbin * sizeof(uint64_t), st));
+  fold_plan_kernel<<<(unsigned)ntiles, FOLD_PLAN_THREADS, 0, st>>>(phi0, a, b, (int)nbin, (long long)fold_count,
+                                                                    d_plan, d_hits);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  fold_coherence_kernel<<<dim3((unsigned)ctas, (unsigned)R), FOLD_COH_THREADS, fold_coherence_smem_bytes((int)nbin),
+                          st>>>(static_cast<const float2*>(d_x), static_cast<const float2*>(d_y), time_count, (int)C,
+                                (int)G, (int)nbin, (long long)fold_count, (int)ntiles, d_plan, d_rows, d_krows);
+  ctx->launches++;
+  CK(cudaGetLastError());
+  if (finish) {
+    fold_finish_kernel<<<(unsigned)((outputs + 255) / 256), 256, 0, st>>>(d_rows, d_krows, (int)rows_per_output,
+                                                                          (int)gps, (int)nbin, outputs, d_prof, d_kept);
+    ctx->launches++;
+    CK(cudaGetLastError());
+  }
+  CK(cudaMemcpyAsync(h_coherence, d_prof, outputs * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_hits, d_hits, nbin * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_kept, d_kept, nsub * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
 // tickets wrap at a multiple of the slot count, so ticket % SRTB_B200_RING_SLOTS is always the slot that was used
 static inline int ring_ticket(uint64_t submit_count) {
   return (int)(submit_count % ((uint64_t)SRTB_B200_RING_SLOTS << 28));

@@ -150,6 +150,8 @@ SYMBOLS = {
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "srtb_b200_fold": (_I, [_P, C.POINTER(_P), _I, _SZ, _SZ, _SZ, C.c_double, C.c_double, C.c_double, _SZ, _SZ,
                             _P, _P, _P]),
+    "srtb_b200_fold_coherence": (_I, [_P, _P, _P, _SZ, _SZ, _SZ, C.c_double, C.c_double, C.c_double, _SZ, _SZ,
+                                      _P, _P, _P]),
 }
 INCOHERENT_MAX_DMS = 4096
 FOLD_MAX_BINS = 4096
@@ -384,6 +386,21 @@ class Context:
         self._ck(self.lib.srtb_b200_fold(self.h, arr, streams, time_count, chan_count, fold_count, phi0, a, b, nbin,
                                          nsub, profile.ctypes.data, hits.ctypes.data, kept.ctypes.data))
         return profile, hits, kept
+
+    def fold_coherence(self, d_x, d_y, time_count: int, chan_count: int, fold_count: int, phase, nbin: int,
+                       nsub: int = 1):
+        """fold the coherence products of two [chan_count][time_count] complex64 spectra X = d_x, Y = d_y (the two
+        feeds of one receiver) as fold folds them, over the channels kept in both. Returns numpy arrays (coherence
+        float64 [4][nsub][nbin]: AA, BB, CR, CI; hits uint64 [nbin]; kept uint32 [nsub])"""
+        import numpy as np
+        coherence = np.zeros((4, nsub, nbin), np.float64)
+        hits = np.zeros(nbin, np.uint64)
+        kept = np.zeros(nsub, np.uint32)
+        phi0, a, b = phase
+        self._ck(self.lib.srtb_b200_fold_coherence(self.h, _ptr(d_x), _ptr(d_y), time_count, chan_count, fold_count,
+                                                   phi0, a, b, nbin, nsub, coherence.ctypes.data, hits.ctypes.data,
+                                                   kept.ctypes.data))
+        return coherence, hits, kept
 
     def submit_block(self, cfg: BlockConfig, h_baseband, nbytes: int) -> int:
         """pipelined ingest: H2D on the copy stream overlaps the previous block's compute"""

@@ -25,7 +25,8 @@
 // `dm` and then searches those trial DMs incoherently on each stream's dynamic spectrum; the ring is kept and the sink
 // writes the same files for the best incoherent trial.
 // With fold_period set (a recording only), every block is also folded at that period on the device after its
-// detector, and the sink adds the folds into subintegrations: <prefix>fold.npy, fold.weights.npy and fold.json.
+// detector, and the sink adds the folds into subintegrations: <prefix>fold.npy, fold.weights.npy and fold.json. With
+// fold_coherence also the coherence products of streams 0 and 1: fold.coherence.npy and fold.coherence.weights.npy.
 #include <algorithm>
 #include <atomic>
 #include <chrono>
@@ -290,7 +291,7 @@ int main(int argc, char** argv) {
               << " channel(s), dt = " << fp.dt() << " s, " << fp.block_step / (2 * fp.channels)
               << " spectrum samples per block, " << (fp.subintegration_blocks ? std::to_string(fp.subintegration_blocks)
                                                                               : std::string{"all"})
-              << " block(s) per subintegration";
+              << " block(s) per subintegration" << (fp.coherence ? ", with the coherence products of streams 0 and 1" : "");
   }
   // the device chain between source and sink: one DM, or the trial DMs of dm_list
   auto start_chain = [&](auto in, auto out, int dev) {
@@ -442,7 +443,8 @@ int main(int argc, char** argv) {
   if (folds) {
     folds->finish();
     SRTB_LOGI << " [main] " << "folded " << folds->blocks() << " block(s) into " << folds->subintegrations()
-              << " subintegration(s): " << cfg.baseband_output_file_prefix << "fold.npy";
+              << " subintegration(s): " << cfg.baseband_output_file_prefix << "fold.npy"
+              << (cfg.fold_coherence ? ", " + cfg.baseband_output_file_prefix + "fold.coherence.npy" : std::string{});
   }
   srtb::device_allocator.deallocate_all_free_ptrs();
   srtb::host_allocator.deallocate_all_free_ptrs();

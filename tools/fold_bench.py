@@ -9,7 +9,11 @@ case's kernel time alone.
 Then the per-block cost of folding on the executable's path: config #3 blocks (naocpsr_snap1, 8-bit, device-resident)
 through submit_block_ex / collect_block_ex with two blocks in flight, with and without srtb_b200_fold on each collected
 block's spectra (nsub 1, nbin 256, as baseband_chain_pipe calls it), alternating over --rounds rounds of --blocks blocks;
-a host clock around each round. The card's name and power limit are read in the same run. Prints one JSON line."""
+a host clock around each round. The card's name and power limit are read in the same run. Prints one JSON line.
+
+With --coherence the same cases time srtb_b200_fold_coherence of the two streams instead (the same bytes read), and the
+block path alternates three arms: no fold, srtb_b200_fold, and srtb_b200_fold followed by srtb_b200_fold_coherence, as
+baseband_chain_pipe calls them with fold_coherence = 1."""
 import argparse
 import ctypes as C
 import json
@@ -29,6 +33,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--reps", type=int, default=10)
 ap.add_argument("--blocks", type=int, default=20)
 ap.add_argument("--rounds", type=int, default=5)
+ap.add_argument("--coherence", action="store_true", help="time srtb_b200_fold_coherence of the stream pair")
 args = ap.parse_args()
 
 torch.cuda.set_device(0)
@@ -44,23 +49,38 @@ xs[0][7].zero_()
 phase = srtb_b200.fold_phase(0.0893, 1.25e-13, 8e8, 2 * C_, 123456789)
 PEAK = 3.35e12
 
+
+
+def call(nsub, nbin):
+    """(entry, its arguments, profile elements) of one case; pinned host outputs: at nsub = 2048 the profile is 32 MiB
+    (64 MiB for the coherence products), and its copy to pageable memory would dominate"""
+    P = 4 if args.coherence else S
+    prof = torch.zeros(P * nsub * nbin, dtype=torch.float64).pin_memory()
+    hits = torch.zeros(nbin, dtype=torch.int64).pin_memory()
+    kept = torch.zeros(P * nsub, dtype=torch.int32).pin_memory()
+    keep.append((prof, hits, kept))
+    outs = (prof.data_ptr(), hits.data_ptr(), kept.data_ptr())
+    if args.coherence:
+        return (ctx.lib.srtb_b200_fold_coherence,
+                (ctx.h, xs[0].data_ptr(), xs[1].data_ptr(), L, C_, L, *phase, nbin, nsub, *outs), P * nsub * nbin)
+    arr = (C.c_void_p * S)(*[x.data_ptr() for x in xs])
+    keep.append(arr)
+    return ctx.lib.srtb_b200_fold, (ctx.h, arr, S, L, C_, L, *phase, nbin, nsub, *outs), P * nsub * nbin
+
+
+keep = []  # the host outputs and pointer arrays of the calls
 cases = []
 for nsub in (1, 64, 2048):
     for nbin in (64, 1024):
-        # pinned host outputs: at nsub = 2048 the profile is 32 MiB, and its copy to pageable memory would dominate
-        prof = torch.zeros(S * nsub * nbin, dtype=torch.float64).pin_memory()
-        hits = torch.zeros(nbin, dtype=torch.int64).pin_memory()
-        kept = torch.zeros(S * nsub, dtype=torch.int32).pin_memory()
-        arr = (C.c_void_p * S)(*[x.data_ptr() for x in xs])
-        args_ = (ctx.h, arr, S, L, C_, L, *phase, nbin, nsub, prof.data_ptr(), hits.data_ptr(), kept.data_ptr())
+        fn, args_, out_elems = call(nsub, nbin)
         for _ in range(3):
-            assert ctx.lib.srtb_b200_fold(*args_) == 0
+            assert fn(*args_) == 0
         l0 = ctx.launch_count
         times = []
         for _ in range(args.reps):
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-            rc = ctx.lib.srtb_b200_fold(*args_)
+            rc = fn(*args_)
             e1.record()
             assert rc == 0, rc
             e1.synchronize()
@@ -68,7 +88,7 @@ for nsub in (1, 64, 2048):
         ms = float(np.median(times))
         nbytes = S * C_ * L * 8
         cases.append({"nsub": nsub, "nbin": nbin, "ms_per_call": ms, "ms_all": times, "bytes": nbytes,
-                      "output_bytes_copied_to_host": S * nsub * nbin * 8,
+                      "output_bytes_copied_to_host": out_elems * 8,
                       "gb_per_s": nbytes / (ms * 1e-3) / 1e9, "share_of_3_35_tb_s": nbytes / (ms * 1e-3) / PEAK,
                       "launches_per_call": (ctx.launch_count - l0) / args.reps})
 
@@ -76,14 +96,10 @@ from torch.profiler import ProfilerActivity, profile  # noqa: E402
 
 for case in cases:
     nsub, nbin = case["nsub"], case["nbin"]
-    prof = torch.zeros(S * nsub * nbin, dtype=torch.float64).pin_memory()
-    hits = torch.zeros(nbin, dtype=torch.int64).pin_memory()
-    kept = torch.zeros(S * nsub, dtype=torch.int32).pin_memory()
-    arr = (C.c_void_p * S)(*[x.data_ptr() for x in xs])
+    fn, args_, _ = call(nsub, nbin)
     with profile(activities=[ProfilerActivity.CUDA]) as pr:
         for _ in range(5):
-            ctx.lib.srtb_b200_fold(ctx.h, arr, S, L, C_, L, *phase, nbin, nsub, prof.data_ptr(), hits.data_ptr(),
-                                   kept.data_ptr())
+            fn(*args_)
     us = 0.0
     for e in pr.events():
         if e.device_type.name == "CUDA" and "srtb_b200::fold" in e.name:
@@ -108,15 +124,21 @@ NBIN = 256
 fprof = np.zeros((S, 1, NBIN))
 fhits = np.zeros(NBIN, np.uint64)
 fkept = np.zeros((S, 1), np.uint32)
+fcoh = np.zeros((4, 1, NBIN))
+fckept = np.zeros(1, np.uint32)
 
 
 def run(fold, blocks):
+    """fold: 0 = none, 1 = srtb_b200_fold, 2 = srtb_b200_fold and srtb_b200_fold_coherence"""
     def collect(ticket):
         _, _, dspec = ctx.collect_block_ex(ticket)
         if fold:
             arr = (C.c_void_p * S)(*dspec[:S])
             assert ctx.lib.srtb_b200_fold(ctx.h, arr, S, L, C_, L, *phase, NBIN, 1, fprof.ctypes.data,
                                           fhits.ctypes.data, fkept.ctypes.data) == 0
+        if fold == 2:
+            assert ctx.lib.srtb_b200_fold_coherence(ctx.h, dspec[0], dspec[1], L, C_, L, *phase, NBIN, 1,
+                                                    fcoh.ctypes.data, fhits.ctypes.data, fckept.ctypes.data) == 0
 
     torch.cuda.synchronize()
     t0 = time.perf_counter()
@@ -130,17 +152,23 @@ def run(fold, blocks):
     return (time.perf_counter() - t0) / blocks * 1e3
 
 
-for f in (False, True):
+arms = (0, 1, 2) if args.coherence else (0, 1)
+for f in arms:
     run(f, 3)
-ms = {False: [], True: []}
+ms = {f: [] for f in arms}
 for _ in range(args.rounds):
-    for f in (False, True):
+    for f in arms:
         ms[f].append(run(f, args.blocks))
-off, on = float(np.median(ms[False])), float(np.median(ms[True]))
+off, on = float(np.median(ms[0])), float(np.median(ms[1]))
+block_path = {"blocks_per_round": args.blocks, "rounds": args.rounds, "fold_nsub": 1, "fold_nbin": NBIN,
+              "ms_per_block_off": off, "ms_per_block_on": on, "overhead": on / off - 1,
+              "ms_off_all": ms[0], "ms_on_all": ms[1]}
+if args.coherence:
+    coh = float(np.median(ms[2]))
+    block_path.update({"ms_per_block_fold_and_coherence": coh, "coherence_ms_per_block": coh - on,
+                       "ms_fold_and_coherence_all": ms[2]})
 print(json.dumps({
-    "workload": f"fold, config #3 stream shape: {S} streams of 2^26 samples, C = {C_}, L = {L}",
-    "card": card, "cases": cases,
-    "block_path": {"blocks_per_round": args.blocks, "rounds": args.rounds, "fold_nsub": 1, "fold_nbin": NBIN,
-                   "ms_per_block_off": off, "ms_per_block_on": on, "overhead": on / off - 1,
-                   "ms_off_all": ms[False], "ms_on_all": ms[True]}}))
+    "workload": f"fold{' coherence' if args.coherence else ''}, config #3 stream shape: {S} streams of 2^26 samples, "
+                f"C = {C_}, L = {L}",
+    "card": card, "cases": cases, "block_path": block_path}))
 ctx.close()
