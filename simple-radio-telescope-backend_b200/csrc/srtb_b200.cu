@@ -239,6 +239,63 @@ static inline unsigned grid_for(const srtb_b200_ctx* ctx, size_t work_items, int
   return (unsigned)std::max<size_t>(1, std::min(need, cap));
 }
 
+// Every counted kernel launch goes through here, so srtb_b200_launch_count counts each launch the runtime accepted.
+// Returns the launch's error, else cudaGetLastError().
+template <typename... KArgs, typename... Args>
+static cudaError_t launch(srtb_b200_ctx* ctx, const cudaLaunchConfig_t& cfg, void (*kern)(KArgs...), Args&&... args) {
+  const cudaError_t e = cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
+  if (e != cudaSuccess) return e;
+  ctx->launches++;
+  return cudaGetLastError();
+}
+
+// A launch on the current lane's stream. pdl: programmatic dependent launch along the block path (ctx->pdl_auto): the
+// kernel's set-up (tables into shared memory, barriers) overlaps its predecessor's tail, so such a kernel must call
+// pdl_wait() before touching anything a predecessor produces. It pays where kernels are short (2^24-sample blocks) and
+// can cost where they are long, since the early-resident CTAs of the next kernel only take shared memory from the
+// running one. Hence: on for blocks up to 2^25 samples, off above and outside a block.
+template <typename... KArgs, typename... Args>
+static cudaError_t launch(srtb_b200_ctx* ctx, bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem,
+                          Args&&... args) {
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr.val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = grid;
+  cfg.blockDim = block;
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = ctx->lane.stream;
+  cfg.attrs = &attr;
+  cfg.numAttrs = pdl && ctx->pdl_auto ? 1 : 0;
+  return launch(ctx, cfg, kern, std::forward<Args>(args)...);
+}
+
+// a kernel's dynamic shared-memory limit, set once per context to `bytes`: the largest size any of its launches asks for
+template <class K>
+static int set_smem_max(srtb_b200_ctx* ctx, K kern, size_t bytes) {
+  const void* key = reinterpret_cast<const void*>(kern);
+  if (ctx->configured.count(key)) return 0;
+  CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  ctx->configured.insert(key);
+  return 0;
+}
+
+// grid of a persistent kernel: ntiles CTAs, at most one wave (resident CTAs per SM found once, at the smem of the first
+// launch, under a limit of smem_max)
+template <class K>
+static int persistent_grid(srtb_b200_ctx* ctx, K kern, int threads, size_t smem, size_t smem_max, size_t ntiles,
+                           unsigned* grid) {
+  if (int rc = set_smem_max(ctx, kern, smem_max)) return rc;
+  const void* key = reinterpret_cast<const void*>(kern);
+  if (!ctx->occupancy.count(key)) {
+    int per_sm = 1;
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
+    ctx->occupancy[key] = std::max(1, per_sm);
+  }
+  *grid = (unsigned)std::min<size_t>(ntiles, (size_t)ctx->sm_count * ctx->occupancy[key]);
+  return 0;
+}
+
 // records a CUDA-event pair around one stage call when per-stage statistics are enabled
 struct stage_scope {
   srtb_b200_ctx* ctx;
@@ -385,22 +442,17 @@ static int launch_unpack_simple(srtb_b200_ctx* ctx, const void* d_in, float* out
   const bool aligned = ((reinterpret_cast<uintptr_t>(d_in) & 15u) == 0) &&
                        ((reinterpret_cast<uintptr_t>(out) & 15u) == 0);
   if (!aligned) {
-    unpack_simple_scalar_kernel<BITS><<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(d_in, out, n, window);
-  } else if (window == 0) {
-    unpack_simple_kernel<BITS, false><<<grid_for(ctx, n / 16 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, out, n, window);
+    CK(launch(ctx, false, unpack_simple_scalar_kernel<BITS>, grid_for(ctx, n, 256), 256, 0, d_in, out, n, window));
   } else {
-    unpack_simple_kernel<BITS, true><<<grid_for(ctx, n / 16 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, out, n, window);
+    auto kern = window == 0 ? unpack_simple_kernel<BITS, false> : unpack_simple_kernel<BITS, true>;
+    CK(launch(ctx, false, kern, grid_for(ctx, n / 16 + 1, 256), 256, 0, d_in, out, n, window));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   return 0;
 }
 
 template <int BITS>
 static int launch_unpack_il2(srtb_b200_ctx* ctx, const void* d_in, float* o1, float* o2, size_t n, int window) {
-  unpack_interleaved2_kernel<BITS><<<grid_for(ctx, n / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, o1, o2, n, window);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, unpack_interleaved2_kernel<BITS>, grid_for(ctx, n / 4 + 1, 256), 256, 0, d_in, o1, o2, n, window));
   return 0;
 }
 
@@ -474,19 +526,18 @@ extern "C" int srtb_b200_unpack(srtb_b200_ctx* ctx, const void* d_in, size_t in_
     case SRTB_B200_FORMAT_NAOCPSR_SNAP1:
       if (bits != -8)
         return fail(ctx, SRTB_B200_E_UNSUPPORTED, "naocpsr_snap1 requires baseband_input_bits = -8");
-      unpack_snap1_kernel<<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(d_in, d_out[0], d_out[1], out_count, window);
+      CK(launch(ctx, false, unpack_snap1_kernel, grid_for(ctx, out_count / 4 + 1, 256), 256, 0, d_in, d_out[0], d_out[1],
+                out_count, window));
       break;
     case SRTB_B200_FORMAT_GZNUPSR_A1_2:
-      unpack_gznupsr_kernel<2><<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(
-          d_in, d_out[0], d_out[1], nullptr, nullptr, out_count, window);
+      CK(launch(ctx, false, unpack_gznupsr_kernel<2>, grid_for(ctx, out_count / 4 + 1, 256), 256, 0, d_in, d_out[0],
+                d_out[1], nullptr, nullptr, out_count, window));
       break;
     case SRTB_B200_FORMAT_GZNUPSR_A1_4:
-      unpack_gznupsr_kernel<4><<<grid_for(ctx, out_count / 4 + 1, 256), 256, 0, ctx->lane.stream>>>(
-          d_in, d_out[0], d_out[1], d_out[2], d_out[3], out_count, window);
+      CK(launch(ctx, false, unpack_gznupsr_kernel<4>, grid_for(ctx, out_count / 4 + 1, 256), 256, 0, d_in, d_out[0],
+                d_out[1], d_out[2], d_out[3], out_count, window));
       break;
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   return 0;
 }
 
@@ -544,16 +595,11 @@ template <int LOGL, int T, int MODE, bool FWD, class IO>
 static int launch_pass(srtb_b200_ctx* ctx, const IO& io, unsigned grid, size_t extra_smem) {
   auto kern = fft_pass_kernel<LOGL, T, MODE, FWD, IO>;
   const size_t smem = (size_t)tile_layout<LOGL, T, MODE>::ELEMS * sizeof(float2) + extra_smem;
-  const void* key = reinterpret_cast<const void*>(kern);
-  if (smem > 48 * 1024 && !ctx->configured.count(key)) {
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(200 * 1024)));
-    ctx->configured.insert(key);
-  }
+  if (smem > 48 * 1024)
+    if (int rc = set_smem_max(ctx, kern, 200 * 1024)) return rc;
   const float2* tw = nullptr;
   if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-  kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(io, tw);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, kern, grid, pass_threads<LOGL, T>::value, smem, io, tw));
   return 0;
 }
 
@@ -586,30 +632,19 @@ static int launch_row(srtb_b200_ctx* ctx, const float2* in, float2* out, size_t 
       if (int rc = persistent_grid(ctx, kern, threads, smem, smem, ntiles, &grid)) return rc;
       const float2* tw = nullptr;
       if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-      CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem, in, out, nrows, tw, row_sk_params{}, row_chirp_params{}));
-      ctx->launches++;
-      CK(cudaGetLastError());
+      CK(launch(ctx, true, kern, grid, threads, smem, in, out, nrows, tw, row_sk_params{}, row_chirp_params{}));
       return 0;
     }
   } else if ((reinterpret_cast<uintptr_t>(in) & 15u) == 0) {
     // persistent TMA-fed kernel (cp.async.bulk needs 16-byte aligned rows)
     auto kern = fft_row_tma_kernel<LOGL, T, FWD>;
+    constexpr int threads = pass_threads<LOGL, T>::value;
     constexpr size_t smem = row_tma_smem<LOGL, T>::bytes;
-    const void* key = reinterpret_cast<const void*>(kern);
-    if (!ctx->configured.count(key)) {
-      CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      int per_sm = 1;
-      CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, pass_threads<LOGL, T>::value, smem));
-      ctx->occupancy[key] = std::max(1, per_sm);
-      ctx->configured.insert(key);
-    }
+    unsigned grid = 1;
+    if (int rc = persistent_grid(ctx, kern, threads, smem, smem, (nrows + T - 1) / T, &grid)) return rc;
     const float2* tw = nullptr;
     if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
-    const size_t ntiles = (nrows + T - 1) / T;
-    const unsigned grid = (unsigned)std::min<size_t>(ntiles, (size_t)ctx->sm_count * ctx->occupancy[key]);
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(in, out, nrows, tw, row_sk_params{});
-    ctx->launches++;
-    CK(cudaGetLastError());
+    CK(launch(ctx, false, kern, grid, threads, smem, in, out, nrows, tw, row_sk_params{}));
     return 0;
   }
   row_io<LOGL, T> io;
@@ -654,42 +689,6 @@ static bool make_tensor_map(tensor_map_blob* out, const void* base, int rank, co
   if (r != CUDA_SUCCESS) return false;
   std::memcpy(out->bytes, &m, sizeof(m));
   return true;
-}
-
-// Programmatic dependent launch along the block path: each kernel's set-up (tables into shared memory, barriers) overlaps
-// its predecessor's tail; every such kernel calls pdl_wait() before touching anything a predecessor produces. It pays
-// where kernels are short (2^24-sample blocks) and can cost where they are long, since the
-// early-resident CTAs of the next kernel only take shared memory from the running one. Hence: on for blocks up to 2^25
-// samples, off above and outside a block.
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_pdl(srtb_b200_ctx* ctx, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args&&... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = ctx->lane.stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = ctx->pdl_auto ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
-}
-
-template <class K>
-static int persistent_grid(srtb_b200_ctx* ctx, K kern, int threads, size_t smem, size_t smem_max, size_t ntiles,
-                           unsigned* grid) {
-  const void* key = reinterpret_cast<const void*>(kern);
-  if (!ctx->configured.count(key)) {
-    // the attribute is set once per kernel: use the largest size any later launch can ask for
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-    int per_sm = 1;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
-    ctx->occupancy[key] = std::max(1, per_sm);
-    ctx->configured.insert(key);
-  }
-  *grid = (unsigned)std::min<size_t>(ntiles, (size_t)ctx->sm_count * ctx->occupancy[key]);
-  return 0;
 }
 
 // three-sweep factorisation of 2^q: the first sweep takes ceil(q/3); of the rest the longer half goes to the
@@ -753,26 +752,23 @@ static int launch_col_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, siz
       if (chirp) {  // s1 + chirp applied as the tile is read (long waterfall rows: a 2^8 or 2^9 first sweep)
         auto kernc = fft_col16_tma_kernel<LOGL, T, FWD, 0, true>;
         if (int rc = persistent_grid(ctx, kernc, threads, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-        CK(launch_pdl(ctx, kernc, dim3(grid), dim3(threads), smem, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
-                      raw_params{}, *chirp));
-        ctx->launches++;
-        CK(cudaGetLastError());
+        CK(launch(ctx, true, kernc, grid, threads, smem, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
+                  raw_params{}, *chirp));
         *done = true;
         return 0;
       }
     } else {
       if (chirp) return 0;  // no chirp-on-load kernel for a 2^7 column sweep (nor for a forward one)
     }
-    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
-                  raw_params{}, row_chirp_params{}));
+    CK(launch(ctx, true, kern16, grid, threads, smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw,
+              raw_params{}, row_chirp_params{}));
   } else {
     if (chirp) return 0;  // the chirp-on-load sweep exists for the sixteen-point kernel only
     auto kern = fft_col_tma_kernel<LOGL, T, FWD>;
     if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, tile_tma_smem<LOGL, T>::bytes(10), ntiles, &grid)) return rc;
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw);
+    CK(launch(ctx, false, kern, grid, pass_threads<LOGL, T>::value, smem, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles,
+              btw, tw));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   *done = true;
   return 0;
 }
@@ -821,15 +817,13 @@ static int launch_col_tma_raw(srtb_b200_ctx* ctx, const raw_source& src, float2*
     static_assert(T == 8, "the 2^11-point raw sweep has 32-byte raw rows and 64-byte stores");
     auto kern = r2c_raw_col2048_kernel<RAW>;
     if (int rc = persistent_grid(ctx, kern, threads, smem16, smem16, ntiles, &grid)) return rc;
-    CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp));
+    CK(launch(ctx, true, kern, grid, threads, smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp));
   } else {
     auto kern16 = fft_col16_tma_kernel<LOGL, T, true, RAW>;
     if (int rc = persistent_grid(ctx, kern16, threads, smem16, smem16, ntiles, &grid)) return rc;
-    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
-                  row_chirp_params{}));
+    CK(launch(ctx, true, kern16, grid, threads, smem16, tm, out, B, (uint32_t)(B / T), (uint32_t)ntiles, btw, tw, rp,
+              row_chirp_params{}));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   *done = true;
   return 0;
 }
@@ -874,17 +868,15 @@ static int launch_trans_tma(srtb_b200_ctx* ctx, const float2* in, float2* out, s
     auto kern16 = fft_trans16_tma_kernel<LOGL, T, FWD>;
     constexpr int threads = T * (L / 16);
     if (int rc = persistent_grid(ctx, kern16, threads, smem, smem, ntiles, &grid)) return rc;
-    kern16<<<grid, threads, smem, ctx->lane.stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1, (uint32_t)k1tiles,
-                                                      (uint32_t)ntiles, tw, (uint32_t)rest_inner, tile_stats);
+    CK(launch(ctx, false, kern16, grid, threads, smem, tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1, (uint32_t)k1tiles,
+              (uint32_t)ntiles, tw, (uint32_t)rest_inner, tile_stats));
   } else {
     if (rest_inner > 1) return 0;  // only the sixteen-point kernel knows the four-sweep row order
     auto kern = fft_trans_tma_kernel<LOGL, T, FWD>;
     if (int rc = persistent_grid(ctx, kern, pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
-                                                                         (uint32_t)k1tiles, (uint32_t)ntiles, tw, tile_stats);
+    CK(launch(ctx, false, kern, grid, pass_threads<LOGL, T>::value, smem, tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
+              (uint32_t)k1tiles, (uint32_t)ntiles, tw, tile_stats));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   *done = true;
   return 0;
 }
@@ -1008,10 +1000,8 @@ static int launch_bigrow(srtb_b200_ctx* ctx, const float2* in, float2* out, size
       sk->partial = ctx->lane.colsum_partial.p;
       p = *sk;
     }
-    CK(launch_pdl(ctx, kern, dim3(grid), dim3(C::NT), smem, in, out, (unsigned)nrows, tabs, p,
-                  chirp ? *chirp : row_chirp_params{}, extra...));
-    ctx->launches++;
-    CK(cudaGetLastError());
+    CK(launch(ctx, true, kern, grid, C::NT, smem, in, out, (unsigned)nrows, tabs, p, chirp ? *chirp : row_chirp_params{},
+              extra...));
     if (chunks_out) *chunks_out = grid;
     return 0;
   };
@@ -1062,24 +1052,20 @@ static int launch_r2c_rows(srtb_b200_ctx* ctx, const float2* s, float2* out, siz
   cfg.stream = ctx->lane.stream;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
+  if (int rc = set_smem_max(ctx, kern, C::bytes_r2c)) return rc;
   const void* key = reinterpret_cast<const void*>(kern);
-  if (!ctx->configured.count(key)) {
-    CK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C::bytes_r2c));
+  if (!ctx->occupancy.count(key)) {
     int clusters = 0;
     cfg.gridDim = dim3(2 * (unsigned)ctx->sm_count);
     CK(cudaOccupancyMaxActiveClusters(&clusters, kern, &cfg));
     if (clusters < 1) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "r2c: no two-CTA cluster of the row sweep fits an SM pair");
     ctx->occupancy[key] = clusters;
-    ctx->configured.insert(key);
   }
   const unsigned clusters = (unsigned)std::min<size_t>(P / 2, (size_t)ctx->occupancy[key]);
   if (2 * clusters > 4096) return fail(ctx, SRTB_B200_E_SIZE, "r2c: partial buffer too small");
   cfg.gridDim = dim3(2 * clusters);
   cfg.numAttrs = ctx->pdl_auto ? 2 : 1;
-  CK(cudaLaunchKernelEx(&cfg, kern, s, out, (unsigned)P, tabs,
-                        r2c_rows_params{ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean}));
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, cfg, kern, s, out, (unsigned)P, tabs, r2c_rows_params{ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean}));
   return 0;
 }
 
@@ -1108,9 +1094,7 @@ static int fft_c2c_impl(srtb_b200_ctx* ctx, float2* x, size_t n, size_t batch) {
   const int q = ilog2(n);
   if (q == 0) return 0;
   if (q <= 2) {
-    tiny_fft_kernel<FWD><<<(unsigned)((batch + 255) / 256), 256, 0, ctx->lane.stream>>>(x, q, batch);
-    ctx->launches++;
-    CK(cudaGetLastError());
+    CK(launch(ctx, false, tiny_fft_kernel<FWD>, (unsigned)((batch + 255) / 256), 256, 0, x, q, batch));
     return 0;
   }
   if (q <= 12) return dispatch_row<FWD>(ctx, q, x, x, batch);
@@ -1190,9 +1174,7 @@ extern "C" int srtb_b200_fft_r2c_inplace(srtb_b200_ctx* ctx, float* d_inout, siz
     return fft_r2c_with_power_mean(ctx, d_inout, n_real);  // multi-sweep sizes: split fused into the last sweep
   float2* H = reinterpret_cast<float2*>(d_inout);
   if (int rc = fft_c2c_impl<true>(ctx, H, M, 1)) return rc;
-  r2c_post_kernel<false><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(H, M, nullptr, nullptr, nullptr);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, r2c_post_kernel<false>, grid_for(ctx, M / 2 + 1, 256), 256, 0, H, M, nullptr, nullptr, nullptr));
   return 0;
 }
 
@@ -1219,28 +1201,23 @@ static int launch_trans_r2c(srtb_b200_ctx* ctx, const float2* in, float2* out, s
     constexpr int threads = 2 * T * (L / 16);
     if (int rc = persistent_grid(ctx, kern16, threads, smem, smem, ntiles, &grid)) return rc;
     grid = std::min<unsigned>(grid, 2048);
-    CK(launch_pdl(ctx, kern16, dim3(grid), dim3(threads), smem, tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
-                  (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw, ctx->lane.partial, (uint32_t)rest_inner));
+    CK(launch(ctx, true, kern16, grid, threads, smem, tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
+              (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw, ctx->lane.partial, (uint32_t)rest_inner));
   } else {
     if (rest_inner > 1) return 0;  // four-sweep row order: sixteen-point kernel only
     auto kern = fft_trans_r2c_tma_kernel<LOGL, T>;
     if (int rc = persistent_grid(ctx, kern, 2 * pass_threads<LOGL, T>::value, smem, smem, ntiles, &grid)) return rc;
     grid = std::min<unsigned>(grid, 2048);
-    kern<<<grid, 2 * pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(tm, out, (uint32_t)A, (uint32_t)S, (uint32_t)L1,
-                                                                        (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw,
-                                                                        ctx->lane.partial);
+    CK(launch(ctx, false, kern, grid, 2 * pass_threads<LOGL, T>::value, smem, tm, out, (uint32_t)A, (uint32_t)S,
+              (uint32_t)L1, (uint32_t)tiles_per_rest, (uint32_t)ntiles, tw, ctx->lane.partial));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   {
     const size_t pairs = ((A << LOGL) / L1) / 2 + 1;
     const unsigned fgrid = (unsigned)std::min<size_t>((pairs + 255) / 256, 2048);
     if (grid + fgrid > 4096) return fail(ctx, SRTB_B200_E_SIZE, "r2c: partial buffer too small");
-    CK(launch_pdl(ctx, r2c_col0_fixup_kernel, dim3(fgrid), dim3(256), 0, out, (size_t)(A << LOGL), (size_t)L1, ctx->lane.partial,
-                  (unsigned)grid, ctx->lane.ticket, ctx->lane.mean));
+    CK(launch(ctx, true, r2c_col0_fixup_kernel, fgrid, 256, 0, out, (size_t)(A << LOGL), (size_t)L1, ctx->lane.partial,
+              (unsigned)grid, ctx->lane.ticket, ctx->lane.mean));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   *done = true;
   return 0;
 }
@@ -1315,18 +1292,14 @@ static int fft_r2c_with_power_mean(srtb_b200_ctx* ctx, float* d_inout, size_t n_
       // tensor map refused: finish with the plain last pass + split kernel
       if (int rc2 = dispatch_trans<true>(ctx, llast, s, H, 1, A, L1)) return rc2;
       const unsigned grid = std::min<unsigned>(grid_for(ctx, M / 2 + 1, 256), 4096);
-      r2c_post_kernel<true><<<grid, 256, 0, ctx->lane.stream>>>(H, M, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean);
-      ctx->launches++;
-      CK(cudaGetLastError());
+      CK(launch(ctx, false, r2c_post_kernel<true>, grid, 256, 0, H, M, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean));
       return 0;
     }
   }
   if (raw && raw->base) return SRTB_B200_E_UNSUPPORTED;  // fused unpack needs the multi-pass TMA route
   if (int rc = fft_c2c_impl<true>(ctx, H, M, 1)) return rc;
   const unsigned grid = std::min<unsigned>(grid_for(ctx, M / 2 + 1, 256), 4096);
-  r2c_post_kernel<true><<<grid, 256, 0, ctx->lane.stream>>>(H, M, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, r2c_post_kernel<true>, grid, 256, 0, H, M, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean));
   return 0;
 }
 
@@ -1410,9 +1383,7 @@ static int zero_bin_ranges(srtb_b200_ctx* ctx, float2* x, const std::vector<size
       longest = std::max<size_t>(longest, br.hi[r] - br.lo[r] + 1);
     }
     dim3 g(grid_for(ctx, longest, 256), (unsigned)nr);
-    CK(launch_pdl(ctx, rfi_zero_ranges_kernel, g, dim3(256), 0, x, br));
-    ctx->launches++;
-    CK(cudaGetLastError());
+    CK(launch(ctx, true, rfi_zero_ranges_kernel, g, 256, 0, x, br));
   }
   return 0;
 }
@@ -1433,13 +1404,10 @@ extern "C" int srtb_b200_rfi_s1(srtb_b200_ctx* ctx, void* d_x, size_t count, flo
   stage_scope stats_(ctx, SRTB_B200_STAGE_RFI_S1, 24.0 * (double)count);
   float2* x = static_cast<float2*>(d_x);
   const unsigned grid = std::min<unsigned>(grid_for(ctx, count / 2 + 1, 256), 4096);
-  power_sum_kernel<<<grid, 256, 0, ctx->lane.stream>>>(x, count, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, power_sum_kernel, grid, 256, 0, x, count, ctx->lane.partial, ctx->lane.ticket, ctx->lane.mean));
   if (d_mean_out) CK(cudaMemcpyAsync(d_mean_out, ctx->lane.mean, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
-  rfi_s1_apply_kernel<<<grid_for(ctx, count / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(x, count, ctx->lane.mean, avg_threshold, norm_coef);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, rfi_s1_apply_kernel, grid_for(ctx, count / 2 + 1, 256), 256, 0, x, count, ctx->lane.mean,
+            avg_threshold, norm_coef));
   return zero_bin_ranges(ctx, x, bins);
 }
 
@@ -1456,10 +1424,9 @@ extern "C" int srtb_b200_dedisperse(srtb_b200_ctx* ctx, void* d_x, size_t count,
   stage_scope stats_(ctx, SRTB_B200_STAGE_DEDISPERSE, 16.0 * (double)count);
   constexpr double D = 4.148808e3;  // coherent_dedispersion.hpp:67
   const double ddm = (D * 1e6) * (double)dm;
-  dedisperse_kernel<false><<<grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, ctx->lane.stream>>>(
-      static_cast<const float2*>(d_x), static_cast<float2*>(d_x), count, (double)f_min, (double)df, (double)f_c, ddm, nullptr, 0.f, 1.f);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, dedisperse_kernel<false>, grid_for(ctx, count / 2 + 1, 256, 16), 256, 0,
+            static_cast<const float2*>(d_x), static_cast<float2*>(d_x), count, (double)f_min, (double)df, (double)f_c, ddm,
+            nullptr, 0.f, 1.f));
   return 0;
 }
 
@@ -1470,10 +1437,8 @@ static int rfi_s1_dedisperse_fused(srtb_b200_ctx* ctx, float2* x, const float2* 
                                    float coef, const std::vector<size_t>& bins, float f_min, float f_c, float df, float dm) {
   constexpr double D = 4.148808e3;
   const double ddm = (D * 1e6) * (double)dm;
-  dedisperse_kernel<true><<<grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, ctx->lane.stream>>>(
-      src, x, count, (double)f_min, (double)df, (double)f_c, ddm, ctx->lane.mean, avg_threshold, coef);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, dedisperse_kernel<true>, grid_for(ctx, count / 2 + 1, 256, 16), 256, 0, src, x, count,
+            (double)f_min, (double)df, (double)f_c, ddm, ctx->lane.mean, avg_threshold, coef));
   return zero_bin_ranges(ctx, x, bins);
 }
 
@@ -1515,9 +1480,7 @@ extern "C" int srtb_b200_rfi_s2_sk(srtb_b200_ctx* ctx, void* d_x, size_t time_co
   CK(cudaSetDevice(ctx->device));
   stage_scope stats_(ctx, SRTB_B200_STAGE_RFI_S2, 8.0 * (double)time_count * (double)chan_count);
   const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
-  sk_kernel<<<(unsigned)chan_count, 256, 0, ctx->lane.stream>>>(static_cast<float2*>(d_x), time_count, lo_, hi_, d_sk_out);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, sk_kernel, (unsigned)chan_count, 256, 0, static_cast<float2*>(d_x), time_count, lo_, hi_, d_sk_out));
   return 0;
 }
 
@@ -1581,22 +1544,13 @@ static int detect_tail(srtb_b200_ctx* ctx, const detect_out& out, const float* p
   std::optional<stage_scope> stats_;
   if (partial) stats_.emplace(ctx, SRTB_B200_STAGE_FUSED_DETECT_TAIL, 4.0 * (double)chunks * (double)ts_count);
   const size_t scan_ctas = partial ? (ts_count + 31) / 32 : (chan_count + 1023) / 1024;
-  CK(launch_pdl(ctx, colsum_final_scan_kernel, dim3((unsigned)std::min<size_t>(scan_ctas, (size_t)ctx->sm_count)),
-                dim3(1024), 0, partial, ts_count, chunks, ctx->series[slot].p, ctx->lane.acc.p, x, zero_stride,
-                chan_count, chan_thr, max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0, out.raw));
-  ctx->launches++;
-  CK(cudaGetLastError());
-  const unsigned max_nb = boxcar_ctas(max_boxcar, ts_count);
-  if (out.peak)
-    CK(launch_pdl(ctx, detect_boxcar_kernel<true>, dim3(max_nb), dim3(1024), 0, ctx->series[slot].p, time_count,
-                  (const float*)ctx->lane.acc.p, ts_count, snr, ctx->d_res + slot, out.host_series, out.peak, (size_t)0,
-                  (size_t)0));
-  else
-    CK(launch_pdl(ctx, detect_boxcar_kernel<false>, dim3(max_nb), dim3(1024), 0, ctx->series[slot].p, time_count,
-                  (const float*)ctx->lane.acc.p, ts_count, snr, ctx->d_res + slot, out.host_series,
-                  (detect_dev_peak*)nullptr, (size_t)0, (size_t)0));
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, true, colsum_final_scan_kernel, (unsigned)std::min<size_t>(scan_ctas, (size_t)ctx->sm_count), 1024, 0,
+            partial, ts_count, chunks, ctx->series[slot].p, ctx->lane.acc.p, x, zero_stride, chan_count, chan_thr,
+            max_boxcar, ctx->lane.detect_ticket, ctx->d_res + slot, (size_t)0, (size_t)0, out.raw));
+  auto boxcar = out.peak ? detect_boxcar_kernel<true> : detect_boxcar_kernel<false>;
+  CK(launch(ctx, true, boxcar, boxcar_ctas(max_boxcar, ts_count), 1024, 0, ctx->series[slot].p, time_count,
+            (const float*)ctx->lane.acc.p, ts_count, snr, ctx->d_res + slot, out.host_series, out.peak, (size_t)0,
+            (size_t)0));
   ctx->slot_time_count[slot] = time_count;
   return 0;
 }
@@ -1609,10 +1563,8 @@ static int detect_enqueue(srtb_b200_ctx* ctx, const detect_out& out, const float
   if (int rc = detect_prepare(ctx, out.slot, time_count, cg.chunks * ts_count)) return rc;
   CK(cudaMemsetAsync(ctx->d_res + out.slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
   dim3 g((unsigned)cg.ctas_per_chunk, (unsigned)cg.chunks);
-  colsum_partial_kernel<<<g, 256, 0, ctx->lane.stream>>>(const_cast<float2*>(x), time_count, chan_count, ts_count,
-                                                         cg.rows_per_chunk, ctx->lane.colsum_partial.p, nullptr);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, colsum_partial_kernel, g, 256, 0, const_cast<float2*>(x), time_count, chan_count, ts_count,
+            cg.rows_per_chunk, ctx->lane.colsum_partial.p, nullptr));
   return detect_tail(ctx, out, ctx->lane.colsum_partial.p, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr,
                      max_boxcar);
 }
@@ -1643,7 +1595,7 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
     if (int rc = grow(ctx, ctx->lane.colsum_partial, (size_t)grid * ts_count * sizeof(float))) return rc;
     if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
     row_sk_params p{lo_, hi_, ctx->lane.colsum_partial.p, (unsigned)ts_count};
-    CK(launch_pdl(ctx, kern, dim3(grid), dim3(threads), smem, src, x, chan_count, tw, p, chirp ? *chirp : row_chirp_params{}));
+    CK(launch(ctx, true, kern, grid, threads, smem, src, x, chan_count, tw, p, chirp ? *chirp : row_chirp_params{}));
   } else {
     if (chirp || src != x) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: fused chirp needs the sixteen-point row kernel");
     constexpr int T = row_t<LOGL>::value;
@@ -1654,10 +1606,8 @@ static int watfft_sk_launch(srtb_b200_ctx* ctx, float2* x, size_t chan_count, fl
     if (int rc = grow(ctx, ctx->lane.colsum_partial, (size_t)grid * ts_count * sizeof(float))) return rc;
     if (int rc = get_stage_twiddles(ctx, LOGL, &tw)) return rc;
     row_sk_params p{lo_, hi_, ctx->lane.colsum_partial.p, (unsigned)ts_count};
-    kern<<<grid, pass_threads<LOGL, T>::value, smem, ctx->lane.stream>>>(x, x, chan_count, tw, p);
+    CK(launch(ctx, false, kern, grid, pass_threads<LOGL, T>::value, smem, x, x, chan_count, tw, p));
   }
-  ctx->launches++;
-  CK(cudaGetLastError());
   *chunks_out = grid;
   return 0;
 }
@@ -1774,19 +1724,15 @@ static int watfft_long_fused(srtb_b200_ctx* ctx, const detect_out& out, float2* 
   if (rc) return rc;
   if (!done) return fail(ctx, SRTB_B200_E_UNSUPPORTED, "watfft: long fused plan needs the TMA last sweep");
   const auto [lo_, hi_] = sk_bounds(sk_threshold, time_count);
-  sk_decide_kernel<<<(unsigned)((chan_count + 255) / 256), 256, 0, ctx->lane.stream>>>(
-      stats, (unsigned)tiles_per_row, chan_count, static_cast<float>(time_count), lo_, hi_, zap);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, sk_decide_kernel, (unsigned)((chan_count + 255) / 256), 256, 0, stats, (unsigned)tiles_per_row,
+            chan_count, static_cast<float>(time_count), lo_, hi_, zap));
   // partial column sums (all time samples are visited so that flagged rows are zeroed completely)
   const colsum_chunks cg = colsum_geometry(ctx, time_count, chan_count);
   if (int rc2 = detect_prepare(ctx, out.slot, time_count, cg.chunks * ts_count)) return rc2;
   if (!out.header_zeroed) CK(cudaMemsetAsync(ctx->d_res + out.slot, 0, sizeof(detect_dev_result), ctx->lane.stream));
   dim3 g((unsigned)cg.ctas_per_chunk, (unsigned)cg.chunks);
-  colsum_partial_kernel<<<g, 256, 0, ctx->lane.stream>>>(x, time_count, chan_count, ts_count, cg.rows_per_chunk,
-                                                         ctx->lane.colsum_partial.p, zap);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, colsum_partial_kernel, g, 256, 0, x, time_count, chan_count, ts_count, cg.rows_per_chunk,
+            ctx->lane.colsum_partial.p, zap));
   stats_.reset();
   return detect_tail(ctx, out, ctx->lane.colsum_partial.p, x, time_count, chan_count, ts_count, cg.chunks, snr, chan_thr,
                      max_boxcar);
@@ -1840,13 +1786,11 @@ static int sk_v1_enqueue(srtb_b200_ctx* ctx, float2* x, size_t fft_bins, size_t 
   if (int rc = grow(ctx, ctx->lane.long_zap, fft_bins)) return rc;
   unsigned char* zap = ctx->lane.long_zap.p;
   const auto [lo_, hi_] = sk_bounds(sk_threshold, time_counts);
-  sk_v1_stats_kernel<<<(unsigned)((fft_bins + 31) / 32), 256, 0, ctx->lane.stream>>>(x, fft_bins, time_counts, lo_, hi_, zap, d_sk_out);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, sk_v1_stats_kernel, (unsigned)((fft_bins + 31) / 32), 256, 0, x, fft_bins, time_counts, lo_, hi_,
+            zap, d_sk_out));
   const unsigned gy = (unsigned)std::max<size_t>(1, std::min<size_t>(time_counts, 64));
-  sk_v1_zero_kernel<<<dim3((unsigned)((fft_bins + 255) / 256), gy), 256, 0, ctx->lane.stream>>>(x, fft_bins, time_counts, zap);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, sk_v1_zero_kernel, dim3((unsigned)((fft_bins + 255) / 256), gy), 256, 0, x, fft_bins, time_counts,
+            zap));
   return 0;
 }
 
@@ -1875,9 +1819,8 @@ extern "C" int srtb_b200_signal_detect_v1(srtb_b200_ctx* ctx, void* d_x, size_t 
   // batch_size values, masked channels counted over the first spectrum
   if (int rc = detect_prepare(ctx, 0, batch_size, batch_size)) return rc;
   CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result), ctx->lane.stream));
-  rowsum_norm_kernel<<<(unsigned)((batch_size + 7) / 8), 256, 0, ctx->lane.stream>>>(x, count_per_batch, batch_size, ctx->lane.colsum_partial.p);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, rowsum_norm_kernel, (unsigned)((batch_size + 7) / 8), 256, 0, x, count_per_batch, batch_size,
+            ctx->lane.colsum_partial.p));
   if (int rc = detect_tail(ctx, detect_out{}, ctx->lane.colsum_partial.p, x, batch_size, count_per_batch, batch_size, 1,
                            snr_threshold, channel_threshold, max_boxcar_length, /*zero_stride=*/1))
     return rc;
@@ -1954,6 +1897,7 @@ static int get_chirp_table(srtb_b200_ctx* ctx, size_t n, const row_chirp_params&
   }
   if (int rc = grow(ctx, ctx->chirp_tab, n * sizeof(float))) return rc;
   if (int rc = sync_lanes(ctx)) return rc;  // a block still in flight may be reading the previous table
+  // a synchronous table build, like the twiddle uploads: not counted as a launch
   chirp_phase_table_kernel<<<grid_for(ctx, n, 256), 256, 0, ctx->lane.stream>>>(ctx->chirp_tab.p, n, cp.f_min, cp.df, cp.inv_fc,
                                                                            cp.f_c, cp.ddm);
   CK(cudaGetLastError());
@@ -2173,13 +2117,9 @@ static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* buf
     in.raw[s] = raw + (size_t)s * L;
   }
   CK(cudaMemsetAsync(ctx->d_res + SUM_SLOT, 0, sizeof(detect_dev_result), ctx->lane.stream));
-  stream_sum_mask_kernel<<<1, 1024, 0, ctx->lane.stream>>>(in, p.streams, L, C, mask, mis, n_mis);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  CK(launch_pdl(ctx, stream_sum_kernel, dim3(grid_for(ctx, ts, 256)), dim3(256), 0, in, p.streams, L, ts,
-                (const uint2*)mis, (const unsigned*)n_mis, ctx->series[SUM_SLOT].p));
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, stream_sum_mask_kernel, 1, 1024, 0, in, p.streams, L, C, mask, mis, n_mis));
+  CK(launch(ctx, true, stream_sum_kernel, grid_for(ctx, ts, 256), 256, 0, in, p.streams, L, ts, (const uint2*)mis,
+            (const unsigned*)n_mis, ctx->series[SUM_SLOT].p));
   // the tail counts the mask's zeros (stride 1): the union count. The first lane's ticket and scan buffer are free here:
   // its own stream's tail has finished in stream order.
   const detect_out out{SUM_SLOT, host_series ? host_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * L : nullptr,
@@ -2198,7 +2138,7 @@ static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* buf
 static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* d_baseband, size_t baseband_bytes,
                          int res_base, float* const* bufs, float* host_series, bool join_lanes = true,
                          bool* alt_used = nullptr) {
-  struct pdl_scope {  // launch_pdl reads ctx->pdl_auto; it is only meaningful inside this call
+  struct pdl_scope {  // launch reads ctx->pdl_auto; it is only meaningful inside this call
     srtb_b200_ctx* c;
     ~pdl_scope() { c->pdl_auto = false; }
   } pdl_scope_{ctx};
@@ -2508,6 +2448,7 @@ extern "C" int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, fl
 static int incoherent_tables(srtb_b200_ctx* ctx, size_t C, float freq_low, float bandwidth, float sample_rate,
                              float dm, const float* dms, size_t n_dm) {
   std::vector<double> key = {(double)C, freq_low, bandwidth, sample_rate, dm};
+  key.reserve(key.size() + n_dm);  // no reallocating insert: g++ 13 warns falsely on it once this is inlined
   key.insert(key.end(), dms, dms + n_dm);
   if (key == ctx->inc_key) return 0;
   ctx->inc_key.clear();
@@ -2614,31 +2555,19 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   CK(cudaMemsetAsync(work + res_o, 0, work_b - res_o, st));  // headers (zero_count is atomically added), peaks, tickets
   const unsigned spread = ctx->inc_spread;
   const size_t smem = incoherent_smem_bytes(spread);
-  if (smem > 48 * 1024) {
-    const void* key = reinterpret_cast<const void*>(incoherent_dedisperse_kernel);
-    if (!ctx->configured.count(key)) {  // once, for the largest spread any group may have
-      CK(cudaFuncSetAttribute(incoherent_dedisperse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                              (int)incoherent_smem_bytes(INC_SPREAD_MAX)));
-      ctx->configured.insert(key);
-    }
-  }
+  if (smem > 48 * 1024)  // once, for the largest spread any group may have
+    if (int rc = set_smem_max(ctx, incoherent_dedisperse_kernel, incoherent_smem_bytes(INC_SPREAD_MAX))) return rc;
   const dim3 grid((unsigned)n_groups, (unsigned)((T + INC_TILE - 1) / INC_TILE));
-  incoherent_dedisperse_kernel<<<grid, INC_THREADS, smem, st>>>(
-      static_cast<const float2*>(d_spectrum), time_count, chan_count, T, n_dm, reinterpret_cast<const int*>(tab),
-      reinterpret_cast<const int2*>(tab + gspan_o), reinterpret_cast<const int2*>(tab + groups_o),
-      reinterpret_cast<const int*>(tab + off_b), INC_TILE + spread, d_series, series_stride);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, incoherent_dedisperse_kernel, grid, INC_THREADS, smem, static_cast<const float2*>(d_spectrum),
+            time_count, chan_count, T, n_dm, reinterpret_cast<const int*>(tab),
+            reinterpret_cast<const int2*>(tab + gspan_o), reinterpret_cast<const int2*>(tab + groups_o),
+            reinterpret_cast<const int*>(tab + off_b), INC_TILE + spread, d_series, series_stride));
   // the series are already in place: no partial sums (partial == nullptr); one CTA per trial zero-counts and scans
-  colsum_final_scan_kernel<<<dim3(1, (unsigned)n_dm), 1024, 0, st>>>(
-      nullptr, T, 0, d_series, d_acc, static_cast<const float2*>(d_spectrum), time_count, chan_count, channel_threshold,
-      max_boxcar_length, d_ticket, d_res, series_stride, T, nullptr);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  detect_boxcar_kernel<true><<<dim3(max_nb, (unsigned)n_dm), 1024, 0, st>>>(
-      d_series, T, d_acc, T, snr, d_res, nullptr, d_peak, series_stride, T);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, colsum_final_scan_kernel, dim3(1, (unsigned)n_dm), 1024, 0, nullptr, T, 0, d_series, d_acc,
+            static_cast<const float2*>(d_spectrum), time_count, chan_count, channel_threshold, max_boxcar_length,
+            d_ticket, d_res, series_stride, T, nullptr));
+  CK(launch(ctx, false, detect_boxcar_kernel<true>, dim3(max_nb, (unsigned)n_dm), 1024, 0, d_series, T, d_acc, T, snr,
+            d_res, nullptr, d_peak, series_stride, T));
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
   static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
   std::vector<srtb_b200_peak> own_peaks(h_peaks ? 0 : n_dm);
@@ -2685,6 +2614,69 @@ extern "C" int srtb_b200_fold_phase(double period, double period_derivative, dou
   return 0;
 }
 
+// srtb_b200_fold and srtb_b200_fold_coherence past their own pointer checks: the checks both make (messages prefixed
+// `who`), then the bin plan, `kern` (its leading arguments `in`), the rows' sum and the copies back. kern's CTAs take G
+// channels of one of S streams by R tile ranges, up to one wave of per_sm CTAs per SM; a subband has P output rows (the
+// streams, or the four coherence products), and the first S nsub kept counts are copied back.
+template <class... KArgs, class... In>
+static int fold_run(srtb_b200_ctx* ctx, const char* who, size_t time_count, size_t chan_count, size_t fold_count,
+                    double phi0, double a, double b, size_t nbin, size_t nsub, double* h_out, uint64_t* h_hits,
+                    uint32_t* h_kept, size_t P, size_t S, size_t per_sm, void (*kern)(KArgs...), int threads,
+                    size_t (*smem_bytes)(int), In... in) {
+  const std::string pre = std::string(who) + ": ";
+  if (fold_count == 0 || fold_count > time_count)
+    return fail(ctx, SRTB_B200_E_SIZE, pre + "fold_count must be 1 to time_count");
+  if (nbin < 1 || nbin > (size_t)FOLD_MAX_BINS) return fail(ctx, SRTB_B200_E_SIZE, pre + "nbin must be 1 to 4096");
+  if (nsub == 0 || chan_count % nsub) return fail(ctx, SRTB_B200_E_SIZE, pre + "nsub must divide chan_count");
+  if (chan_count > ((size_t)1 << 24) || fold_count > ((size_t)1 << 40))
+    return fail(ctx, SRTB_B200_E_SIZE, pre + "chan_count above 2^24 or fold_count above 2^40");
+  if (!std::isfinite(phi0) || !std::isfinite(a) || !std::isfinite(b))
+    return fail(ctx, SRTB_B200_E_INVALID, pre + "a phase coefficient is not finite");
+  CK(cudaSetDevice(ctx->device));
+  const size_t C = chan_count, csub = C / nsub;
+  size_t G = std::min<size_t>(csub, FOLD_MAX_GROUP);
+  while (csub % G) G--;  // channels per CTA: the largest divisor of the subband width up to FOLD_MAX_GROUP
+  const size_t ntiles = (fold_count + FOLD_TILE - 1) / FOLD_TILE, ctas = S * (C / G);
+  // tile ranges per channel group: up to one wave of the CTAs an SM holds (nsub = 1 then still spreads over the SMs)
+  const size_t target = (size_t)ctx->sm_count * per_sm;
+  const size_t R = std::max<size_t>(1, std::min<size_t>(ntiles, target / ctas));
+  const size_t gps = csub / G, rows_per_output = gps * R, outputs = P * nsub * nbin;
+  // scratch: plan u32 [ntiles][FOLD_TILE], hits u64 [nbin], profile f64 [P][nsub][nbin], kept u32 [P][nsub] (for the
+  // coherence products the same count four times: fold_finish_kernel's layout); with more than one CTA row per output
+  // also rows f64 [P (C / G) R nbin] and kept rows u32 [P (C / G)]
+  const auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
+  const size_t hits_o = up(ntiles * FOLD_TILE * sizeof(uint32_t));
+  const size_t prof_o = hits_o + up(nbin * sizeof(uint64_t));
+  const size_t kept_o = prof_o + up(outputs * sizeof(double));
+  const size_t rows_o = kept_o + up(P * nsub * sizeof(uint32_t));
+  const bool finish = rows_per_output > 1;
+  const size_t krow_o = rows_o + (finish ? up(P * (C / G) * R * nbin * sizeof(double)) : 0);
+  const size_t work_b = krow_o + (finish ? P * (C / G) * sizeof(uint32_t) : 0);
+  if (int rc = grow(ctx, ctx->fold_work, work_b)) return rc;
+  char* w = ctx->fold_work.p;
+  uint32_t* d_plan = reinterpret_cast<uint32_t*>(w);
+  unsigned long long* d_hits = reinterpret_cast<unsigned long long*>(w + hits_o);
+  double* d_prof = reinterpret_cast<double*>(w + prof_o);
+  unsigned* d_kept = reinterpret_cast<unsigned*>(w + kept_o);
+  double* d_rows = finish ? reinterpret_cast<double*>(w + rows_o) : d_prof;
+  unsigned* d_krows = finish ? reinterpret_cast<unsigned*>(w + krow_o) : d_kept;
+  cudaStream_t st = ctx->lane.stream;
+  if (int rc = set_smem_max(ctx, kern, smem_bytes(FOLD_MAX_BINS))) return rc;
+  CK(cudaMemsetAsync(d_hits, 0, nbin * sizeof(uint64_t), st));
+  CK(launch(ctx, false, fold_plan_kernel, (unsigned)ntiles, FOLD_PLAN_THREADS, 0, phi0, a, b, (int)nbin,
+            (long long)fold_count, d_plan, d_hits));
+  CK(launch(ctx, false, kern, dim3((unsigned)ctas, (unsigned)R), threads, smem_bytes((int)nbin), in..., time_count,
+            (int)C, (int)G, (int)nbin, (long long)fold_count, (int)ntiles, d_plan, d_rows, d_krows));
+  if (finish)
+    CK(launch(ctx, false, fold_finish_kernel, (unsigned)((outputs + 255) / 256), 256, 0, d_rows, d_krows,
+              (int)rows_per_output, (int)gps, (int)nbin, outputs, d_prof, d_kept));
+  CK(cudaMemcpyAsync(h_out, d_prof, outputs * sizeof(double), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_hits, d_hits, nbin * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_kept, d_kept, S * nsub * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
+}
+
 extern "C" int srtb_b200_fold(srtb_b200_ctx* ctx, const void* const* d_spectra, int streams, size_t time_count,
                               size_t chan_count, size_t fold_count, double phi0, double a, double b, size_t nbin,
                               size_t nsub, double* h_profile, uint64_t* h_hits, uint32_t* h_kept) {
@@ -2699,72 +2691,13 @@ extern "C" int srtb_b200_fold(srtb_b200_ctx* ctx, const void* const* d_spectra, 
       return fail(ctx, SRTB_B200_E_INVALID, "fold: spectrum " + std::to_string(s) + " is not 8-byte aligned");
     sp.x[s] = static_cast<const float2*>(d_spectra[s]);
   }
-  if (fold_count == 0 || fold_count > time_count)
-    return fail(ctx, SRTB_B200_E_SIZE, "fold: fold_count must be 1 to time_count");
-  if (nbin < 1 || nbin > (size_t)FOLD_MAX_BINS) return fail(ctx, SRTB_B200_E_SIZE, "fold: nbin must be 1 to 4096");
-  if (nsub == 0 || chan_count % nsub) return fail(ctx, SRTB_B200_E_SIZE, "fold: nsub must divide chan_count");
-  if (chan_count > ((size_t)1 << 24) || fold_count > ((size_t)1 << 40))
-    return fail(ctx, SRTB_B200_E_SIZE, "fold: chan_count above 2^24 or fold_count above 2^40");
-  if (!std::isfinite(phi0) || !std::isfinite(a) || !std::isfinite(b))
-    return fail(ctx, SRTB_B200_E_INVALID, "fold: a phase coefficient is not finite");
-  CK(cudaSetDevice(ctx->device));
-  const size_t C = chan_count, S = (size_t)streams, csub = C / nsub;
-  size_t G = std::min<size_t>(csub, FOLD_MAX_GROUP);
-  while (csub % G) G--;  // channels per CTA: the largest divisor of the subband width up to FOLD_MAX_GROUP
-  const size_t ntiles = (fold_count + FOLD_TILE - 1) / FOLD_TILE, ctas = S * (C / G);
-  // tile ranges per channel group: up to one wave of four CTAs per SM (nsub = 1 then still spreads over the SMs)
-  const size_t target = (size_t)ctx->sm_count * 4;
-  const size_t R = std::max<size_t>(1, std::min<size_t>(ntiles, target / ctas));
-  const size_t gps = csub / G, rows_per_output = gps * R, outputs = S * nsub * nbin;
-  // scratch: plan u32 [ntiles][FOLD_TILE], hits u64 [nbin], profile f64 [outputs], kept u32 [S nsub]; with more than
-  // one CTA row per output also rows f64 [ctas R nbin] and kept rows u32 [ctas]
-  const auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t hits_o = up(ntiles * FOLD_TILE * sizeof(uint32_t));
-  const size_t prof_o = hits_o + up(nbin * sizeof(uint64_t));
-  const size_t kept_o = prof_o + up(outputs * sizeof(double));
-  const size_t rows_o = kept_o + up(S * nsub * sizeof(uint32_t));
-  const bool finish = rows_per_output > 1;
-  const size_t krow_o = rows_o + (finish ? up(ctas * R * nbin * sizeof(double)) : 0);
-  const size_t work_b = krow_o + (finish ? ctas * sizeof(uint32_t) : 0);
-  if (int rc = grow(ctx, ctx->fold_work, work_b)) return rc;
-  char* w = ctx->fold_work.p;
-  uint32_t* d_plan = reinterpret_cast<uint32_t*>(w);
-  unsigned long long* d_hits = reinterpret_cast<unsigned long long*>(w + hits_o);
-  double* d_prof = reinterpret_cast<double*>(w + prof_o);
-  unsigned* d_kept = reinterpret_cast<unsigned*>(w + kept_o);
-  double* d_rows = finish ? reinterpret_cast<double*>(w + rows_o) : d_prof;
-  unsigned* d_krows = finish ? reinterpret_cast<unsigned*>(w + krow_o) : d_kept;
-  cudaStream_t st = ctx->lane.stream;
-  const void* key = reinterpret_cast<const void*>(fold_kernel);
-  if (!ctx->configured.count(key)) {
-    CK(cudaFuncSetAttribute(fold_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)fold_smem_bytes(FOLD_MAX_BINS)));
-    ctx->configured.insert(key);
-  }
-  CK(cudaMemsetAsync(d_hits, 0, nbin * sizeof(uint64_t), st));
-  fold_plan_kernel<<<(unsigned)ntiles, FOLD_PLAN_THREADS, 0, st>>>(phi0, a, b, (int)nbin, (long long)fold_count,
-                                                                    d_plan, d_hits);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  fold_kernel<<<dim3((unsigned)ctas, (unsigned)R), FOLD_THREADS, fold_smem_bytes((int)nbin), st>>>(
-      sp, time_count, (int)C, (int)G, (int)nbin, (long long)fold_count, (int)ntiles, d_plan, d_rows, d_krows);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  if (finish) {
-    fold_finish_kernel<<<(unsigned)((outputs + 255) / 256), 256, 0, st>>>(d_rows, d_krows, (int)rows_per_output,
-                                                                          (int)gps, (int)nbin, outputs, d_prof, d_kept);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
-  CK(cudaMemcpyAsync(h_profile, d_prof, outputs * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(h_hits, d_hits, nbin * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(h_kept, d_kept, S * nsub * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  // four CTAs per SM (fold_kernel's launch bounds)
+  return fold_run(ctx, "fold", time_count, chan_count, fold_count, phi0, a, b, nbin, nsub, h_profile, h_hits, h_kept,
+                  streams, streams, 4, fold_kernel, FOLD_THREADS, fold_smem_bytes, sp);
 }
 
-// the coherence products of a stream pair: srtb_b200_fold's plan and finish around fold_coherence_kernel, whose CTA
-// rows stand for four streams (AA, BB, CR, CI)
+// the coherence products of a stream pair: srtb_b200_fold's plan and finish around fold_coherence_kernel, whose CTAs
+// read both streams and whose CTA rows stand for four streams (AA, BB, CR, CI)
 extern "C" int srtb_b200_fold_coherence(srtb_b200_ctx* ctx, const void* d_x, const void* d_y, size_t time_count,
                                         size_t chan_count, size_t fold_count, double phi0, double a, double b,
                                         size_t nbin, size_t nsub, double* h_coherence, uint64_t* h_hits,
@@ -2775,72 +2708,10 @@ extern "C" int srtb_b200_fold_coherence(srtb_b200_ctx* ctx, const void* d_x, con
   if (!aligned8(d_x) || !aligned8(d_y))
     return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: a spectrum is not 8-byte aligned");
   if (d_x == d_y) return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: d_x and d_y are the same spectrum");
-  if (fold_count == 0 || fold_count > time_count)
-    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: fold_count must be 1 to time_count");
-  if (nbin < 1 || nbin > (size_t)FOLD_MAX_BINS)
-    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: nbin must be 1 to 4096");
-  if (nsub == 0 || chan_count % nsub)
-    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: nsub must divide chan_count");
-  if (chan_count > ((size_t)1 << 24) || fold_count > ((size_t)1 << 40))
-    return fail(ctx, SRTB_B200_E_SIZE, "fold_coherence: chan_count above 2^24 or fold_count above 2^40");
-  if (!std::isfinite(phi0) || !std::isfinite(a) || !std::isfinite(b))
-    return fail(ctx, SRTB_B200_E_INVALID, "fold_coherence: a phase coefficient is not finite");
-  CK(cudaSetDevice(ctx->device));
-  const size_t C = chan_count, P = 4, csub = C / nsub;
-  size_t G = std::min<size_t>(csub, FOLD_MAX_GROUP);
-  while (csub % G) G--;  // channels per CTA, as srtb_b200_fold
-  const size_t ntiles = (fold_count + FOLD_TILE - 1) / FOLD_TILE, ctas = C / G;
-  // tile ranges per channel group: up to one wave of two CTAs per SM (the shared memory of nbin <= 1024 allows two)
-  const size_t target = (size_t)ctx->sm_count * 2;
-  const size_t R = std::max<size_t>(1, std::min<size_t>(ntiles, target / ctas));
-  const size_t gps = csub / G, rows_per_output = gps * R, outputs = P * nsub * nbin;
-  // scratch: plan u32 [ntiles][FOLD_TILE], hits u64 [nbin], coherence f64 [4][nsub][nbin], kept u32 [4][nsub] (the
-  // same count four times: fold_finish_kernel's layout); with more than one CTA row per output also rows
-  // f64 [4 ctas R nbin] and kept rows u32 [4 ctas]
-  const auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t hits_o = up(ntiles * FOLD_TILE * sizeof(uint32_t));
-  const size_t prof_o = hits_o + up(nbin * sizeof(uint64_t));
-  const size_t kept_o = prof_o + up(outputs * sizeof(double));
-  const size_t rows_o = kept_o + up(P * nsub * sizeof(uint32_t));
-  const bool finish = rows_per_output > 1;
-  const size_t krow_o = rows_o + (finish ? up(P * ctas * R * nbin * sizeof(double)) : 0);
-  const size_t work_b = krow_o + (finish ? P * ctas * sizeof(uint32_t) : 0);
-  if (int rc = grow(ctx, ctx->fold_work, work_b)) return rc;
-  char* w = ctx->fold_work.p;
-  uint32_t* d_plan = reinterpret_cast<uint32_t*>(w);
-  unsigned long long* d_hits = reinterpret_cast<unsigned long long*>(w + hits_o);
-  double* d_prof = reinterpret_cast<double*>(w + prof_o);
-  unsigned* d_kept = reinterpret_cast<unsigned*>(w + kept_o);
-  double* d_rows = finish ? reinterpret_cast<double*>(w + rows_o) : d_prof;
-  unsigned* d_krows = finish ? reinterpret_cast<unsigned*>(w + krow_o) : d_kept;
-  cudaStream_t st = ctx->lane.stream;
-  const void* key = reinterpret_cast<const void*>(fold_coherence_kernel);
-  if (!ctx->configured.count(key)) {
-    CK(cudaFuncSetAttribute(fold_coherence_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                            (int)fold_coherence_smem_bytes(FOLD_MAX_BINS)));
-    ctx->configured.insert(key);
-  }
-  CK(cudaMemsetAsync(d_hits, 0, nbin * sizeof(uint64_t), st));
-  fold_plan_kernel<<<(unsigned)ntiles, FOLD_PLAN_THREADS, 0, st>>>(phi0, a, b, (int)nbin, (long long)fold_count,
-                                                                    d_plan, d_hits);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  fold_coherence_kernel<<<dim3((unsigned)ctas, (unsigned)R), FOLD_COH_THREADS, fold_coherence_smem_bytes((int)nbin),
-                          st>>>(static_cast<const float2*>(d_x), static_cast<const float2*>(d_y), time_count, (int)C,
-                                (int)G, (int)nbin, (long long)fold_count, (int)ntiles, d_plan, d_rows, d_krows);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  if (finish) {
-    fold_finish_kernel<<<(unsigned)((outputs + 255) / 256), 256, 0, st>>>(d_rows, d_krows, (int)rows_per_output,
-                                                                          (int)gps, (int)nbin, outputs, d_prof, d_kept);
-    ctx->launches++;
-    CK(cudaGetLastError());
-  }
-  CK(cudaMemcpyAsync(h_coherence, d_prof, outputs * sizeof(double), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(h_hits, d_hits, nbin * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
-  CK(cudaMemcpyAsync(h_kept, d_kept, nsub * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
-  CK(cudaStreamSynchronize(st));
-  return 0;
+  // two CTAs per SM (the shared memory of nbin <= 1024 allows two); the four products share one kept count
+  return fold_run(ctx, "fold_coherence", time_count, chan_count, fold_count, phi0, a, b, nbin, nsub, h_coherence,
+                  h_hits, h_kept, 4, 1, 2, fold_coherence_kernel, FOLD_COH_THREADS, fold_coherence_smem_bytes,
+                  static_cast<const float2*>(d_x), static_cast<const float2*>(d_y));
 }
 
 // tickets wrap at a multiple of the slot count, so ticket % SRTB_B200_RING_SLOTS is always the slot that was used
@@ -3006,22 +2877,13 @@ extern "C" int srtb_b200_simplify_spectrum(srtb_b200_ctx* ctx, const void* d_spe
 
   const float2* spec = static_cast<const float2*>(d_spectrum);
   const dim3 row_grid((unsigned)in_height, (unsigned)tiles);
-  if (in_width % 2 == 0 && (reinterpret_cast<uintptr_t>(d_spectrum) & 15u) == 0)
-    thumb_row_kernel<true><<<row_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(spec, in_width, out_width, G,
-                                                                           ctx->thumb_rows.p);
-  else
-    thumb_row_kernel<false><<<row_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(spec, in_width, out_width, G,
-                                                                            ctx->thumb_rows.p);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  thumb_col_kernel<<<col_grid, THUMB_THREADS, 0, ctx->lane.stream>>>(ctx->thumb_rows.p, in_height, out_width, out_height,
-                                                                     d_intensity, ctx->thumb_partial.p);
-  ctx->launches++;
-  CK(cudaGetLastError());
-  thumb_norm_kernel<<<grid_for(ctx, n, THUMB_THREADS, 4), THUMB_THREADS, 0, ctx->lane.stream>>>(
-      d_intensity, n, ctx->thumb_partial.p, (int)col_grid, argb_0, argb_1, argb_overflow, d_pixmap, d_average);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  const bool vec = in_width % 2 == 0 && (reinterpret_cast<uintptr_t>(d_spectrum) & 15u) == 0;
+  CK(launch(ctx, false, vec ? thumb_row_kernel<true> : thumb_row_kernel<false>, row_grid, THUMB_THREADS, 0, spec,
+            in_width, out_width, G, ctx->thumb_rows.p));
+  CK(launch(ctx, false, thumb_col_kernel, col_grid, THUMB_THREADS, 0, ctx->thumb_rows.p, in_height, out_width, out_height,
+            d_intensity, ctx->thumb_partial.p));
+  CK(launch(ctx, false, thumb_norm_kernel, grid_for(ctx, n, THUMB_THREADS, 4), THUMB_THREADS, 0, d_intensity, n,
+            ctx->thumb_partial.p, (int)col_grid, argb_0, argb_1, argb_overflow, d_pixmap, d_average));
   return 0;
 }
 
@@ -3032,23 +2894,16 @@ static int launch_cross_spectrum(srtb_b200_ctx* ctx, const float2* a, const floa
                                  float2* out) {
   const bool vec = ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) |
                      reinterpret_cast<uintptr_t>(out)) & 15u) == 0;
-  if (vec)
-    cross_spectrum_kernel<true><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(a, b, M, norm, out);
-  else
-    cross_spectrum_kernel<false><<<grid_for(ctx, M, 256), 256, 0, ctx->lane.stream>>>(a, b, M, norm, out);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, vec ? cross_spectrum_kernel<true> : cross_spectrum_kernel<false>,
+            grid_for(ctx, vec ? M / 2 + 1 : M, 256), 256, 0, a, b, M, norm, out));
   return 0;
 }
 
 // out[i] = |y[i]| for i < M; two bins per access when out is 8-byte aligned (y is a ctx buffer, 16-byte aligned)
 static int launch_magnitude(srtb_b200_ctx* ctx, const float2* y, size_t M, float* out) {
-  if ((reinterpret_cast<uintptr_t>(out) & 7u) == 0)
-    magnitude_kernel<true><<<grid_for(ctx, M / 2 + 1, 256), 256, 0, ctx->lane.stream>>>(y, M, out);
-  else
-    magnitude_kernel<false><<<grid_for(ctx, M, 256), 256, 0, ctx->lane.stream>>>(y, M, out);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  const bool vec = (reinterpret_cast<uintptr_t>(out) & 7u) == 0;
+  CK(launch(ctx, false, vec ? magnitude_kernel<true> : magnitude_kernel<false>, grid_for(ctx, vec ? M / 2 + 1 : M, 256),
+            256, 0, y, M, out));
   return 0;
 }
 
@@ -3131,14 +2986,8 @@ static int launch_corr_pack(srtb_b200_ctx* ctx, const void* in_1, const void* in
   const uintptr_t group = BITS < 0 ? -BITS : BITS;  // bytes of 8 samples: unpack_src<BITS>'s load width
   const bool vec = reinterpret_cast<uintptr_t>(in_1) % group == 0 && reinterpret_cast<uintptr_t>(in_2) % group == 0;
   const size_t pairs = (2 * rows) << log_ls;
-  if (vec)
-    corr_pack_kernel<BITS, true><<<grid_for(ctx, pairs / 8, 256), 256, 0, ctx->lane.stream>>>(in_1, in_2, log_ls,
-                                                                                               n_segments, rows, out);
-  else
-    corr_pack_kernel<BITS, false><<<grid_for(ctx, pairs, 256), 256, 0, ctx->lane.stream>>>(in_1, in_2, log_ls,
-                                                                                           n_segments, rows, out);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, vec ? corr_pack_kernel<BITS, true> : corr_pack_kernel<BITS, false>,
+            grid_for(ctx, vec ? pairs / 8 : pairs, 256), 256, 0, in_1, in_2, log_ls, n_segments, rows, out));
   return 0;
 }
 
@@ -3188,11 +3037,8 @@ extern "C" int srtb_b200_correlate_accumulate(srtb_b200_ctx* ctx, const void* d_
     if (int rc2 = grow(ctx, ctx->corr_partial, groups * Ms * sizeof(double2))) return rc2;
     partial = ctx->corr_partial.p;
   }
-  corr_split_accumulate_kernel<<<dim3((unsigned)tiles, (unsigned)groups), 256, 0, ctx->lane.stream>>>(
-      z, log_ls, log_bt, rows, n_segments, rows_per_group, partial, ctx->corr_tickets, static_cast<double2*>(d_acc),
-      reset);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, corr_split_accumulate_kernel, dim3((unsigned)tiles, (unsigned)groups), 256, 0, z, log_ls, log_bt,
+            rows, n_segments, rows_per_group, partial, ctx->corr_tickets, static_cast<double2*>(d_acc), reset));
   return 0;
 }
 
@@ -3213,10 +3059,8 @@ extern "C" int srtb_b200_correlate_finish(srtb_b200_ctx* ctx, const void* d_acc,
   const float norm = static_cast<float>(std::pow(static_cast<double>(segment_size), -1.5));
   const double scale = static_cast<double>(norm) / static_cast<double>(total_segments);
   float2* y = ctx->corr_rows.p;
-  corr_scale_kernel<<<grid_for(ctx, Ms, 256), 256, 0, ctx->lane.stream>>>(static_cast<const double2*>(d_acc), Ms,
-                                                                           scale, y);
-  ctx->launches++;
-  CK(cudaGetLastError());
+  CK(launch(ctx, false, corr_scale_kernel, grid_for(ctx, Ms, 256), 256, 0, static_cast<const double2*>(d_acc), Ms, scale,
+            y));
   if (int rc = fft_c2c_impl<false>(ctx, y, Ms, 1)) return rc;
   return launch_magnitude(ctx, y, Ms, d_out);
 }
