@@ -333,6 +333,16 @@ const void* srtb_b200_sweep_spectrum(const srtb_b200_ctx* ctx);
  * chan_count, a null h_dms or n_dm == 0 returns SRTB_B200_E_INVALID; a shift that is not finite SRTB_B200_E_INVALID. */
 int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, float bandwidth, float sample_rate, float dm,
                                 const float* h_dms, size_t n_dm, int64_t* shifts, uint64_t* s_plus, uint64_t* s_minus);
+/* The trial groups the search launches with (host only; for tests and tools): the trials stably sorted by DM, then cut
+ * greedily into groups of at most 64 trials whose shift spread (max s - min s over the group's trials) is at most 1792
+ * on every channel; a trial that would break either limit starts the next group. Writes the group count to *n_groups
+ * and, each when not NULL: order [n_dm] (the trial of each sorted slot), groups [n_groups][2] (first sorted slot, trial
+ * count), gspan [n_groups][chan_count][2] (min, max of s + S- over the group) and *spread (the largest max - min of any
+ * group and channel). groups and gspan need room for n_dm groups. Refusals as srtb_b200_incoherent_shifts, and a NULL
+ * n_groups returns SRTB_B200_E_INVALID. */
+int srtb_b200_incoherent_groups(size_t chan_count, float freq_low, float bandwidth, float sample_rate, float dm,
+                                const float* h_dms, size_t n_dm, int32_t* order, int32_t* groups, int32_t* gspan,
+                                uint64_t* n_groups, uint32_t* spread);
 /* The search. With ts = time_count - time_reserved_count and T = ts - S+ - S-, trial d's series is
  *   v_d[j] = sum_c |x[c][j + S- + s[d][c]]|^2, j < T (fp32, channels added in index order: two calls agree bit for bit),
  * so every trial has the same length and time origin. Each v_d goes through signal_detect_pipe_2's detector as the block
@@ -345,7 +355,8 @@ int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, float bandwid
  * returns, and once more when h_series is given and the best trial has a positive boxcar.
  * Before any launch: a null ctx, d_spectrum, h_dms or h_results, n_dm == 0, a zero size or an 8-byte misaligned spectrum
  * returns SRTB_B200_E_INVALID; time_reserved_count >= time_count, T < 2, n_dm > SRTB_B200_INCOHERENT_MAX_DMS or
- * time_count > 2^30 returns SRTB_B200_E_SIZE.
+ * time_count > 2^30 returns SRTB_B200_E_SIZE. Any T up to that limit runs (the dedispersion kernel's CTAs take
+ * several time tiles each past 65535 tiles of 256).
  * Scratch the ctx grows on demand and keeps: at most n_dm (12 C + 132 T + 1448) bytes of device memory (shift tables,
  * the series of every boxcar, the scans, headers and peaks), and the shift tables on the host. */
 #define SRTB_B200_INCOHERENT_MAX_DMS 4096

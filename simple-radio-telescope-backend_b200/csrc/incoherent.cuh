@@ -50,7 +50,8 @@ __device__ __forceinline__ void cp_async_wait2() { asm volatile("cp.async.wait_g
 // x: [C][L] complex64, 8-byte aligned. off: [C][n_dm] absolute offsets s + S- (>= 0) of each trial, the trials in
 // sorted order; gspan: [groups][C] (min, max) of off over the group's trials; groups: [groups] (first sorted slot,
 // trial count); order: [n_dm] trial index of each sorted slot. span_max = INC_TILE + the largest spread.
-// out: trial d's series [T] at out + d * out_stride. Grid: (groups, ceil(T / INC_TILE)).
+// out: trial d's series [T] at out + d * out_stride. Grid: (groups, min(tiles, 65535)) with tiles = ceil(T / INC_TILE);
+// CTA y forms tiles y, y + gridDim.y, ... in turn, so T may exceed 65535 tiles (gridDim.y's limit, T just above 2^24).
 __global__ void __launch_bounds__(INC_THREADS) incoherent_dedisperse_kernel(
     const float2* __restrict__ x, size_t L, size_t C, size_t T, size_t n_dm, const int* __restrict__ off,
     const int2* __restrict__ gspan, const int2* __restrict__ groups, const int* __restrict__ order, unsigned span_max,
@@ -61,75 +62,80 @@ __global__ void __launch_bounds__(INC_THREADS) incoherent_dedisperse_kernel(
   int* s_off = reinterpret_cast<int*>(pw + span_max);                        // [INC_STAGES][INC_GROUP]
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const size_t g = blockIdx.x;
-  const size_t t0 = (size_t)blockIdx.y * INC_TILE;
   const int2 gi = groups[g];
   const int cnt = gi.y;
   const int* goff = off + gi.x;
   const int2* gsp = gspan + g * C;
+  const size_t tiles = (T + INC_TILE - 1) / INC_TILE;
 
-  // channel c's span -> raw[c % 3], its slot offsets -> s_off[c % 3]; one commit group per channel
-  auto stage = [&](size_t c) {
-    const int2 mm = gsp[c];
-    const size_t span = INC_TILE + (size_t)(mm.y - mm.x);
-    const float2* row = x + c * L;
-    const size_t src0 = t0 + (size_t)mm.x;
-    float2* dst = raw + (c % INC_STAGES) * (size_t)span_max;
-    for (size_t e = tid; e < span; e += INC_THREADS) {
-      const bool valid = src0 + e < L;
-      cp_async8(dst + e, valid ? row + src0 + e : row, valid);
-    }
-    if (tid < cnt) cp_async4(s_off + (c % INC_STAGES) * INC_GROUP + tid, goff + c * n_dm + tid);
-    cp_async_commit();
-  };
+  for (size_t tile = blockIdx.y; tile < tiles; tile += gridDim.y) {  // CTA-uniform
+    const size_t t0 = tile * INC_TILE;
 
-  float acc[4][8];
-#pragma unroll
-  for (int i = 0; i < 4; i++)
-#pragma unroll
-    for (int r = 0; r < 8; r++) acc[i][r] = 0.f;
+    // channel c's span -> raw[c % 3], its slot offsets -> s_off[c % 3]; one commit group per channel. The previous
+    // tile read raw and s_off only before its last channel's second barrier, so restaging them here is safe
+    auto stage = [&](size_t c) {
+      const int2 mm = gsp[c];
+      const size_t span = INC_TILE + (size_t)(mm.y - mm.x);
+      const float2* row = x + c * L;
+      const size_t src0 = t0 + (size_t)mm.x;
+      float2* dst = raw + (c % INC_STAGES) * (size_t)span_max;
+      for (size_t e = tid; e < span; e += INC_THREADS) {
+        const bool valid = src0 + e < L;
+        cp_async8(dst + e, valid ? row + src0 + e : row, valid);
+      }
+      if (tid < cnt) cp_async4(s_off + (c % INC_STAGES) * INC_GROUP + tid, goff + c * n_dm + tid);
+      cp_async_commit();
+    };
 
-  stage(0);
-  if (C > 1) stage(1);
-  else cp_async_commit();
-  for (size_t c = 0; c < C; c++) {
-    if (c + 2 < C) stage(c + 2);
-    else cp_async_commit();  // empty groups keep wait_group 2 meaning "channel c has landed"
-    cp_async_wait2();
-    __syncthreads();  // channel c visible to all; every warp is done with the previous channel's pw
-    const int2 mm = gsp[c];
-    const size_t span = INC_TILE + (size_t)(mm.y - mm.x);
-    const float2* src = raw + (c % INC_STAGES) * (size_t)span_max;
-    for (size_t e = tid; e < span; e += INC_THREADS) {
-      const float2 v = src[e];
-      pw[e] = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
-    }
-    // this channel's offsets are read before the barrier: the next iteration's stage() overwrites s_off[c % 3]
-    int rel[4];
+    float acc[4][8];
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int k = warp + 16 * i;
-      rel[i] = (k < cnt) ? s_off[(c % INC_STAGES) * INC_GROUP + k] - mm.x : 0;
-    }
-    __syncthreads();
+    for (int i = 0; i < 4; i++)
 #pragma unroll
-    for (int i = 0; i < 4; i++) {
-      const int k = warp + 16 * i;
-      if (k < cnt) {  // warp-uniform
-        const float* p = pw + rel[i] + lane;
+      for (int r = 0; r < 8; r++) acc[i][r] = 0.f;
+
+    stage(0);
+    if (C > 1) stage(1);
+    else cp_async_commit();
+    for (size_t c = 0; c < C; c++) {
+      if (c + 2 < C) stage(c + 2);
+      else cp_async_commit();  // empty groups keep wait_group 2 meaning "channel c has landed"
+      cp_async_wait2();
+      __syncthreads();  // channel c visible to all; every warp is done with the previous channel's (or tile's) pw
+      const int2 mm = gsp[c];
+      const size_t span = INC_TILE + (size_t)(mm.y - mm.x);
+      const float2* src = raw + (c % INC_STAGES) * (size_t)span_max;
+      for (size_t e = tid; e < span; e += INC_THREADS) {
+        const float2 v = src[e];
+        pw[e] = __fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y));
+      }
+      // this channel's offsets are read before the barrier: the next iteration's stage() overwrites s_off[c % 3]
+      int rel[4];
 #pragma unroll
-        for (int r = 0; r < 8; r++) acc[i][r] += p[32 * r];
+      for (int i = 0; i < 4; i++) {
+        const int k = warp + 16 * i;
+        rel[i] = (k < cnt) ? s_off[(c % INC_STAGES) * INC_GROUP + k] - mm.x : 0;
+      }
+      __syncthreads();
+#pragma unroll
+      for (int i = 0; i < 4; i++) {
+        const int k = warp + 16 * i;
+        if (k < cnt) {  // warp-uniform
+          const float* p = pw + rel[i] + lane;
+#pragma unroll
+          for (int r = 0; r < 8; r++) acc[i][r] += p[32 * r];
+        }
       }
     }
-  }
 #pragma unroll
-  for (int i = 0; i < 4; i++) {
-    const int k = warp + 16 * i;
-    if (k >= cnt) continue;
-    float* o = out + (size_t)order[gi.x + k] * out_stride;
+    for (int i = 0; i < 4; i++) {
+      const int k = warp + 16 * i;
+      if (k >= cnt) continue;
+      float* o = out + (size_t)order[gi.x + k] * out_stride;
 #pragma unroll
-    for (int r = 0; r < 8; r++) {
-      const size_t j = t0 + lane + 32 * r;
-      if (j < T) o[j] = acc[i][r];
+      for (int r = 0; r < 8; r++) {
+        const size_t j = t0 + lane + 32 * r;
+        if (j < T) o[j] = acc[i][r];
+      }
     }
   }
 }

@@ -2442,9 +2442,69 @@ extern "C" int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, fl
   return 0;
 }
 
-// the shift tables of (C, band, dm, trials), cached: the host table, and the kernel's sorted offsets and groups. The
-// trials are sorted by DM and cut greedily into groups of at most INC_GROUP whose spread over every channel is at most
-// INC_SPREAD_MAX (a single trial has none), so neighbouring trials share a group whatever order they came in.
+// the trials sorted by DM (stable) and cut greedily into groups of at most INC_GROUP whose spread over every channel is at
+// most INC_SPREAD_MAX (a single trial has none), so neighbouring trials share a group whatever order they came in.
+// sh: the shift table [n_dm][C]. order: trial of each sorted slot; groups: (first sorted slot, count); gspan:
+// [groups][C] (min, max) of s + S- over the group's trials; spread: the largest max - min of any group and channel.
+static void incoherent_grouping(const std::vector<int64_t>& sh, size_t C, const float* dms, size_t n_dm,
+                                int64_t s_minus, std::vector<int>* order, std::vector<int2>* groups,
+                                std::vector<int2>* gspan, unsigned* spread) {
+  order->resize(n_dm);
+  for (size_t d = 0; d < n_dm; d++) (*order)[d] = (int)d;
+  std::stable_sort(order->begin(), order->end(), [&](int a, int b) { return dms[a] < dms[b]; });
+  groups->clear();
+  gspan->clear();
+  *spread = 0;
+  std::vector<int64_t> gmin(C), gmax(C), nmin(C), nmax(C);
+  size_t first = 0;
+  while (first < n_dm) {
+    for (size_t c = 0; c < C; c++) gmin[c] = gmax[c] = sh[(size_t)(*order)[first] * C + c];
+    size_t count = 1;
+    while (first + count < n_dm && count < (size_t)INC_GROUP) {
+      const size_t d = (size_t)(*order)[first + count];
+      bool fits = true;
+      for (size_t c = 0; c < C && fits; c++) {
+        nmin[c] = std::min(gmin[c], sh[d * C + c]);
+        nmax[c] = std::max(gmax[c], sh[d * C + c]);
+        fits = nmax[c] - nmin[c] <= INC_SPREAD_MAX;
+      }
+      if (!fits) break;
+      gmin.swap(nmin);
+      gmax.swap(nmax);
+      count++;
+    }
+    groups->push_back(make_int2((int)first, (int)count));
+    for (size_t c = 0; c < C; c++) {
+      gspan->push_back(make_int2((int)(gmin[c] + s_minus), (int)(gmax[c] + s_minus)));
+      *spread = std::max(*spread, (unsigned)(gmax[c] - gmin[c]));
+    }
+    first += count;
+  }
+}
+
+extern "C" int srtb_b200_incoherent_groups(size_t chan_count, float freq_low, float bandwidth, float sample_rate,
+                                           float dm, const float* h_dms, size_t n_dm, int32_t* order, int32_t* groups,
+                                           int32_t* gspan, uint64_t* n_groups, uint32_t* spread) {
+  if (chan_count == 0 || !h_dms || n_dm == 0 || !n_groups)
+    return fail(nullptr, SRTB_B200_E_INVALID, "incoherent_groups: bad argument");
+  std::vector<int64_t> tab;
+  uint64_t sp = 0, sm = 0;
+  if (int rc = incoherent_shift_table(chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm, &tab, &sp, &sm))
+    return fail(nullptr, rc, "incoherent_groups: a shift is not finite or out of range");
+  std::vector<int> ord;
+  std::vector<int2> grp, gsp;
+  unsigned spr = 0;
+  incoherent_grouping(tab, chan_count, h_dms, n_dm, (int64_t)sm, &ord, &grp, &gsp, &spr);
+  *n_groups = grp.size();
+  if (order) std::memcpy(order, ord.data(), ord.size() * sizeof(int));
+  if (groups) std::memcpy(groups, grp.data(), grp.size() * sizeof(int2));
+  if (gspan) std::memcpy(gspan, gsp.data(), gsp.size() * sizeof(int2));
+  if (spread) *spread = spr;
+  return 0;
+}
+
+// the shift tables of (C, band, dm, trials), cached: the host table, and the kernel's sorted offsets and groups
+// (incoherent_grouping)
 static int incoherent_tables(srtb_b200_ctx* ctx, size_t C, float freq_low, float bandwidth, float sample_rate,
                              float dm, const float* dms, size_t n_dm) {
   std::vector<double> key = {(double)C, freq_low, bandwidth, sample_rate, dm};
@@ -2457,38 +2517,8 @@ static int incoherent_tables(srtb_b200_ctx* ctx, size_t C, float freq_low, float
     return fail(ctx, rc, "incoherent_dm_search: a shift is not finite or out of range");
   const std::vector<int64_t>& sh = ctx->inc_shifts;
   const int64_t s_minus = (int64_t)ctx->inc_s_minus;
-  std::vector<int>& order = ctx->inc_order;
-  order.resize(n_dm);
-  for (size_t d = 0; d < n_dm; d++) order[d] = (int)d;
-  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return dms[a] < dms[b]; });
-  ctx->inc_groups.clear();
-  ctx->inc_gspan.clear();
-  ctx->inc_spread = 0;
-  std::vector<int64_t> gmin(C), gmax(C), nmin(C), nmax(C);
-  size_t first = 0;
-  while (first < n_dm) {
-    for (size_t c = 0; c < C; c++) gmin[c] = gmax[c] = sh[(size_t)order[first] * C + c];
-    size_t count = 1;
-    while (first + count < n_dm && count < (size_t)INC_GROUP) {
-      const size_t d = (size_t)order[first + count];
-      bool fits = true;
-      for (size_t c = 0; c < C && fits; c++) {
-        nmin[c] = std::min(gmin[c], sh[d * C + c]);
-        nmax[c] = std::max(gmax[c], sh[d * C + c]);
-        fits = nmax[c] - nmin[c] <= INC_SPREAD_MAX;
-      }
-      if (!fits) break;
-      gmin.swap(nmin);
-      gmax.swap(nmax);
-      count++;
-    }
-    ctx->inc_groups.push_back(make_int2((int)first, (int)count));
-    for (size_t c = 0; c < C; c++) {
-      ctx->inc_gspan.push_back(make_int2((int)(gmin[c] + s_minus), (int)(gmax[c] + s_minus)));
-      ctx->inc_spread = std::max(ctx->inc_spread, (unsigned)(gmax[c] - gmin[c]));
-    }
-    first += count;
-  }
+  const std::vector<int>& order = ctx->inc_order;
+  incoherent_grouping(sh, C, dms, n_dm, s_minus, &ctx->inc_order, &ctx->inc_groups, &ctx->inc_gspan, &ctx->inc_spread);
   ctx->inc_off.resize(C * n_dm);
   for (size_t c = 0; c < C; c++)
     for (size_t i = 0; i < n_dm; i++) ctx->inc_off[c * n_dm + i] = (int)(sh[(size_t)order[i] * C + c] + s_minus);
@@ -2557,7 +2587,8 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   const size_t smem = incoherent_smem_bytes(spread);
   if (smem > 48 * 1024)  // once, for the largest spread any group may have
     if (int rc = set_smem_max(ctx, incoherent_dedisperse_kernel, incoherent_smem_bytes(INC_SPREAD_MAX))) return rc;
-  const dim3 grid((unsigned)n_groups, (unsigned)((T + INC_TILE - 1) / INC_TILE));
+  // gridDim.y is at most 65535: a longer series (T above 65535 INC_TILE, just over 2^24) has CTAs form several tiles
+  const dim3 grid((unsigned)n_groups, (unsigned)std::min<size_t>((T + INC_TILE - 1) / INC_TILE, 65535));
   CK(launch(ctx, false, incoherent_dedisperse_kernel, grid, INC_THREADS, smem, static_cast<const float2*>(d_spectrum),
             time_count, chan_count, T, n_dm, reinterpret_cast<const int*>(tab),
             reinterpret_cast<const int2*>(tab + gspan_o), reinterpret_cast<const int2*>(tab + groups_o),

@@ -144,6 +144,8 @@ SYMBOLS = {
     "srtb_b200_correlate_finish": (_I, [_P, _P, _SZ, C.c_uint64, _P]),
     "srtb_b200_incoherent_shifts": (_I, [_SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _P, C.POINTER(C.c_uint64),
                                          C.POINTER(C.c_uint64)]),
+    "srtb_b200_incoherent_groups": (_I, [_SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _P, _P, _P, C.POINTER(C.c_uint64),
+                                         C.POINTER(C.c_uint32)]),
     "srtb_b200_incoherent_dm_search": (_I, [_P, _P, _SZ, _SZ, _SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _F, _F, _SZ,
                                             C.POINTER(DetectResult), _P, _P, _P]),
     "srtb_b200_fold_phase": (_I, [C.c_double, C.c_double, C.c_double, C.c_uint64, C.c_uint64,
@@ -524,6 +526,25 @@ def incoherent_shifts(chan_count: int, freq_low: float, bandwidth: float, sample
     if rc < 0:
         raise SrtbError(rc, lib.srtb_b200_last_error(None).decode())
     return out, int(sp.value), int(sm.value)
+
+
+def incoherent_groups(chan_count: int, freq_low: float, bandwidth: float, sample_rate: float, dm: float, dms):
+    """the trial groups srtb_b200_incoherent_dm_search launches with: (order [n_dm], groups [n_groups][2] (first sorted
+    slot, count), gspan [n_groups][chan_count][2] (min, max of s + S-), spread), int numpy arrays and an int"""
+    import numpy as np
+    lib = load_library()
+    n_dm = len(dms)
+    arr = (C.c_float * n_dm)(*[float(d) for d in dms])
+    order = np.zeros(n_dm, np.int32)
+    groups = np.zeros((n_dm, 2), np.int32)
+    gspan = np.zeros((n_dm, chan_count, 2), np.int32)
+    ng, spread = C.c_uint64(), C.c_uint32()
+    rc = lib.srtb_b200_incoherent_groups(chan_count, freq_low, bandwidth, sample_rate, dm, arr, n_dm,
+                                         order.ctypes.data, groups.ctypes.data, gspan.ctypes.data, C.byref(ng),
+                                         C.byref(spread))
+    if rc < 0:
+        raise SrtbError(rc, lib.srtb_b200_last_error(None).decode())
+    return order, groups[:ng.value].copy(), gspan[:ng.value].copy(), int(spread.value)
 
 
 def fold_phase(period: float, period_derivative: float, sample_rate: float, samples_per_spectrum_sample: int,
