@@ -61,6 +61,9 @@ struct configs {
   // with fold_period: also fold the coherence products AA, BB, CR, CI of streams 0 and 1 (the two feeds of a
   // dual-polarisation format) over the channels kept in both; needs a two-stream format (not gznupsr_a1_4)
   bool fold_coherence = false;
+  // with dm_list or incoherent_dm_list: also list each block's single-pulse candidates, every above-threshold run of
+  // every trial and boxcar grouped friends-of-friends over DM, width and time (<prefix><counter>.<id>.candidates.csv)
+  bool dm_search_candidates = false;
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

@@ -98,6 +98,39 @@ inline std::vector<srtb::work::time_series_holder> positive_series(const srtb_b2
   return out;
 }
 
+/** the block's own share of candidate windows (series indices): min(step, valid_samples) / 2C, step = fold_block_step(),
+ *  or step / 2C for a block without a first_sample (UDP). Consecutive blocks start step samples apart, so a pulse in the
+ *  coherent sweep's overlap is listed by one block only; the incoherent search's series are step / 2C long, so it keeps
+ *  every candidate. A representative within a few samples of the boundary may be chosen differently by the two blocks */
+inline uint64_t candidate_share(const srtb::work::write_signal_work& w) {
+  const uint64_t two_c = 2 * (uint64_t)w.batch_size, step = fold_block_step();
+  if (two_c == 0) return 0;
+  return (w.first_sample != w.no_first_sample ? std::min(step, w.valid_samples) : step) / two_c;
+}
+
+/** dm_search_candidates: stream s's events (at most cap of the true total n_events) clustered into w's candidates; a
+ *  warning names both counts when the cap cut the list */
+inline void attach_candidates(srtb::work::write_signal_work& w, const srtb_b200_event* events, uint64_t n_events,
+                              size_t cap, const std::vector<srtb::real>& dms, uint64_t sample_offset) {
+  const size_t n = (size_t)std::min<uint64_t>(n_events, cap);
+  if (n_events > cap)
+    SRTB_LOGW << " [dm_search_candidates] " << "stream " << w.data_stream_id << ": " << n_events
+              << " events, only the first " << cap << " clustered";
+  std::vector<srtb_b200_candidate> c(std::max<size_t>(n, 1));
+  uint64_t n_c = 0;
+  if (srtb_b200_cluster_events(events, n, dms.data(), dms.size(), c.data(), c.size(), &n_c) != 0)
+    throw std::runtime_error(std::string{"[dm_search_candidates] "} + srtb_b200_last_error(nullptr));
+  w.has_candidates = true;
+  w.candidate_share = candidate_share(w);
+  w.candidate_sample_offset = sample_offset;
+  for (size_t i = 0; i < std::min<uint64_t>(n_c, c.size()); i++)
+    w.candidates.push_back({c[i].snr, c[i].dm, c[i].dm_low, c[i].dm_high, c[i].boxcar_length, c[i].peak_index,
+                            c[i].window, c[i].members, c[i].span_begin, c[i].span_end, c[i].trial});
+}
+
+/** events per stream and block a DM search lists for its candidates (dm_search_candidates) */
+constexpr size_t candidate_event_cap = (size_t)1 << 18;
+
 class baseband_chain_pipe {
  protected:
   srtb::cuda_queue q;
@@ -113,6 +146,7 @@ class baseband_chain_pipe {
     bool sum = false;                       // signal_detect_sum_streams: the sum's result follows the streams'
   };
   std::deque<pending_block> pending;  // blocks in the pinned-host ring of this queue's context
+  std::vector<srtb_b200_event> events;  // dm_search_candidates: one stream's events, reused
 
  public:
   /** ring_depth blocks are kept in flight through srtb_b200_submit_block_ex / collect_block_ex (block k's H2D
@@ -249,12 +283,26 @@ class baseband_chain_pipe {
     std::vector<srtb_b200_detect_result> tr(n_dm);
     std::vector<srtb_b200_peak> peaks(n_dm);
     int32_t best = 0;
-    q.check(srtb_b200_incoherent_dm_search(
-        q.ctx(), p.d_spectrum[s].get(), p.L, p.C, p.L - block_res.time_series_count, cfg.baseband_freq_low,
-        cfg.baseband_bandwidth, cfg.baseband_sample_rate, cfg.dm, dms.data(), n_dm,
-        cfg.signal_detect_signal_noise_threshold, cfg.signal_detect_channel_threshold,
-        cfg.signal_detect_max_boxcar_length, tr.data(), peaks.data(), &best,
-        h_inc.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L));
+    if (srtb::config.dm_search_candidates) {
+      events.resize(candidate_event_cap);
+      uint64_t n_events = 0, s_minus = 0;
+      q.check(srtb_b200_incoherent_dm_search_events(
+          q.ctx(), p.d_spectrum[s].get(), p.L, p.C, p.L - block_res.time_series_count, cfg.baseband_freq_low,
+          cfg.baseband_bandwidth, cfg.baseband_sample_rate, cfg.dm, dms.data(), n_dm,
+          cfg.signal_detect_signal_noise_threshold, cfg.signal_detect_channel_threshold,
+          cfg.signal_detect_max_boxcar_length, tr.data(), peaks.data(), &best,
+          h_inc.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L, events.data(), events.size(), &n_events));
+      q.check(srtb_b200_incoherent_shifts(p.C, cfg.baseband_freq_low, cfg.baseband_bandwidth, cfg.baseband_sample_rate,
+                                          cfg.dm, dms.data(), n_dm, nullptr, nullptr, &s_minus));
+      attach_candidates(w, events.data(), n_events, events.size(), dms, s_minus);
+    } else {
+      q.check(srtb_b200_incoherent_dm_search(
+          q.ctx(), p.d_spectrum[s].get(), p.L, p.C, p.L - block_res.time_series_count, cfg.baseband_freq_low,
+          cfg.baseband_bandwidth, cfg.baseband_sample_rate, cfg.dm, dms.data(), n_dm,
+          cfg.signal_detect_signal_noise_threshold, cfg.signal_detect_channel_threshold,
+          cfg.signal_detect_max_boxcar_length, tr.data(), peaks.data(), &best,
+          h_inc.get() + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L));
+    }
     const srtb_b200_detect_result& r = tr[best];
     w.time_series = positive_series(r, h_inc, s, p.L, r.time_series_count);
     w.dm = dms[best];

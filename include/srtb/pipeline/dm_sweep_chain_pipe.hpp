@@ -26,6 +26,7 @@ class dm_sweep_chain_pipe {
  protected:
   srtb::cuda_queue q;
   block_config_holder holder;
+  std::vector<srtb_b200_event> events;  // dm_search_candidates: [streams][candidate_event_cap], reused
 
  public:
   explicit dm_sweep_chain_pipe(srtb::cuda_queue q_) : q{q_} {}
@@ -60,9 +61,18 @@ class dm_sweep_chain_pipe {
     int32_t best[4] = {0, 0, 0, 0};
     outputs.h_peaks = peaks.data();
     outputs.h_best_trial = best;
-    q.check(srtb_b200_process_block_dm_sweep_ex(q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(),
-                                                in_work.baseband_data.baseband_input_bytes, /*on_device=*/0, dms.data(),
-                                                n_dm, res.data(), &outputs));
+    const bool candidates = srtb::config.dm_search_candidates;
+    uint64_t n_events[4] = {0, 0, 0, 0};
+    if (candidates) {
+      events.resize((size_t)streams * candidate_event_cap);
+      q.check(srtb_b200_process_block_dm_sweep_events(
+          q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(), in_work.baseband_data.baseband_input_bytes,
+          /*on_device=*/0, dms.data(), n_dm, res.data(), &outputs, events.data(), candidate_event_cap, n_events));
+    } else {
+      q.check(srtb_b200_process_block_dm_sweep_ex(q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(),
+                                                  in_work.baseband_data.baseband_input_bytes, /*on_device=*/0,
+                                                  dms.data(), n_dm, res.data(), &outputs));
+    }
 
     for (int s = 0; s < streams; s++) {
       const srtb_b200_detect_result& r = res[(size_t)best[s] * streams + s];
@@ -86,6 +96,8 @@ class dm_sweep_chain_pipe {
                                pk.peak_index[b]});
         w.dm_trials.push_back(std::move(d));
       }
+      if (candidates)
+        attach_candidates(w, events.data() + (size_t)s * candidate_event_cap, n_events[s], candidate_event_cap, dms, 0);
       out.push_back(std::move(w));
     }
     return std::optional{std::move(out)};

@@ -7,6 +7,7 @@
 //   <prefix><counter>.<i>.npy        complex64 dynamic spectrum, shape {batch_size, count} (:209-246)
 //   <prefix><counter>.<boxcar>.tim   float32 time series per detected boxcar           (:249-280)
 // and, for a DM search (dm_list), <prefix><counter>.dm<DM>.<boxcar>.tim and <prefix><counter>.<id>.dm_sweep.csv.
+// With dm_search_candidates, also <prefix><counter>.<id>.candidates.csv: the block's single-pulse candidates.
 // With signal_detect_sum_polarizations, a block whose total intensity is positive keeps every stream's work, and the
 // first stream's work writes the sum's series as <prefix><counter>.sum.<boxcar>.tim (once per block).
 // counter = udp_packet_counter, or the timestamp when there is none (:145-148).
@@ -148,6 +149,34 @@ class write_signal_pipe {
           << fmt("%.9g", b.threshold) << "," << fmt("%.9g", b.peak_snr) << "," << b.peak_index << "\n";
     }
     if (!f) SRTB_LOGE << " [write_signal_pipe] " << "cannot write " << stem << ".dm_sweep.csv";
+    if (w.has_candidates) write_candidates(w, stem);
+  }
+
+  /** <stem>.<data_stream_id>.candidates.csv: a header row, then one row per candidate in the block's own share, those
+   *  whose window is below the work's candidate_share (candidate_share() in baseband_chain_pipe.hpp). sample = window +
+   *  the work's offset (S- for the incoherent search), time = (first_sample + 2C sample) / sample_rate in seconds from
+   *  input_file_offset_bytes, topocentric and referred to f_c (empty without a first_sample). */
+  static void write_candidates(const srtb::work::write_signal_work& w, const std::string& stem) {
+    auto fmt = [](const char* f, double v) {
+      char buf[64];
+      std::snprintf(buf, sizeof buf, f, v);
+      return std::string{buf};
+    };
+    const uint64_t two_c = 2 * (uint64_t)w.batch_size;
+    const bool placed = w.first_sample != w.no_first_sample;
+    std::ofstream f(stem + "." + std::to_string(w.data_stream_id) + ".candidates.csv", std::ios::trunc);
+    f << "snr,dm,boxcar_length,sample,time,members,dm_low,dm_high,span_begin,span_end,trial,peak_index\n";
+    for (const auto& c : w.candidates) {
+      if (c.window >= w.candidate_share) continue;
+      const uint64_t sample = c.window + w.candidate_sample_offset;
+      const std::string time =
+          placed ? fmt("%.12g", ((double)w.first_sample + (double)two_c * (double)sample) / srtb::config.baseband_sample_rate)
+                 : "";
+      f << fmt("%.9g", c.snr) << "," << fmt("%g", c.dm) << "," << c.boxcar_length << "," << sample << "," << time << ","
+        << c.members << "," << fmt("%g", c.dm_low) << "," << fmt("%g", c.dm_high) << "," << c.span_begin << ","
+        << c.span_end << "," << c.trial << "," << c.peak_index << "\n";
+    }
+    if (!f) SRTB_LOGE << " [write_signal_pipe] " << "cannot write " << stem << ".candidates.csv";
   }
 };
 

@@ -239,7 +239,7 @@ inline const std::vector<std::string>& known_options() {
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length",
       "signal_detect_sum_polarizations", "fold_period", "fold_period_derivative", "fold_bin_count",
-      "fold_subband_count", "fold_subintegration_blocks", "fold_coherence"};
+      "fold_subband_count", "fold_subintegration_blocks", "fold_coherence", "dm_search_candidates"};
   return names;
 }
 
@@ -379,6 +379,7 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(fold_subband_count)
   SRTB_PARSE(fold_subintegration_blocks)
   SRTB_PARSE(fold_coherence)
+  SRTB_PARSE(dm_search_candidates)
   SRTB_PARSE(thread_query_work_wait_time)
   SRTB_PARSE(gui_enable)
   SRTB_PARSE(gui_pixmap_width)
@@ -401,6 +402,13 @@ inline void check_dm_search_keys(const srtb::configs& config) {
     throw std::invalid_argument(
         "[program_options] dm_list and incoherent_dm_list are both set: choose the coherent DM sweep (dm_list) or the "
         "incoherent search around dm (incoherent_dm_list)");
+}
+
+/** dm_search_candidates lists the candidates of a DM search: it needs one (dm_list or incoherent_dm_list) */
+inline void check_dm_search_candidates(const srtb::configs& config) {
+  if (config.dm_search_candidates && trim(config.dm_list).empty() && trim(config.incoherent_dm_list).empty())
+    throw std::invalid_argument("[program_options] dm_search_candidates needs a DM search: set dm_list (the coherent "
+                                "DM sweep) or incoherent_dm_list (the incoherent search around dm)");
 }
 
 /** signal_detect_sum_polarizations adds the streams of a block: it needs two or more (`streams`, the format's count),

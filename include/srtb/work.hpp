@@ -220,6 +220,14 @@ struct fold_block {
   std::vector<uint32_t> coherence_kept;  // [subbands]
 };
 
+/** one single-pulse candidate of a DM search (srtb_b200_candidate): its representative event's S/N, DM, boxcar, trial
+ *  and window (the series index its boxcar window starts at), and the members' count, DM range and span */
+struct dm_candidate {
+  float snr = 0, dm = 0, dm_low = 0, dm_high = 0;
+  uint64_t boxcar_length = 0, peak_index = 0, window = 0, members = 0, span_begin = 0, span_end = 0;
+  uint32_t trial = 0;
+};
+
 struct write_signal_work : public write_file_work {
   std::vector<time_series_holder> time_series;  // non-empty <=> has_signal
   size_t zero_count = 0;
@@ -233,6 +241,12 @@ struct write_signal_work : public write_file_work {
   // DM search only (dm_sweep_chain_pipe): the best trial's DM, which ptr and time_series belong to, and every trial
   srtb::real dm = 0;
   std::vector<dm_trial_summary> dm_trials;
+  // dm_search_candidates: the block's candidates, the bound on their window of the block's own share (write_signal_pipe
+  // writes those below it) and the spectrum sample of series index 0 (S- for the incoherent search, 0 for the sweep)
+  bool has_candidates = false;
+  std::vector<dm_candidate> candidates;
+  uint64_t candidate_share = 0;
+  uint64_t candidate_sample_offset = 0;
   // fold_period: the block's fold (srtb_b200_fold), carried by the block's first stream
   std::shared_ptr<const fold_block> fold;
 };

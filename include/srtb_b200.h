@@ -367,6 +367,83 @@ int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, s
                                    srtb_b200_peak* h_peaks /* [n_dm] or NULL */, int32_t* h_best_trial /* or NULL */,
                                    float* h_series /* [SRTB_B200_MAX_BOXCARS][T] or NULL */);
 
+/* ---- single-pulse events and candidates of a DM search ------------------------------------------------------------
+ * An event is a maximal run [begin, end) of consecutive indices of one boxcar series v of one trial (and stream) with
+ * every v[j] > threshold[b] (count_signal's strict comparison, so the lengths of a row's events add up to its
+ * signal_count). peak_index is the smallest index holding the run's largest value, snr that value / sqrt(variance[b])
+ * (0 when the variance is 0): srtb_b200_peak's definition, so a row's largest-snr event is its peak record. trial is an
+ * index into h_dms as given, boxcar the index b (length 2^b). The rows searched are those the detector headers describe:
+ * boxcars b < n_boxcars of every trial with detect_enabled, each series_length[b] long, read on the device.
+ * Events are listed in (stream, trial, boxcar, begin) order, the same bytes on every call. When more than max_events
+ * exist the first max_events are written and *n_events is the total. Two kernel launches per (trial group, stream): a
+ * tile summary with the scan of run counts, then the events (csrc/events.cuh); the list crosses PCIe as it is written,
+ * into pinned memory the ctx grows on demand and keeps (max_events per stream), and the ctx's device scratch holds 24
+ * bytes per tile of 4096 samples of the rows searched. */
+typedef struct {
+  uint64_t begin, end;  /* the run [begin, end) in the boxcar series */
+  uint64_t peak_index;  /* smallest index of the run's largest value */
+  float snr;            /* that value / sqrt(variance), 0 when the variance is 0 */
+  uint32_t trial;       /* index into h_dms (srtb_b200_series_events: the record index) */
+  uint32_t boxcar;      /* b: boxcar length 2^b */
+  uint32_t stream;
+} srtb_b200_event;
+/* The event pass on caller-owned series: record y's boxcar b is d_series + y trial_stride + b boxcar_stride (floats),
+ * described by h_results[y] (detect_enabled, n_boxcars, series_length, threshold, variance; the other fields are not
+ * read). Events carry trial = y, stream = 0. Before any launch: a null ctx, d_series, h_results or n_events, a null
+ * h_events with max_events > 0, n_trials == 0 or above 65535, n_boxcars above 32, a row longer than boxcar_stride (when
+ * n_boxcars > 1) or n_boxcars rows longer than trial_stride (when n_trials > 1) returns SRTB_B200_E_INVALID.
+ * Synchronises the ctx's stream. */
+int srtb_b200_series_events(srtb_b200_ctx* ctx, const float* d_series, size_t boxcar_stride, size_t trial_stride,
+                            const srtb_b200_detect_result* h_results, size_t n_trials, srtb_b200_event* h_events,
+                            size_t max_events, uint64_t* n_events);
+/* srtb_b200_incoherent_dm_search, which also lists the events of every trial's series (stream 0). Indices are in the
+ * searched series: spectrum sample = index + S-. Results, peaks, best trial and series are bit-identical to the plain
+ * entry's; two launches more, the same synchronisations. Refusals as the plain entry, and SRTB_B200_E_INVALID for a null
+ * n_events or a null h_events with max_events > 0. */
+int srtb_b200_incoherent_dm_search_events(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count,
+                                          size_t chan_count, size_t time_reserved_count, float freq_low,
+                                          float bandwidth, float sample_rate, float dm, const float* h_dms, size_t n_dm,
+                                          float snr, float channel_threshold, size_t max_boxcar_length,
+                                          srtb_b200_detect_result* h_results, srtb_b200_peak* h_peaks,
+                                          int32_t* h_best_trial, float* h_series, srtb_b200_event* h_events,
+                                          size_t max_events, uint64_t* n_events);
+/* srtb_b200_process_block_dm_sweep_ex, which also lists the events of every trial of the loop (never of the best trial's
+ * re-run): stream s's events go to h_events + s max_events (up to max_events of them), their total to n_events[s].
+ * Results, peaks, best trial, spectra and series are bit-identical to _ex's; two launches more per trial and stream, the
+ * same synchronisations (once, and once more when the best trial is re-run). Refusals as _ex, and SRTB_B200_E_INVALID
+ * for a null n_events or a null h_events with max_events > 0. */
+int srtb_b200_process_block_dm_sweep_events(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
+                                            const void* baseband, size_t baseband_bytes, int on_device,
+                                            const float* h_dms, size_t n_dm, srtb_b200_detect_result* h_results,
+                                            const srtb_b200_sweep_outputs* outputs /* or NULL */,
+                                            srtb_b200_event* h_events /* [streams][max_events] */, size_t max_events,
+                                            uint64_t* n_events /* [streams] */);
+/* Candidates: events grouped into astrophysical detections (host only, deterministic; friends of friends, no tunables).
+ *   span: the base-series samples an event's boxcar windows add, [begin + o, end - 1 + o + 2^b) with o = 0 for b = 0
+ *         and o = 1 otherwise (v_b[j] sums samples j+1 .. j+b of the scan);
+ *   rank: a trial's position after a stable sort of h_dms by DM (repeated DMs are adjacent ranks);
+ *   friends: the same stream, ranks at most 1 apart, intersecting spans. A candidate is a connected component.
+ * Its representative is the member with the largest snr (ties: the smaller trial, boxcar, begin), whose snr, DM, trial,
+ * boxcar length and peak_index it carries, with window = peak_index + o (the series index the boxcar's window starts
+ * at); members, dm_low / dm_high over the members, and [span_begin, span_end), the union of their spans. Candidates are
+ * ordered by (stream, span_begin, representative trial, boxcar, begin); the first max_candidates are written and
+ * *n_candidates is the total. A sweep over the spans keeps one active event per rank, O(n log n) in the events. A null
+ * n_candidates, a null h_events with n_events > 0, a null h_dms, n_dm == 0, a null h_candidates with
+ * max_candidates > 0, an event with trial >= n_dm, boxcar above 31 or end <= begin returns SRTB_B200_E_INVALID. */
+typedef struct {
+  float snr, dm;              /* the representative's */
+  float dm_low, dm_high;      /* over the members */
+  uint64_t boxcar_length;     /* the representative's, 2^b */
+  uint64_t peak_index;        /* the representative's, in its boxcar series */
+  uint64_t window;            /* peak_index + o */
+  uint64_t members;
+  uint64_t span_begin, span_end;
+  uint32_t trial;             /* the representative's */
+  uint32_t stream;
+} srtb_b200_candidate;
+int srtb_b200_cluster_events(const srtb_b200_event* h_events, size_t n_events, const float* h_dms, size_t n_dm,
+                             srtb_b200_candidate* h_candidates, size_t max_candidates, uint64_t* n_candidates);
+
 /* ---- folding at a known pulsar period --------------------------------------------------------------------------
  * Time of a spectrum sample. A block whose first baseband sample (per stream) is first_sample holds the spectrum
  * samples j < L at t_j = (first_sample + 2C j) / sample_rate; t = 0 is the first sample after input_file_offset_bytes.

@@ -27,6 +27,7 @@
 #include "incoherent.cuh"
 #include "stream_sum.cuh"
 #include "fold.cuh"
+#include "events.cuh"
 
 using namespace srtb_b200;
 
@@ -161,6 +162,10 @@ struct srtb_b200_ctx {
   buffer<char> inc_tab, inc_work;
   // fold: the sorted bin plan, hits, profile and kept, and the per-CTA rows fold_finish_kernel adds (srtb_b200_fold)
   buffer<char> fold_work;
+  // events (events.cuh): tile summaries, scan offsets, per-stream event counts, ticket and uploaded headers on the
+  // device; the counts, then [streams][max_events] events in pinned memory the emit kernel writes through
+  buffer<char> ev_work;
+  buffer<char, true> ev_host;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -2255,6 +2260,238 @@ extern "C" int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block
   return srtb_b200_process_block_device(ctx, cfg, ctx->d_baseband.p, baseband_bytes, h_results, h_series, copy_all);
 }
 
+// ---- events: every above-threshold run of the detector's series (events.cuh) -----------------------------------------
+static_assert(sizeof(ev_event) == sizeof(srtb_b200_event) && sizeof(ev_event) == 40, "event layout");
+
+// where a DM search's events go: max_events per stream into h_events, the totals into n_events[streams]
+struct ev_request {
+  srtb_b200_event* h_events;
+  size_t max_events;
+  uint64_t* n_events;
+};
+
+// the device scratch of the event launches of one call: tile summaries and offsets for n_rec records of max_nb rows of at
+// most row_len samples, the streams' running counts (zeroed) and the ticket, and room for n_headers uploaded headers;
+// the pinned list holds the counts, then max_events per stream. Grows before any launch of the call.
+struct ev_scratch {
+  ev_tile* tile;
+  unsigned long long* offset;
+  unsigned long long* count;  // [4]
+  unsigned* ticket;
+  detect_dev_result* headers;
+  size_t tiles;
+};
+static int events_prepare(srtb_b200_ctx* ctx, const char* who, size_t n_rec, unsigned max_nb, size_t row_len,
+                          int streams, size_t max_events, size_t n_headers, ev_scratch* sc) {
+  sc->tiles = std::max<size_t>(1, (row_len + EV_TILE - 1) / EV_TILE);
+  const size_t nt = n_rec * max_nb * sc->tiles;
+  if (n_rec > 65535 || sc->tiles > 0x7fffffffu || nt >= ((size_t)1 << 32))
+    return fail(ctx, SRTB_B200_E_SIZE, std::string(who) + ": too many tiles for the event pass");
+  const size_t off_o = (nt * sizeof(ev_tile) + 255) & ~(size_t)255;
+  const size_t cnt_o = (off_o + nt * sizeof(unsigned long long) + 255) & ~(size_t)255;
+  const size_t hdr_o = cnt_o + 256;
+  if (int rc = grow(ctx, ctx->ev_work, hdr_o + n_headers * sizeof(detect_dev_result))) return rc;
+  const size_t list_b = 256 + (size_t)streams * std::max<size_t>(max_events, 1) * sizeof(ev_event);
+  if (int rc = grow(ctx, ctx->ev_host, list_b)) return rc;
+  char* w = ctx->ev_work.p;
+  sc->tile = reinterpret_cast<ev_tile*>(w);
+  sc->offset = reinterpret_cast<unsigned long long*>(w + off_o);
+  sc->count = reinterpret_cast<unsigned long long*>(w + cnt_o);
+  sc->ticket = reinterpret_cast<unsigned*>(w + cnt_o + 4 * sizeof(unsigned long long));
+  sc->headers = reinterpret_cast<detect_dev_result*>(w + hdr_o);
+  CK(cudaMemsetAsync(w + cnt_o, 0, 256, ctx->lane.stream));
+  return 0;
+}
+
+// the two event launches over n_rec records (rows as r describes them), into stream r.stream's list
+static int events_enqueue(srtb_b200_ctx* ctx, const ev_scratch& sc, const ev_rows& r, size_t n_rec, size_t max_events) {
+  const dim3 grid((unsigned)sc.tiles, r.max_nb, (unsigned)n_rec);
+  ev_event* list = reinterpret_cast<ev_event*>(ctx->ev_host.p + 256) + (size_t)r.stream * max_events;
+  CK(launch(ctx, false, ev_count_kernel, grid, EV_THREADS, 0, r, sc.tile, sc.offset, sc.ticket, sc.count + r.stream));
+  CK(launch(ctx, false, ev_emit_kernel, grid, EV_THREADS, 0, r, (const ev_tile*)sc.tile,
+            (const unsigned long long*)sc.offset, list, (unsigned long long)max_events));
+  return 0;
+}
+
+// enqueued before the call's synchronisation: the streams' counts into the pinned list's head
+static int events_fetch_counts(srtb_b200_ctx* ctx, const ev_scratch& sc, int streams) {
+  CK(cudaMemcpyAsync(ctx->ev_host.p, sc.count, streams * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                     ctx->lane.stream));
+  return 0;
+}
+
+// after the synchronisation: the counts and the written events to the caller
+static void events_collect(srtb_b200_ctx* ctx, int streams, const ev_request& ev) {
+  const unsigned long long* counts = reinterpret_cast<const unsigned long long*>(ctx->ev_host.p);
+  const ev_event* list = reinterpret_cast<const ev_event*>(ctx->ev_host.p + 256);
+  for (int s = 0; s < streams; s++) {
+    ev.n_events[s] = counts[s];
+    const size_t k = (size_t)std::min<unsigned long long>(counts[s], ev.max_events);
+    if (k) std::memcpy(ev.h_events + (size_t)s * ev.max_events, list + (size_t)s * ev.max_events, k * sizeof(ev_event));
+  }
+}
+
+static bool ev_request_ok(const ev_request* ev) {
+  return !ev || (ev->n_events && (ev->h_events || ev->max_events == 0));
+}
+
+extern "C" int srtb_b200_series_events(srtb_b200_ctx* ctx, const float* d_series, size_t boxcar_stride,
+                                       size_t trial_stride, const srtb_b200_detect_result* h_results, size_t n_trials,
+                                       srtb_b200_event* h_events, size_t max_events, uint64_t* n_events) {
+  API_LOCK(ctx);
+  const ev_request ev{h_events, max_events, n_events};
+  if (!ctx || !d_series || !h_results || !ev_request_ok(&ev) || n_trials == 0 || n_trials > 65535)
+    return fail(ctx, SRTB_B200_E_INVALID, "series_events: bad argument");
+  unsigned max_nb = 0;
+  size_t row_len = 0;
+  for (size_t y = 0; y < n_trials; y++) {
+    const srtb_b200_detect_result& r = h_results[y];
+    if (r.n_boxcars < 0 || r.n_boxcars > SRTB_B200_MAX_BOXCARS)
+      return fail(ctx, SRTB_B200_E_INVALID, "series_events: n_boxcars outside 0..32");
+    if (!r.detect_enabled) continue;
+    max_nb = std::max(max_nb, (unsigned)r.n_boxcars);
+    size_t extent = 0;  // of the trial's rows
+    for (int b = 0; b < r.n_boxcars; b++) {
+      row_len = std::max<size_t>(row_len, r.series_length[b]);
+      extent = std::max<size_t>(extent, (size_t)b * boxcar_stride + r.series_length[b]);
+      if (r.n_boxcars > 1 && r.series_length[b] > boxcar_stride)
+        return fail(ctx, SRTB_B200_E_INVALID, "series_events: a row is longer than boxcar_stride");
+    }
+    if (n_trials > 1 && extent > trial_stride)
+      return fail(ctx, SRTB_B200_E_INVALID, "series_events: a trial's rows are longer than trial_stride");
+  }
+  CK(cudaSetDevice(ctx->device));
+  ev_scratch sc;
+  if (int rc = events_prepare(ctx, "series_events", n_trials, std::max(max_nb, 1u), row_len, 1, max_events, n_trials, &sc))
+    return rc;
+  static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
+  CK(cudaMemcpyAsync(sc.headers, h_results, n_trials * sizeof(detect_dev_result), cudaMemcpyHostToDevice,
+                     ctx->lane.stream));
+  if (max_nb > 0) {
+    const ev_rows r{d_series, boxcar_stride, trial_stride, sc.headers, max_nb, sc.tiles, 0u, 0u};
+    if (int rc = events_enqueue(ctx, sc, r, n_trials, max_events)) return rc;
+  }
+  if (int rc = events_fetch_counts(ctx, sc, 1)) return rc;
+  CK(cudaStreamSynchronize(ctx->lane.stream));
+  events_collect(ctx, 1, ev);
+  return 0;
+}
+
+// friends of friends over the events (include/srtb_b200.h): union-find, joined by one sweep over the spans per stream
+extern "C" int srtb_b200_cluster_events(const srtb_b200_event* h_events, size_t n_events, const float* h_dms,
+                                        size_t n_dm, srtb_b200_candidate* h_candidates, size_t max_candidates,
+                                        uint64_t* n_candidates) {
+  if (!n_candidates || (!h_events && n_events) || !h_dms || n_dm == 0 || (!h_candidates && max_candidates))
+    return fail(nullptr, SRTB_B200_E_INVALID, "cluster_events: bad argument");
+  for (size_t i = 0; i < n_events; i++) {
+    const srtb_b200_event& e = h_events[i];
+    if (e.trial >= n_dm || e.boxcar > 31 || e.end <= e.begin)
+      return fail(nullptr, SRTB_B200_E_INVALID, "cluster_events: event " + std::to_string(i) + " is malformed");
+  }
+  std::vector<uint32_t> rank(n_dm), order(n_dm);
+  for (size_t d = 0; d < n_dm; d++) order[d] = (uint32_t)d;
+  std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return h_dms[a] < h_dms[b]; });
+  for (size_t r = 0; r < n_dm; r++) rank[order[r]] = (uint32_t)r;
+  auto o_of = [](const srtb_b200_event& e) -> uint64_t { return e.boxcar ? 1 : 0; };
+  auto lo_of = [&](const srtb_b200_event& e) { return e.begin + o_of(e); };
+  auto hi_of = [&](const srtb_b200_event& e) { return e.end - 1 + o_of(e) + ((uint64_t)1 << e.boxcar); };
+  std::vector<size_t> parent(n_events);
+  for (size_t i = 0; i < n_events; i++) parent[i] = i;
+  auto find = [&](size_t i) {
+    while (parent[i] != i) {
+      parent[i] = parent[parent[i]];
+      i = parent[i];
+    }
+    return i;
+  };
+  auto unite = [&](size_t a, size_t b) {
+    a = find(a);
+    b = find(b);
+    if (a != b) parent[std::max(a, b)] = std::min(a, b);
+  };
+  // sweep by (stream, span begin): every active event of a rank contains the sweep point, so those of one rank are
+  // friends of each other and of the event at the sweep point when the ranks are at most 1 apart. One active event per
+  // rank (the one whose span ends last) stands for all of them.
+  std::vector<size_t> by(n_events);
+  for (size_t i = 0; i < n_events; i++) by[i] = i;
+  std::sort(by.begin(), by.end(), [&](size_t a, size_t b) {
+    const srtb_b200_event &x = h_events[a], &y = h_events[b];
+    if (x.stream != y.stream) return x.stream < y.stream;
+    if (lo_of(x) != lo_of(y)) return lo_of(x) < lo_of(y);
+    return a < b;
+  });
+  std::vector<uint64_t> act_end(n_dm, 0);
+  std::vector<size_t> act_id(n_dm, 0);
+  std::vector<uint32_t> act_stream(n_dm, ~0u);
+  for (size_t i : by) {
+    const srtb_b200_event& e = h_events[i];
+    const uint64_t x = lo_of(e), end = hi_of(e);
+    const uint32_t r = rank[e.trial];
+    for (uint32_t q = r ? r - 1 : 0; q <= r + 1 && q < n_dm; q++)
+      if (act_stream[q] == e.stream && act_end[q] > x) unite(i, act_id[q]);
+    if (act_stream[r] != e.stream || act_end[r] <= x || end > act_end[r]) {
+      act_stream[r] = e.stream;
+      act_end[r] = end;
+      act_id[r] = i;
+    }
+  }
+  // components: representative, members, DM range, span
+  std::vector<size_t> comp(n_events, SIZE_MAX);
+  std::vector<srtb_b200_candidate> cands;
+  std::vector<size_t> rep;  // event index of each candidate's representative
+  auto better = [&](const srtb_b200_event& a, const srtb_b200_event& b) {  // a beats b
+    if (a.snr != b.snr) return a.snr > b.snr;
+    if (a.trial != b.trial) return a.trial < b.trial;
+    if (a.boxcar != b.boxcar) return a.boxcar < b.boxcar;
+    return a.begin < b.begin;
+  };
+  for (size_t i = 0; i < n_events; i++) {
+    const size_t root = find(i);
+    const srtb_b200_event& e = h_events[i];
+    const float dm = h_dms[e.trial];
+    if (comp[root] == SIZE_MAX) {
+      comp[root] = cands.size();
+      srtb_b200_candidate c{};
+      c.dm_low = c.dm_high = dm;
+      c.span_begin = lo_of(e);
+      c.span_end = hi_of(e);
+      c.stream = e.stream;
+      cands.push_back(c);
+      rep.push_back(i);
+    }
+    srtb_b200_candidate& c = cands[comp[root]];
+    c.members++;
+    c.dm_low = std::min(c.dm_low, dm);
+    c.dm_high = std::max(c.dm_high, dm);
+    c.span_begin = std::min(c.span_begin, lo_of(e));
+    c.span_end = std::max(c.span_end, hi_of(e));
+    if (better(e, h_events[rep[comp[root]]])) rep[comp[root]] = i;
+  }
+  for (size_t k = 0; k < cands.size(); k++) {
+    const srtb_b200_event& e = h_events[rep[k]];
+    srtb_b200_candidate& c = cands[k];
+    c.snr = e.snr;
+    c.dm = h_dms[e.trial];
+    c.trial = e.trial;
+    c.boxcar_length = (uint64_t)1 << e.boxcar;
+    c.peak_index = e.peak_index;
+    c.window = e.peak_index + o_of(e);
+  }
+  std::vector<size_t> out(cands.size());
+  for (size_t k = 0; k < out.size(); k++) out[k] = k;
+  std::sort(out.begin(), out.end(), [&](size_t a, size_t b) {
+    const srtb_b200_candidate &x = cands[a], &y = cands[b];
+    if (x.stream != y.stream) return x.stream < y.stream;
+    if (x.span_begin != y.span_begin) return x.span_begin < y.span_begin;
+    if (x.trial != y.trial) return x.trial < y.trial;
+    if (x.boxcar_length != y.boxcar_length) return x.boxcar_length < y.boxcar_length;
+    return h_events[rep[a]].begin < h_events[rep[b]].begin;
+  });
+  *n_candidates = cands.size();
+  for (size_t k = 0; k < std::min(max_candidates, out.size()); k++) h_candidates[k] = cands[out[k]];
+  return 0;
+}
+
 // ---- DM sweep on one block (BASELINE config #4): unpack + R2C + mean once per stream, then for every
 // trial DM the s1-apply + chirp (out of place, the spectrum is kept), waterfall FFT, SK and detector.
 // Each trial's result equals process_block with cfg->dm = that DM on the same block.
@@ -2294,13 +2531,12 @@ extern "C" int srtb_b200_process_block_dm_sweep(srtb_b200_ctx* ctx, const srtb_b
                                              nullptr);
 }
 
-extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
-                                                   const void* baseband, size_t baseband_bytes, int on_device,
-                                                   const float* h_dms, size_t n_dm,
-                                                   srtb_b200_detect_result* h_results /* [n_dm][streams] */,
-                                                   const srtb_b200_sweep_outputs* outputs /* or NULL */) {
+// ev (or null): every trial's events, listed by the two event launches after its detector
+static int dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* baseband, size_t baseband_bytes,
+                    int on_device, const float* h_dms, size_t n_dm, srtb_b200_detect_result* h_results,
+                    const srtb_b200_sweep_outputs* outputs, const ev_request* ev) {
   API_LOCK(ctx);
-  if (!ctx || !cfg || !baseband || !h_dms || !h_results || n_dm == 0)
+  if (!ctx || !cfg || !baseband || !h_dms || !h_results || n_dm == 0 || !ev_request_ok(ev))
     return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: bad argument");
   if (cfg->signal_detect_sum_streams)
     return fail(ctx, SRTB_B200_E_UNSUPPORTED, "dm_sweep: signal_detect_sum_streams is not supported by the DM sweep");
@@ -2344,6 +2580,11 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
   float* const d_means = outputs ? reinterpret_cast<float*>(d_peaks + n_rec) : nullptr;
   // zeroed once before the first kernel: a memset between kernels would break the dependent-launch chain
   if (outputs) CK(cudaMemsetAsync(d_peaks, 0, n_rec * sizeof(detect_dev_peak), ctx->lane.stream));
+  // events: rows of at most L samples and boxcar_ctas(max, L) boxcars per trial, one trial per launch pair
+  ev_scratch sc{};
+  const unsigned ev_nb = boxcar_ctas(cfg->signal_detect_max_boxcar_length, p.L);
+  if (ev)
+    if (int rc = events_prepare(ctx, "dm_sweep", 1, ev_nb, p.L, p.streams, ev->max_events, 0, &sc)) return rc;
   block_input in{d_baseband, baseband_bytes, bufs};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
   for (int s = 0; s < p.streams; s++) {
@@ -2358,19 +2599,27 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
       if (int rc = stream_tail(ctx, p, out, W, buf, h_dms[j], /*phase_table=*/false)) return rc;
       CK(cudaMemcpyAsync(d_sweep + j * p.streams + s, ctx->d_res, sizeof(detect_dev_result), cudaMemcpyDeviceToDevice,
                          ctx->lane.stream));
+      if (ev) {  // the trial's series and header, before the next trial overwrites them
+        const ev_rows r{ctx->series[0].p, p.L, 0, ctx->d_res, ev_nb, sc.tiles, (unsigned)j, (unsigned)s};
+        if (int rc = events_enqueue(ctx, sc, r, 1, ev->max_events)) return rc;
+      }
     }
   }
+  if (ev)
+    if (int rc = events_fetch_counts(ctx, sc, p.streams)) return rc;
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
   static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
   CK(cudaMemcpyAsync(h_results, d_sweep, n_rec * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
   if (!outputs) {
     CK(cudaStreamSynchronize(ctx->lane.stream));
+    if (ev) events_collect(ctx, p.streams, *ev);
     return p.streams;
   }
   std::vector<detect_dev_peak> own_peaks(outputs->h_peaks ? 0 : n_rec);
   detect_dev_peak* h_peaks = outputs->h_peaks ? reinterpret_cast<detect_dev_peak*>(outputs->h_peaks) : own_peaks.data();
   CK(cudaMemcpyAsync(h_peaks, d_peaks, n_rec * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, ctx->lane.stream));
   CK(cudaStreamSynchronize(ctx->lane.stream));
+  if (ev) events_collect(ctx, p.streams, *ev);
   int best[4] = {0, 0, 0, 0};
   for (int s = 0; s < p.streams; s++) {
     best[s] = best_trial(h_results, h_peaks, n_dm, p.streams, s);
@@ -2394,6 +2643,25 @@ extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srt
       return fail(ctx, SRTB_B200_E_CUDA,
                   "dm_sweep: the best trial's re-run of stream " + std::to_string(s) + " differs from its trial");
   return p.streams;
+}
+
+extern "C" int srtb_b200_process_block_dm_sweep_ex(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
+                                                   const void* baseband, size_t baseband_bytes, int on_device,
+                                                   const float* h_dms, size_t n_dm,
+                                                   srtb_b200_detect_result* h_results /* [n_dm][streams] */,
+                                                   const srtb_b200_sweep_outputs* outputs /* or NULL */) {
+  return dm_sweep(ctx, cfg, baseband, baseband_bytes, on_device, h_dms, n_dm, h_results, outputs, nullptr);
+}
+
+extern "C" int srtb_b200_process_block_dm_sweep_events(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
+                                                       const void* baseband, size_t baseband_bytes, int on_device,
+                                                       const float* h_dms, size_t n_dm,
+                                                       srtb_b200_detect_result* h_results,
+                                                       const srtb_b200_sweep_outputs* outputs,
+                                                       srtb_b200_event* h_events, size_t max_events,
+                                                       uint64_t* n_events) {
+  const ev_request ev{h_events, max_events, n_events};
+  return dm_sweep(ctx, cfg, baseband, baseband_bytes, on_device, h_dms, n_dm, h_results, outputs, &ev);
 }
 
 // ---- incoherent DM search on one stream's dynamic spectrum (incoherent.cuh): every trial's series in one kernel, then
@@ -2527,14 +2795,15 @@ static int incoherent_tables(srtb_b200_ctx* ctx, size_t C, float freq_low, float
   return 0;
 }
 
-extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count,
-                                              size_t chan_count, size_t time_reserved_count, float freq_low,
-                                              float bandwidth, float sample_rate, float dm, const float* h_dms,
-                                              size_t n_dm, float snr, float channel_threshold,
-                                              size_t max_boxcar_length, srtb_b200_detect_result* h_results,
-                                              srtb_b200_peak* h_peaks, int32_t* h_best_trial, float* h_series) {
+// ev (or null): every trial's events, listed by two launches after the detector
+static int incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count, size_t chan_count,
+                                size_t time_reserved_count, float freq_low, float bandwidth, float sample_rate,
+                                float dm, const float* h_dms, size_t n_dm, float snr, float channel_threshold,
+                                size_t max_boxcar_length, srtb_b200_detect_result* h_results, srtb_b200_peak* h_peaks,
+                                int32_t* h_best_trial, float* h_series, const ev_request* ev) {
   API_LOCK(ctx);
-  if (!ctx || !d_spectrum || !h_dms || !h_results || n_dm == 0 || time_count == 0 || chan_count == 0)
+  if (!ctx || !d_spectrum || !h_dms || !h_results || n_dm == 0 || time_count == 0 || chan_count == 0 ||
+      !ev_request_ok(ev))
     return fail(ctx, SRTB_B200_E_INVALID, "incoherent_dm_search: bad argument");
   if (!aligned8(d_spectrum)) return fail(ctx, SRTB_B200_E_INVALID, "incoherent_dm_search: spectrum not 8-byte aligned");
   if (time_reserved_count >= time_count)
@@ -2567,6 +2836,9 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   const size_t ticket_o = peak_o + n_dm * sizeof(detect_dev_peak);
   const size_t work_b = ticket_o + n_dm * sizeof(unsigned);
   if (int rc = grow(ctx, ctx->inc_work, work_b)) return rc;
+  ev_scratch sc{};
+  if (ev)
+    if (int rc = events_prepare(ctx, "incoherent_dm_search", n_dm, max_nb, T, 1, ev->max_events, 0, &sc)) return rc;
   char* tab = ctx->inc_tab.p;
   char* work = ctx->inc_work.p;
   float* d_series = reinterpret_cast<float*>(work);
@@ -2599,6 +2871,11 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
             d_ticket, d_res, series_stride, T, nullptr));
   CK(launch(ctx, false, detect_boxcar_kernel<true>, dim3(max_nb, (unsigned)n_dm), 1024, 0, d_series, T, d_acc, T, snr,
             d_res, nullptr, d_peak, series_stride, T));
+  if (ev) {
+    const ev_rows r{d_series, T, series_stride, d_res, max_nb, sc.tiles, 0u, 0u};
+    if (int rc = events_enqueue(ctx, sc, r, n_dm, ev->max_events)) return rc;
+    if (int rc = events_fetch_counts(ctx, sc, 1)) return rc;
+  }
   static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
   static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
   std::vector<srtb_b200_peak> own_peaks(h_peaks ? 0 : n_dm);
@@ -2606,6 +2883,7 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   CK(cudaMemcpyAsync(h_results, d_res, n_dm * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(peaks, d_peak, n_dm * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
+  if (ev) events_collect(ctx, 1, *ev);
   const int best = best_trial(h_results, reinterpret_cast<const detect_dev_peak*>(peaks), n_dm, 1, 0);
   if (h_best_trial) *h_best_trial = best;
   if (!h_series) return 0;
@@ -2620,6 +2898,30 @@ extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_
   }
   if (any) CK(cudaStreamSynchronize(st));
   return 0;
+}
+
+extern "C" int srtb_b200_incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count,
+                                              size_t chan_count, size_t time_reserved_count, float freq_low,
+                                              float bandwidth, float sample_rate, float dm, const float* h_dms,
+                                              size_t n_dm, float snr, float channel_threshold,
+                                              size_t max_boxcar_length, srtb_b200_detect_result* h_results,
+                                              srtb_b200_peak* h_peaks, int32_t* h_best_trial, float* h_series) {
+  return incoherent_dm_search(ctx, d_spectrum, time_count, chan_count, time_reserved_count, freq_low, bandwidth,
+                              sample_rate, dm, h_dms, n_dm, snr, channel_threshold, max_boxcar_length, h_results,
+                              h_peaks, h_best_trial, h_series, nullptr);
+}
+
+extern "C" int srtb_b200_incoherent_dm_search_events(srtb_b200_ctx* ctx, const void* d_spectrum, size_t time_count,
+                                                     size_t chan_count, size_t time_reserved_count, float freq_low,
+                                                     float bandwidth, float sample_rate, float dm, const float* h_dms,
+                                                     size_t n_dm, float snr, float channel_threshold,
+                                                     size_t max_boxcar_length, srtb_b200_detect_result* h_results,
+                                                     srtb_b200_peak* h_peaks, int32_t* h_best_trial, float* h_series,
+                                                     srtb_b200_event* h_events, size_t max_events, uint64_t* n_events) {
+  const ev_request ev{h_events, max_events, n_events};
+  return incoherent_dm_search(ctx, d_spectrum, time_count, chan_count, time_reserved_count, freq_low, bandwidth,
+                              sample_rate, dm, h_dms, n_dm, snr, channel_threshold, max_boxcar_length, h_results,
+                              h_peaks, h_best_trial, h_series, &ev);
 }
 
 // ---- fold at a pulsar period (fold.cuh): the bin plan of each time tile, one read of the spectra into per-CTA bin

@@ -84,6 +84,31 @@ class SweepOutputs(C.Structure):
                 ("d_spectrum", C.c_void_p * 4)]
 
 
+class Event(C.Structure):
+    """srtb_b200_event: one above-threshold run [begin, end) of one boxcar series of one trial and stream"""
+    _fields_ = [("begin", C.c_uint64), ("end", C.c_uint64), ("peak_index", C.c_uint64), ("snr", C.c_float),
+                ("trial", C.c_uint32), ("boxcar", C.c_uint32), ("stream", C.c_uint32)]
+
+
+class Candidate(C.Structure):
+    """srtb_b200_candidate: one friends-of-friends group of events (srtb_b200_cluster_events)"""
+    _fields_ = [("snr", C.c_float), ("dm", C.c_float), ("dm_low", C.c_float), ("dm_high", C.c_float),
+                ("boxcar_length", C.c_uint64), ("peak_index", C.c_uint64), ("window", C.c_uint64),
+                ("members", C.c_uint64), ("span_begin", C.c_uint64), ("span_end", C.c_uint64),
+                ("trial", C.c_uint32), ("stream", C.c_uint32)]
+
+
+def _dtype_of(struct):
+    """the numpy structured dtype with struct's field names, offsets and size"""
+    import numpy as np
+    names, formats, offsets = [], [], []
+    for name, ctype in struct._fields_:
+        names.append(name)
+        formats.append(np.dtype(ctype))
+        offsets.append(getattr(struct, name).offset)
+    return np.dtype({"names": names, "formats": formats, "offsets": offsets, "itemsize": C.sizeof(struct)})
+
+
 class SrtbError(RuntimeError):
     def __init__(self, code: int, message: str):
         super().__init__(f"srtb_b200 error {code}: {message}")
@@ -148,6 +173,15 @@ SYMBOLS = {
                                          C.POINTER(C.c_uint32)]),
     "srtb_b200_incoherent_dm_search": (_I, [_P, _P, _SZ, _SZ, _SZ, _F, _F, _F, _F, C.POINTER(_F), _SZ, _F, _F, _SZ,
                                             C.POINTER(DetectResult), _P, _P, _P]),
+    "srtb_b200_series_events": (_I, [_P, _P, _SZ, _SZ, C.POINTER(DetectResult), _SZ, _P, _SZ,
+                                     C.POINTER(C.c_uint64)]),
+    "srtb_b200_incoherent_dm_search_events": (_I, [_P, _P, _SZ, _SZ, _SZ, C.c_float, C.c_float, C.c_float,
+                                                   C.c_float, C.POINTER(C.c_float), _SZ, C.c_float, C.c_float, _SZ,
+                                                   C.POINTER(DetectResult), _P, _P, _P, _P, _SZ,
+                                                   C.POINTER(C.c_uint64)]),
+    "srtb_b200_process_block_dm_sweep_events": (_I, [_P, _P, _P, _SZ, _I, C.POINTER(C.c_float), _SZ,
+                                                     C.POINTER(DetectResult), _P, _P, _SZ, C.POINTER(C.c_uint64)]),
+    "srtb_b200_cluster_events": (_I, [_P, _SZ, C.POINTER(C.c_float), _SZ, _P, _SZ, C.POINTER(C.c_uint64)]),
     "srtb_b200_fold_phase": (_I, [C.c_double, C.c_double, C.c_double, C.c_uint64, C.c_uint64,
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "srtb_b200_fold": (_I, [_P, C.POINTER(_P), _I, _SZ, _SZ, _SZ, C.c_double, C.c_double, C.c_double, _SZ, _SZ,
@@ -300,8 +334,16 @@ class Context:
         n = self._ck(fn(self.h, C.byref(cfg), _ptr(baseband), nbytes, res, _ptr(h_series), int(copy_all)))
         return [res[i] for i in range(n + (1 if cfg.signal_detect_sum_streams else 0))]
 
+    def process_block_dm_sweep_events(self, cfg: BlockConfig, baseband, nbytes: int, dms, max_events: int,
+                                      on_device: bool = False, h_series=None, d_spectrum=None):
+        """process_block_dm_sweep(outputs=True) that also lists every trial's events (srtb_b200_event): returns
+        (results, peaks, best_trial, h_series, d_spectrum, events, n_events), events[s] a numpy structured array of
+        stream s's first min(n_events[s], max_events) events"""
+        return self.process_block_dm_sweep(cfg, baseband, nbytes, dms, on_device, True, h_series, d_spectrum,
+                                           max_events=max_events)
+
     def process_block_dm_sweep(self, cfg: BlockConfig, baseband, nbytes: int, dms, on_device: bool = False,
-                               outputs: bool = False, h_series=None, d_spectrum=None):
+                               outputs: bool = False, h_series=None, d_spectrum=None, max_events=None):
         """one block, many trial DMs: returns results[dm_index][stream].
         outputs=True: returns (results, peaks, best_trial, h_series, d_spectrum) instead, where peaks = (snr, index),
         numpy arrays [n_dm][streams][n_boxcars] (n_boxcars = the most any trial used), best_trial = [streams] ints,
@@ -332,19 +374,51 @@ class Context:
         out.h_series = _ptr(h_series)
         for i, t in enumerate(d_spectrum):
             out.d_spectrum[i] = _ptr(t)
-        streams = self._ck(self.lib.srtb_b200_process_block_dm_sweep_ex(
-            self.h, C.byref(cfg), _ptr(baseband), nbytes, int(on_device), arr, n_dm, res, C.byref(out)))
+        if max_events is None:
+            streams = self._ck(self.lib.srtb_b200_process_block_dm_sweep_ex(
+                self.h, C.byref(cfg), _ptr(baseband), nbytes, int(on_device), arr, n_dm, res, C.byref(out)))
+        else:
+            ev = np.zeros(streams * max(max_events, 1), _dtype_of(Event))
+            n_ev = (C.c_uint64 * 4)()
+            streams = self._ck(self.lib.srtb_b200_process_block_dm_sweep_events(
+                self.h, C.byref(cfg), _ptr(baseband), nbytes, int(on_device), arr, n_dm, res, C.byref(out),
+                ev.ctypes.data, max_events, n_ev))
         results = [[res[j * streams + s] for s in range(streams)] for j in range(n_dm)]
         nb = max([r.n_boxcars for row in results for r in row] + [0])
         snr = np.array([[list(peaks[j * streams + s].snr)[:nb] for s in range(streams)] for j in range(n_dm)],
                        np.float32).reshape(n_dm, streams, nb)
         idx = np.array([[list(peaks[j * streams + s].peak_index)[:nb] for s in range(streams)] for j in range(n_dm)],
                        np.uint64).reshape(n_dm, streams, nb)
-        return results, (snr, idx), [int(best[s]) for s in range(streams)], h_series, list(d_spectrum)
+        if max_events is None:
+            return results, (snr, idx), [int(best[s]) for s in range(streams)], h_series, list(d_spectrum)
+        totals = [int(n_ev[s]) for s in range(streams)]
+        events = [ev[s * max_events:s * max_events + min(totals[s], max_events)].copy() for s in range(streams)]
+        return results, (snr, idx), [int(best[s]) for s in range(streams)], h_series, list(d_spectrum), events, totals
+
+    def incoherent_dm_search_events(self, d_spectrum, time_count: int, chan_count: int, time_reserved_count: int,
+                                    freq_low: float, bandwidth: float, sample_rate: float, dm: float, dms, snr: float,
+                                    channel_threshold: float, max_boxcar_length: int, max_events: int,
+                                    h_series=None):
+        """incoherent_dm_search that also lists every trial's events: returns (results, peaks, best_trial, h_series,
+        events, n_events), events a numpy structured array (srtb_b200_event) of the first min(n_events, max_events)"""
+        return self.incoherent_dm_search(d_spectrum, time_count, chan_count, time_reserved_count, freq_low, bandwidth,
+                                         sample_rate, dm, dms, snr, channel_threshold, max_boxcar_length, h_series,
+                                         max_events=max_events)
+
+    def series_events(self, d_series, boxcar_stride: int, trial_stride: int, results, max_events: int):
+        """the event pass on caller-owned float32 device series under the headers `results` (DetectResult per
+        record): returns (events, n_events), events a numpy structured array of the first min(n_events, max_events)"""
+        import numpy as np
+        hdr = (DetectResult * len(results))(*results)
+        ev = np.zeros(max(max_events, 1), _dtype_of(Event))
+        n = C.c_uint64()
+        self._ck(self.lib.srtb_b200_series_events(self.h, _ptr(d_series), boxcar_stride, trial_stride, hdr,
+                                                  len(results), ev.ctypes.data, max_events, C.byref(n)))
+        return ev[:min(n.value, max_events)].copy(), int(n.value)
 
     def incoherent_dm_search(self, d_spectrum, time_count: int, chan_count: int, time_reserved_count: int,
                              freq_low: float, bandwidth: float, sample_rate: float, dm: float, dms, snr: float,
-                             channel_threshold: float, max_boxcar_length: int, h_series=None):
+                             channel_threshold: float, max_boxcar_length: int, h_series=None, max_events=None):
         """semi-coherent DM search of one stream's [chan_count][time_count] complex64 dynamic spectrum (coherently
         dedispersed at dm) over the trial DMs `dms`. Returns (results, (snr, idx), best_trial, h_series): results[d] per
         trial, peaks as numpy arrays [n_dm][n_boxcars] (n_boxcars = the most any trial used), the best trial's index,
@@ -360,15 +434,26 @@ class Context:
             _, sp, sm = incoherent_shifts(chan_count, freq_low, bandwidth, sample_rate, dm, dms, table=False)
             T = max(time_count - time_reserved_count - sp - sm, 1)
             h_series = np.zeros((MAX_BOXCARS, T), np.float32)
-        self._ck(self.lib.srtb_b200_incoherent_dm_search(
-            self.h, _ptr(d_spectrum), time_count, chan_count, time_reserved_count, freq_low, bandwidth, sample_rate,
-            dm, arr, n_dm, snr, channel_threshold, max_boxcar_length, res, C.cast(peaks, C.c_void_p),
-            C.byref(best), _ptr(h_series)))
+        if max_events is None:
+            self._ck(self.lib.srtb_b200_incoherent_dm_search(
+                self.h, _ptr(d_spectrum), time_count, chan_count, time_reserved_count, freq_low, bandwidth,
+                sample_rate, dm, arr, n_dm, snr, channel_threshold, max_boxcar_length, res, C.cast(peaks, C.c_void_p),
+                C.byref(best), _ptr(h_series)))
+        else:
+            ev = np.zeros(max(max_events, 1), _dtype_of(Event))
+            n_ev = C.c_uint64()
+            self._ck(self.lib.srtb_b200_incoherent_dm_search_events(
+                self.h, _ptr(d_spectrum), time_count, chan_count, time_reserved_count, freq_low, bandwidth,
+                sample_rate, dm, arr, n_dm, snr, channel_threshold, max_boxcar_length, res, C.cast(peaks, C.c_void_p),
+                C.byref(best), _ptr(h_series), ev.ctypes.data, max_events, C.byref(n_ev)))
         results = [res[d] for d in range(n_dm)]
         nb = max([r.n_boxcars for r in results] + [0])
         snr_a = np.array([list(peaks[d].snr)[:nb] for d in range(n_dm)], np.float32).reshape(n_dm, nb)
         idx_a = np.array([list(peaks[d].peak_index)[:nb] for d in range(n_dm)], np.uint64).reshape(n_dm, nb)
-        return results, (snr_a, idx_a), int(best.value), h_series
+        if max_events is None:
+            return results, (snr_a, idx_a), int(best.value), h_series
+        return (results, (snr_a, idx_a), int(best.value), h_series, ev[:min(n_ev.value, max_events)].copy(),
+                int(n_ev.value))
 
     def _submitted(self, cfg: BlockConfig, ticket: int) -> int:
         self._sum_tickets[ticket] = bool(cfg.signal_detect_sum_streams)
@@ -509,6 +594,24 @@ def nsamps_reserved(baseband_input_count: int, channel_count: int, freq_low: flo
                     sample_rate: float, dm: float, reserve_sample: bool) -> int:
     return int(load_library().srtb_b200_nsamps_reserved(baseband_input_count, channel_count, freq_low,
                                                          bandwidth, sample_rate, dm, int(reserve_sample)))
+
+
+def cluster_events(events, dms, max_candidates: int | None = None):
+    """friends-of-friends candidates of an event list (numpy structured array of Event's dtype) searched over the
+    trial DMs `dms` (srtb_b200_cluster_events). Returns (candidates, n_candidates): a numpy structured array
+    (Candidate's dtype) of the first min(n_candidates, max_candidates) candidates (all when max_candidates is None)"""
+    import numpy as np
+    lib = load_library()
+    ev = np.ascontiguousarray(events, dtype=_dtype_of(Event))
+    arr = (C.c_float * max(len(dms), 1))(*[float(d) for d in dms])
+    cap = len(ev) if max_candidates is None else max_candidates
+    out = np.zeros(max(cap, 1), _dtype_of(Candidate))
+    n = C.c_uint64()
+    rc = lib.srtb_b200_cluster_events(ev.ctypes.data if len(ev) else None, len(ev), arr, len(dms), out.ctypes.data,
+                                      cap, C.byref(n))
+    if rc != 0:
+        raise SrtbError(rc, lib.srtb_b200_last_error(None).decode())
+    return out[:min(n.value, cap)].copy(), int(n.value)
 
 
 def incoherent_shifts(chan_count: int, freq_low: float, bandwidth: float, sample_rate: float, dm: float, dms,
