@@ -64,6 +64,10 @@ struct configs {
   // with dm_list or incoherent_dm_list: also list each block's single-pulse candidates, every above-threshold run of
   // every trial and boxcar grouped friends-of-friends over DM, width and time (<prefix><counter>.<id>.candidates.csv)
   bool dm_search_candidates = false;
+  // the block path (no DM search): also list each block's single-pulse candidates at its one dm, every above-threshold
+  // run of every stream's boxcar series grouped friends-of-friends over width and time (<prefix><counter>.<id>.candidates
+  // .csv), and the total intensity's with signal_detect_sum_polarizations (<prefix><counter>.sum.candidates.csv)
+  bool signal_detect_candidates = false;
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

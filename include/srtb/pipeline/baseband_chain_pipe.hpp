@@ -108,28 +108,42 @@ inline uint64_t candidate_share(const srtb::work::write_signal_work& w) {
   return (w.first_sample != w.no_first_sample ? std::min(step, w.valid_samples) : step) / two_c;
 }
 
-/** dm_search_candidates: stream s's events (at most cap of the true total n_events) clustered into w's candidates; a
- *  warning names both counts when the cap cut the list */
-inline void attach_candidates(srtb::work::write_signal_work& w, const srtb_b200_event* events, uint64_t n_events,
-                              size_t cap, const std::vector<srtb::real>& dms, uint64_t sample_offset) {
+/** events (at most cap of the true total n_events) clustered into out; a warning names both counts, and `who`, when the
+ *  cap cut the list */
+inline void cluster_candidates(std::vector<srtb::work::dm_candidate>& out, const srtb_b200_event* events,
+                               uint64_t n_events, size_t cap, const std::vector<srtb::real>& dms,
+                               const std::string& who) {
   const size_t n = (size_t)std::min<uint64_t>(n_events, cap);
   if (n_events > cap)
-    SRTB_LOGW << " [dm_search_candidates] " << "stream " << w.data_stream_id << ": " << n_events
-              << " events, only the first " << cap << " clustered";
+    SRTB_LOGW << " [dm_search_candidates] " << who << ": " << n_events << " events, only the first " << cap
+              << " clustered";
   std::vector<srtb_b200_candidate> c(std::max<size_t>(n, 1));
   uint64_t n_c = 0;
   if (srtb_b200_cluster_events(events, n, dms.data(), dms.size(), c.data(), c.size(), &n_c) != 0)
     throw std::runtime_error(std::string{"[dm_search_candidates] "} + srtb_b200_last_error(nullptr));
+  for (size_t i = 0; i < std::min<uint64_t>(n_c, c.size()); i++)
+    out.push_back({c[i].snr, c[i].dm, c[i].dm_low, c[i].dm_high, c[i].boxcar_length, c[i].peak_index, c[i].window,
+                   c[i].members, c[i].span_begin, c[i].span_end, c[i].trial});
+}
+
+/** dm_search_candidates: stream s's events (at most cap of the true total n_events) clustered into w's candidates; a
+ *  warning names both counts when the cap cut the list */
+inline void attach_candidates(srtb::work::write_signal_work& w, const srtb_b200_event* events, uint64_t n_events,
+                              size_t cap, const std::vector<srtb::real>& dms, uint64_t sample_offset) {
+  cluster_candidates(w.candidates, events, n_events, cap, dms, "stream " + std::to_string(w.data_stream_id));
   w.has_candidates = true;
   w.candidate_share = candidate_share(w);
   w.candidate_sample_offset = sample_offset;
-  for (size_t i = 0; i < std::min<uint64_t>(n_c, c.size()); i++)
-    w.candidates.push_back({c[i].snr, c[i].dm, c[i].dm_low, c[i].dm_high, c[i].boxcar_length, c[i].peak_index,
-                            c[i].window, c[i].members, c[i].span_begin, c[i].span_end, c[i].trial});
 }
 
 /** events per stream and block a DM search lists for its candidates (dm_search_candidates) */
 constexpr size_t candidate_event_cap = (size_t)1 << 18;
+
+/** events per stream (and sum) and block the block path lists for its candidates (signal_detect_candidates): 2.5 MiB
+ *  of pinned list per detector and ring slot. A row of L' samples holds at most L'/2 runs, so a config #3 block
+ *  (L = 2^14, 9 boxcars) could exceed it only when most of its samples sit above threshold, i.e. on RFI; noise at the
+ *  configured threshold lists a handful. Above the cap the first events in (boxcar, begin) order are clustered. */
+constexpr size_t block_candidate_event_cap = (size_t)1 << 16;
 
 class baseband_chain_pipe {
  protected:
@@ -144,6 +158,8 @@ class baseband_chain_pipe {
     std::vector<std::shared_ptr<srtb::complex<srtb::real>>> d_spectrum;  // per stream: N + 2 floats, [C][L] when done
     std::shared_ptr<srtb::real> h_series;  // pinned [streams (+ 1 with the sum)][MAX_BOXCARS][L]
     bool sum = false;                       // signal_detect_sum_streams: the sum's result follows the streams'
+    bool events = false;                    // signal_detect_candidates: submitted through submit_block_events
+    srtb::real dm = 0;                      // the block's dm, which its candidates carry
   };
   std::deque<pending_block> pending;  // blocks in the pinned-host ring of this queue's context
   std::vector<srtb_b200_event> events;  // dm_search_candidates: one stream's events, reused
@@ -192,8 +208,15 @@ class baseband_chain_pipe {
     p.h_series = srtb::host_allocator.allocate_shared<srtb::real>((size_t)(p.streams + (p.sum ? 1 : 0)) *
                                                                   SRTB_B200_MAX_BOXCARS * p.L);
     outputs.h_series = p.h_series.get();
-    p.ticket = srtb_b200_submit_block_ex(q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(),
-                                         in_work.baseband_data.baseband_input_bytes, /*on_device=*/0, &outputs);
+    p.events = srtb::config.signal_detect_candidates;
+    p.dm = cfg.dm;
+    if (p.events)
+      p.ticket = srtb_b200_submit_block_events(q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(),
+                                               in_work.baseband_data.baseband_input_bytes, /*on_device=*/0, &outputs,
+                                               block_candidate_event_cap);
+    else
+      p.ticket = srtb_b200_submit_block_ex(q.ctx(), &cfg, in_work.baseband_data.baseband_ptr.get(),
+                                           in_work.baseband_data.baseband_input_bytes, /*on_device=*/0, &outputs);
     q.check(p.ticket);
     p.work = std::move(in_work);
     pending.push_back(std::move(p));
@@ -203,8 +226,14 @@ class baseband_chain_pipe {
     pending_block p = std::move(pending.front());
     pending.pop_front();
     srtb_b200_detect_result res[5];
-    const int n = srtb_b200_collect_block_ex(q.ctx(), p.ticket, res, nullptr, nullptr);
+    const srtb_b200_event* ev_list = nullptr;
+    uint64_t n_ev[5] = {0, 0, 0, 0, 0};
+    const int n = p.events ? srtb_b200_collect_block_events(q.ctx(), p.ticket, res, nullptr, nullptr, &ev_list, n_ev)
+                           : srtb_b200_collect_block_ex(q.ctx(), p.ticket, res, nullptr, nullptr);
     q.check(n);
+    // signal_detect_candidates: the slot's list is [streams (+1)][cap], clustered at the block's one DM
+    const std::vector<srtb::real> block_dm{p.dm};
+    constexpr size_t cap = block_candidate_event_cap;
     // fold_period: the block's fold, for the sink's accumulator (blocks not read from a file are not folded)
     std::shared_ptr<const srtb::work::fold_block> fold;
     if (srtb::config.fold_period != 0 && p.work.first_sample != p.work.no_first_sample) fold = fold_front(p);
@@ -231,6 +260,13 @@ class baseband_chain_pipe {
         w.sum_zero_count = res[n].zero_count;
         for (int b = 0; b < res[n].n_boxcars; b++) w.sum_signal_count.push_back(res[n].signal_count[b]);
         w.sum_time_series = positive_series(res[n], p.h_series, n, p.L);
+      }
+      if (p.events) {
+        attach_candidates(w, ev_list + (size_t)s * cap, n_ev[s], cap, block_dm, 0);
+        if (p.sum && s == 0) {
+          cluster_candidates(w.sum_candidates, ev_list + (size_t)n * cap, n_ev[n], cap, block_dm, "sum");
+          w.has_sum_candidates = true;
+        }
       }
       if (inc_dms.empty())
         w.time_series = positive_series(res[s], p.h_series, s, p.L);

@@ -7,7 +7,9 @@
 //   <prefix><counter>.<i>.npy        complex64 dynamic spectrum, shape {batch_size, count} (:209-246)
 //   <prefix><counter>.<boxcar>.tim   float32 time series per detected boxcar           (:249-280)
 // and, for a DM search (dm_list), <prefix><counter>.dm<DM>.<boxcar>.tim and <prefix><counter>.<id>.dm_sweep.csv.
-// With dm_search_candidates, also <prefix><counter>.<id>.candidates.csv: the block's single-pulse candidates.
+// With dm_search_candidates, also <prefix><counter>.<id>.candidates.csv: the block's single-pulse candidates. With
+// signal_detect_candidates the block path writes the same file at its one DM, and <prefix><counter>.sum.candidates.csv
+// for the total intensity (signal_detect_sum_polarizations).
 // With signal_detect_sum_polarizations, a block whose total intensity is positive keeps every stream's work, and the
 // first stream's work writes the sum's series as <prefix><counter>.sum.<boxcar>.tim (once per block).
 // counter = udp_packet_counter, or the timestamp when there is none (:145-148).
@@ -138,7 +140,12 @@ class write_signal_pipe {
       std::ofstream f(stem + ".sum." + std::to_string(ts.boxcar_length) + ".tim", std::ios::binary | std::ios::trunc);
       f.write(reinterpret_cast<const char*>(ts.h_time_series.get()), (std::streamsize)(ts.time_series_length * sizeof(srtb::real)));
     }
-    if (!sweep) return;
+    if (!sweep) {
+      // signal_detect_candidates: the block path's candidates, and the total intensity's on the first stream's work
+      if (w.has_candidates) write_candidates(w, stem);
+      if (w.has_sum_candidates) write_candidate_rows(w, w.sum_candidates, stem + ".sum.candidates.csv");
+      return;
+    }
     std::ofstream f(stem + "." + std::to_string(w.data_stream_id) + ".dm_sweep.csv", std::ios::trunc);
     f << "dm,detect_enabled,boxcar_length,series_length,signal_count,threshold,peak_snr,peak_index\n";
     for (const auto& t : w.dm_trials) {
@@ -155,8 +162,15 @@ class write_signal_pipe {
   /** <stem>.<data_stream_id>.candidates.csv: a header row, then one row per candidate in the block's own share, those
    *  whose window is below the work's candidate_share (candidate_share() in baseband_chain_pipe.hpp). sample = window +
    *  the work's offset (S- for the incoherent search), time = (first_sample + 2C sample) / sample_rate in seconds from
-   *  input_file_offset_bytes, topocentric and referred to f_c (empty without a first_sample). */
+   *  input_file_offset_bytes, topocentric and referred to f_c (empty without a first_sample). The block path
+   *  (signal_detect_candidates) writes the same columns: dm = dm_low = dm_high = the block's dm, trial 0. */
   static void write_candidates(const srtb::work::write_signal_work& w, const std::string& stem) {
+    write_candidate_rows(w, w.candidates, stem + "." + std::to_string(w.data_stream_id) + ".candidates.csv");
+  }
+
+  /** write_candidates' file of `candidates` at `path`, under w's share, offset, geometry and first sample */
+  static void write_candidate_rows(const srtb::work::write_signal_work& w,
+                                   const std::vector<srtb::work::dm_candidate>& candidates, const std::string& path) {
     auto fmt = [](const char* f, double v) {
       char buf[64];
       std::snprintf(buf, sizeof buf, f, v);
@@ -164,9 +178,9 @@ class write_signal_pipe {
     };
     const uint64_t two_c = 2 * (uint64_t)w.batch_size;
     const bool placed = w.first_sample != w.no_first_sample;
-    std::ofstream f(stem + "." + std::to_string(w.data_stream_id) + ".candidates.csv", std::ios::trunc);
+    std::ofstream f(path, std::ios::trunc);
     f << "snr,dm,boxcar_length,sample,time,members,dm_low,dm_high,span_begin,span_end,trial,peak_index\n";
-    for (const auto& c : w.candidates) {
+    for (const auto& c : candidates) {
       if (c.window >= w.candidate_share) continue;
       const uint64_t sample = c.window + w.candidate_sample_offset;
       const std::string time =
@@ -176,7 +190,7 @@ class write_signal_pipe {
         << c.members << "," << fmt("%g", c.dm_low) << "," << fmt("%g", c.dm_high) << "," << c.span_begin << ","
         << c.span_end << "," << c.trial << "," << c.peak_index << "\n";
     }
-    if (!f) SRTB_LOGE << " [write_signal_pipe] " << "cannot write " << stem << ".candidates.csv";
+    if (!f) SRTB_LOGE << " [write_signal_pipe] " << "cannot write " << path;
   }
 };
 

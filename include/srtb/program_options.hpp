@@ -239,7 +239,8 @@ inline const std::vector<std::string>& known_options() {
       "mitigate_rfi_spectral_kurtosis_threshold", "mitigate_rfi_freq_list", "spectrum_channel_count",
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length",
       "signal_detect_sum_polarizations", "fold_period", "fold_period_derivative", "fold_bin_count",
-      "fold_subband_count", "fold_subintegration_blocks", "fold_coherence", "dm_search_candidates"};
+      "fold_subband_count", "fold_subintegration_blocks", "fold_coherence", "dm_search_candidates",
+      "signal_detect_candidates"};
   return names;
 }
 
@@ -380,6 +381,7 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(fold_subintegration_blocks)
   SRTB_PARSE(fold_coherence)
   SRTB_PARSE(dm_search_candidates)
+  SRTB_PARSE(signal_detect_candidates)
   SRTB_PARSE(thread_query_work_wait_time)
   SRTB_PARSE(gui_enable)
   SRTB_PARSE(gui_pixmap_width)
@@ -409,6 +411,14 @@ inline void check_dm_search_candidates(const srtb::configs& config) {
   if (config.dm_search_candidates && trim(config.dm_list).empty() && trim(config.incoherent_dm_list).empty())
     throw std::invalid_argument("[program_options] dm_search_candidates needs a DM search: set dm_list (the coherent "
                                 "DM sweep) or incoherent_dm_list (the incoherent search around dm)");
+}
+
+/** signal_detect_candidates lists the block path's candidates; a DM search (dm_list, incoherent_dm_list) lists its own
+ *  through dm_search_candidates, so the two are not combined */
+inline void check_signal_detect_candidates(const srtb::configs& config) {
+  if (config.signal_detect_candidates && (!trim(config.dm_list).empty() || !trim(config.incoherent_dm_list).empty()))
+    throw std::invalid_argument("[program_options] signal_detect_candidates lists the candidates of the block path at "
+                                "its one dm; with dm_list or incoherent_dm_list set, use dm_search_candidates instead");
 }
 
 /** signal_detect_sum_polarizations adds the streams of a block: it needs two or more (`streams`, the format's count),

@@ -247,6 +247,9 @@ struct write_signal_work : public write_file_work {
   std::vector<dm_candidate> candidates;
   uint64_t candidate_share = 0;
   uint64_t candidate_sample_offset = 0;
+  // signal_detect_candidates with the total-intensity sum: the sum's candidates, on the first stream's work (same share)
+  bool has_sum_candidates = false;
+  std::vector<dm_candidate> sum_candidates;
   // fold_period: the block's fold (srtb_b200_fold), carried by the block's first stream
   std::shared_ptr<const fold_block> fold;
 };

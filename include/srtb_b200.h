@@ -443,6 +443,30 @@ typedef struct {
 } srtb_b200_candidate;
 int srtb_b200_cluster_events(const srtb_b200_event* h_events, size_t n_events, const float* h_dms, size_t n_dm,
                              srtb_b200_candidate* h_candidates, size_t max_candidates, uint64_t* n_candidates);
+/* Events of the block path: the ring (submit_block_ex / collect_block_ex) that also lists every single pulse of each
+ * block at its one DM. Everything submit_block_ex / collect_block_ex hand out is the same, bit for bit. In addition
+ * every stream's detector series is searched for events (the definition above) at the end of that stream's chain, on
+ * its lane, in stream order: one record of n_boxcars rows under the header the detector just wrote, read on the device.
+ * With signal_detect_sum_streams the sum's series is searched on the first lane after the sum's tail; its events carry
+ * stream = streams. Events carry trial = 0; indices are in the detector's series (spectrum sample = index, since the
+ * detector searches samples 0 .. L' - 1 of the block).
+ * Per detector (stream, and sum) two kernel launches and an 8-byte count copy, and a 256-byte memset of the lane's
+ * counts where the result headers are zeroed (at the head of a chain, never between two of its kernels); no host
+ * synchronisation. Every detector route of the block path feeds the pass (each ends in the detector's
+ * tail). The list crosses PCIe as it is written, into pinned memory the ring slot owns: a head of 256 bytes with the
+ * counts, then [streams (+1)][max_events] events (40 bytes each), grown by the ctx and kept like the slot's series.
+ * Each lane's device scratch holds 24 bytes per tile of 4096 samples of the rows of one detector.
+ *   submit: max_events above 2^32 returns SRTB_B200_E_INVALID before any launch; max_events == 0 lists counts only.
+ *   collect: n_events[streams (+1)] receives the true totals and *h_events the slot's list, [streams (+1)][max_events]
+ *            in (stream, boxcar, begin) order (the first max_events of each detector); valid until the slot is
+ *            submitted again. A null n_events, a null h_events when the block was submitted with max_events > 0, or a
+ *            ticket submitted through submit_block_ex returns SRTB_B200_E_INVALID and leaves the ticket to collect. */
+int srtb_b200_submit_block_events(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* baseband,
+                                  size_t baseband_bytes, int on_device, const srtb_b200_block_outputs* outputs,
+                                  size_t max_events);
+int srtb_b200_collect_block_events(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result* h_results,
+                                   const float** h_series, const void** d_spectrum, const srtb_b200_event** h_events,
+                                   uint64_t* n_events /* [streams (+1)] */);
 
 /* ---- folding at a known pulsar period --------------------------------------------------------------------------
  * Time of a spectrum sample. A block whose first baseband sample (per stream) is first_sample holds the spectrum

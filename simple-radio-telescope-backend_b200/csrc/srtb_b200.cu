@@ -35,6 +35,8 @@ static thread_local std::string g_last_error;
 
 // result headers per block: one per data stream (at most 4), then the total-intensity sum's (signal_detect_sum_streams)
 constexpr int RES_GROUP = 5, SUM_SLOT = 4;
+// head of a lane's block-path event scratch and of a slot's pinned event list: the counts [RES_GROUP] (and the ticket)
+constexpr size_t LANE_EV_HEAD = 256;
 
 // an allocation the context owns, device memory or (PINNED) pinned host memory, freed with its owner. grow() sizes it;
 // move-only, so a lane_state holding some stays swappable (lane_swap)
@@ -77,6 +79,9 @@ struct lane_state {
   // long waterfall rows: per-tile SK statistics of the last sweep, per-row zap flags
   buffer<float2> long_stats;
   buffer<unsigned char> long_zap;
+  // block-path events (srtb_b200_submit_block_events): the running event counts [RES_GROUP] and the count kernel's
+  // ticket at the head (LANE_EV_HEAD bytes), then the tile summaries and scan offsets of one detector's rows
+  buffer<char> ev_work;
 };
 
 struct srtb_b200_ctx {
@@ -125,6 +130,11 @@ struct srtb_b200_ctx {
   buffer<float, true> slot_h_series[SRTB_B200_RING_SLOTS];
   float* slot_out_spectrum[SRTB_B200_RING_SLOTS][4] = {};
   float* slot_out_series[SRTB_B200_RING_SLOTS] = {nullptr};
+  // per-slot event lists (submit_block_events): pinned, the counts [RES_GROUP] at the head, then [streams (+1)][max]
+  // events the emit kernel writes through; kept and grown by the ctx like slot_h_series
+  buffer<char, true> slot_ev[SRTB_B200_RING_SLOTS];
+  bool slot_events[SRTB_B200_RING_SLOTS] = {false};
+  size_t slot_max_events[SRTB_B200_RING_SLOTS] = {0};
   uint64_t submit_count = 0;
   // DM sweep working copy of the spectrum, per-trial result headers
   buffer<float2> sweep_buf;
@@ -2133,16 +2143,66 @@ static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* buf
                      cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length, /*zero_stride=*/1);
 }
 
+// ---- events of the block path (srtb_b200_submit_block_events): every detector's series of a block searched for
+// above-threshold runs (events.cuh) at the end of its own chain, on its lane, into the ring slot's pinned list. The
+// lane's scratch serves one detector at a time in stream order; the two lanes never share it.
+struct block_events {
+  char* list;         // the slot's pinned list: counts [RES_GROUP] at the head, then [streams (+1)][max_events] events
+  size_t max_events;
+  unsigned max_nb;    // boxcar rows per detector the launches cover
+  size_t tiles;       // tiles of EV_TILE samples per row of L
+};
+
+// the tile summaries of one detector's rows, then their scan offsets, after the lane scratch's head
+static size_t lane_ev_offsets_at(const block_events& ev) {
+  return LANE_EV_HEAD + (((size_t)ev.max_nb * ev.tiles * sizeof(ev_tile) + 255) & ~(size_t)255);
+}
+
+// zeroes the current lane's counts and ticket: at the head of a chain, never between two of its kernels
+static int lane_ev_zero(srtb_b200_ctx* ctx) {
+  CK(cudaMemsetAsync(ctx->lane.ev_work.p, 0, LANE_EV_HEAD, ctx->lane.stream));
+  return 0;
+}
+
+// the two event launches over n_rec records (rows as r describes them), counting from *count (the ticket zero), into
+// list (max_events per stream). Shared by the DM searches' scratch (events_enqueue) and the lanes' (lane_ev_enqueue).
+static int events_launch(srtb_b200_ctx* ctx, const ev_rows& r, size_t n_rec, ev_tile* tile, unsigned long long* offset,
+                         unsigned* ticket, unsigned long long* count, ev_event* list, size_t max_events) {
+  const dim3 grid((unsigned)r.tiles, r.max_nb, (unsigned)n_rec);
+  CK(launch(ctx, false, ev_count_kernel, grid, EV_THREADS, 0, r, tile, offset, ticket, count));
+  CK(launch(ctx, false, ev_emit_kernel, grid, EV_THREADS, 0, r, (const ev_tile*)tile, (const unsigned long long*)offset,
+            list, (unsigned long long)max_events));
+  return 0;
+}
+
+// after detector `slot` (a stream, or SUM_SLOT) has run on the current lane: its events, as list row `row` with
+// stream = row, and their count into the list's head
+static int lane_ev_enqueue(srtb_b200_ctx* ctx, const block_events& ev, int slot, size_t L, unsigned row) {
+  char* const w = ctx->lane.ev_work.p;
+  unsigned long long* const count = reinterpret_cast<unsigned long long*>(w) + slot;
+  unsigned* const ticket = reinterpret_cast<unsigned*>(w + RES_GROUP * sizeof(unsigned long long));
+  const ev_rows r{ctx->series[slot].p, L, 0, ctx->d_res + slot, ev.max_nb, ev.tiles, 0u, row};
+  ev_event* const list = reinterpret_cast<ev_event*>(ev.list + LANE_EV_HEAD) + (size_t)row * ev.max_events;
+  if (int rc = events_launch(ctx, r, 1, reinterpret_cast<ev_tile*>(w + LANE_EV_HEAD),
+                             reinterpret_cast<unsigned long long*>(w + lane_ev_offsets_at(ev)), ticket, count, list,
+                             ev.max_events))
+    return rc;
+  CK(cudaMemcpyAsync(reinterpret_cast<unsigned long long*>(ev.list) + row, count, sizeof(unsigned long long),
+                     cudaMemcpyDeviceToHost, ctx->lane.stream));
+  return 0;
+}
+
 // enqueue every stage of one block (no host sync); results land in ctx->h_res[res_base .. res_base + streams) once the
 // lanes reach their D2H copies. bufs[s]: working buffer of stream s (N + 2 floats, 16-byte aligned for the fused
 // routes), which holds the dynamic spectrum [C][L] when the block is done. host_series (optional): pinned host memory
 // that receives positive series. join_lanes: the first lane waits for the second at the end (process_block); the ring
 // leaves the lanes free-running (each copies its own result headers back, *alt_used tells the caller to record a
 // completion event on both). With cfg->signal_detect_sum_streams the first lane then waits for the second on the device
-// and runs sum_tail; its header lands in h_res[res_base + SUM_SLOT].
+// and runs sum_tail; its header lands in h_res[res_base + SUM_SLOT]. ev (the ring's events entry, or null): every
+// detector's events after its tail, on its lane (two launches and a count copy per stream, and per sum).
 static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* d_baseband, size_t baseband_bytes,
                          int res_base, float* const* bufs, float* host_series, bool join_lanes = true,
-                         bool* alt_used = nullptr) {
+                         bool* alt_used = nullptr, const block_events* ev = nullptr) {
   struct pdl_scope {  // launch reads ctx->pdl_auto; it is only meaningful inside this call
     srtb_b200_ctx* c;
     ~pdl_scope() { c->pdl_auto = false; }
@@ -2161,10 +2221,19 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
   if (alt_used) *alt_used = two_lanes;
   if (two_lanes) {
     if (int rc = ensure_alt_lane(ctx)) return rc;
-  } else {
+  }
+  if (ev) {
+    const size_t bytes = lane_ev_offsets_at(*ev) + (size_t)ev->max_nb * ev->tiles * sizeof(unsigned long long);
+    if (int rc = grow(ctx, ctx->lane.ev_work, bytes)) return rc;
+    if (two_lanes)
+      if (int rc = grow(ctx, ctx->alt.ev_work, bytes)) return rc;
+  }
+  if (!two_lanes) {
     // result headers zeroed before the first kernel (a memset between kernels would break the dependent-launch chain);
-    // with two lanes every stream zeroes its own header at the head of its chain, on its lane
+    // with two lanes every stream zeroes its own header at the head of its chain, on its lane. The event counts alike.
     CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result) * p.streams, ctx->lane.stream));
+    if (ev)
+      if (int rc = lane_ev_zero(ctx)) return rc;
   }
   block_input in{d_baseband, baseband_bytes, bufs};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
@@ -2173,7 +2242,11 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
   const bool sweep_order = r2c_sweep_order(p, in);
   auto enqueue_stream = [&](int s) -> int {
     float2* buf = reinterpret_cast<float2*>(bufs[s]);
-    if (two_lanes) CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
+    if (two_lanes) {
+      CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
+      if (ev)
+        if (int rc = lane_ev_zero(ctx)) return rc;
+    }
     const detect_out out{s, host_series ? host_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
                          raw ? raw + (size_t)s * p.L : nullptr, nullptr, /*header_zeroed=*/true};
     if (sweep_order) {
@@ -2199,6 +2272,8 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     const bool alt = two_lanes && (s & 1);
     if (alt) lane_swap(ctx);
     int rc = enqueue_stream(s);
+    // every route of stream_tail ends in detect_tail, which leaves series[s] and d_res[s] for the event pass
+    if (!rc && ev) rc = lane_ev_enqueue(ctx, *ev, s, p.L, (unsigned)s);
     if (!rc && two_lanes) {
       const cudaError_t e = cudaMemcpyAsync(ctx->h_res + res_base + s, ctx->d_res + s, sizeof(detect_dev_result),
                                             cudaMemcpyDeviceToHost, ctx->lane.stream);
@@ -2215,7 +2290,11 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     CK(cudaMemcpyAsync(ctx->h_res + res_base, ctx->d_res, sizeof(detect_dev_result) * p.streams, cudaMemcpyDeviceToHost,
                        ctx->lane.stream));
   if (sum) {
+    if (ev)  // the sum's chain head, next to sum_tail's header memset
+      if (int rc = lane_ev_zero(ctx)) return rc;
     if (int rc = sum_tail(ctx, p, bufs, raw, host_series)) return rc;
+    if (ev)
+      if (int rc = lane_ev_enqueue(ctx, *ev, SUM_SLOT, p.L, (unsigned)p.streams)) return rc;
     CK(cudaMemcpyAsync(ctx->h_res + res_base + SUM_SLOT, ctx->d_res + SUM_SLOT, sizeof(detect_dev_result),
                        cudaMemcpyDeviceToHost, ctx->lane.stream));
   }
@@ -2305,12 +2384,8 @@ static int events_prepare(srtb_b200_ctx* ctx, const char* who, size_t n_rec, uns
 
 // the two event launches over n_rec records (rows as r describes them), into stream r.stream's list
 static int events_enqueue(srtb_b200_ctx* ctx, const ev_scratch& sc, const ev_rows& r, size_t n_rec, size_t max_events) {
-  const dim3 grid((unsigned)sc.tiles, r.max_nb, (unsigned)n_rec);
   ev_event* list = reinterpret_cast<ev_event*>(ctx->ev_host.p + 256) + (size_t)r.stream * max_events;
-  CK(launch(ctx, false, ev_count_kernel, grid, EV_THREADS, 0, r, sc.tile, sc.offset, sc.ticket, sc.count + r.stream));
-  CK(launch(ctx, false, ev_emit_kernel, grid, EV_THREADS, 0, r, (const ev_tile*)sc.tile,
-            (const unsigned long long*)sc.offset, list, (unsigned long long)max_events));
-  return 0;
+  return events_launch(ctx, r, n_rec, sc.tile, sc.offset, sc.ticket, sc.count + r.stream, list, max_events);
 }
 
 // enqueued before the call's synchronisation: the streams' counts into the pinned list's head
@@ -3063,10 +3138,14 @@ extern "C" int srtb_b200_debug_set_submit_count(srtb_b200_ctx* ctx, uint64_t val
 // ---- pipelined ingest: the pinned-host ring of SURVEY section 8e -------------------------------
 // submit() copies block k on a dedicated copy stream while block k-1 computes; collect() waits for
 // one block's results. Up to SRTB_B200_RING_SLOTS blocks may be in flight.
-extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* baseband,
-                                         size_t baseband_bytes, int on_device, const srtb_b200_block_outputs* outputs) {
+// max_events (or null: the plain entry): list every detector's events into the slot's pinned list
+static int submit_ring(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* baseband,
+                       size_t baseband_bytes, int on_device, const srtb_b200_block_outputs* outputs,
+                       const size_t* max_events) {
   API_LOCK(ctx);
   if (!ctx || !cfg || !baseband) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: null argument");
+  if (max_events && *max_events > ((size_t)1 << 32))
+    return fail(ctx, SRTB_B200_E_INVALID, "submit_block_events: max_events above 2^32");
   CK(cudaSetDevice(ctx->device));
   const int slot = (int)(ctx->submit_count % SRTB_B200_RING_SLOTS);
   if (ctx->slot_busy[slot]) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: ring full, collect a block first");
@@ -3109,10 +3188,20 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
     CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->slot_h2d[slot], 0));
     d_baseband = ctx->slot_baseband[slot].p;
   }
+  block_events ev{};
+  if (max_events) {
+    const size_t rows = (size_t)p.streams + (cfg->signal_detect_sum_streams ? 1 : 0);
+    if (int rc = grow(ctx, ctx->slot_ev[slot], LANE_EV_HEAD + rows * std::max<size_t>(*max_events, 1) * sizeof(ev_event)))
+      return rc;
+    ev = block_events{ctx->slot_ev[slot].p, *max_events, boxcar_ctas(cfg->signal_detect_max_boxcar_length, p.L),
+                      std::max<size_t>(1, (p.L + EV_TILE - 1) / EV_TILE)};
+  }
   bool alt_used = false;
   if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, RES_GROUP * (1 + slot), bufs, h_series, /*join_lanes=*/false,
-                             &alt_used))
+                             &alt_used, max_events ? &ev : nullptr))
     return rc;
+  ctx->slot_events[slot] = max_events != nullptr;
+  ctx->slot_max_events[slot] = max_events ? *max_events : 0;
   ctx->slot_streams[slot] = p.streams;
   ctx->slot_sum[slot] = cfg->signal_detect_sum_streams != 0;
   CK(cudaEventRecord(ctx->slot_done[slot], ctx->lane.stream));
@@ -3130,6 +3219,17 @@ extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_blo
   return ticket;
 }
 
+extern "C" int srtb_b200_submit_block_ex(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const void* baseband,
+                                         size_t baseband_bytes, int on_device, const srtb_b200_block_outputs* outputs) {
+  return submit_ring(ctx, cfg, baseband, baseband_bytes, on_device, outputs, nullptr);
+}
+
+extern "C" int srtb_b200_submit_block_events(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
+                                             const void* baseband, size_t baseband_bytes, int on_device,
+                                             const srtb_b200_block_outputs* outputs, size_t max_events) {
+  return submit_ring(ctx, cfg, baseband, baseband_bytes, on_device, outputs, &max_events);
+}
+
 extern "C" int srtb_b200_submit_block(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg,
                                       const void* h_baseband, size_t baseband_bytes) {
   return srtb_b200_submit_block_ex(ctx, cfg, h_baseband, baseband_bytes, 0, nullptr);
@@ -3141,13 +3241,19 @@ extern "C" int srtb_b200_submit_block_device(srtb_b200_ctx* ctx, const srtb_b200
   return srtb_b200_submit_block_ex(ctx, cfg, d_baseband, baseband_bytes, 1, nullptr);
 }
 
-extern "C" int srtb_b200_collect_block_ex(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result* h_results,
-                                          const float** h_series, const void** d_spectrum) {
+// events (or false: the plain entry): the slot's event list and counts to h_events / n_events
+static int collect_ring(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result* h_results, const float** h_series,
+                        const void** d_spectrum, bool events, const srtb_b200_event** h_events, uint64_t* n_events) {
   API_LOCK(ctx);
-  if (!ctx || !h_results || ticket < 0) return fail(ctx, SRTB_B200_E_INVALID, "collect_block: bad argument");
+  if (!ctx || !h_results || ticket < 0 || (events && !n_events))
+    return fail(ctx, SRTB_B200_E_INVALID, "collect_block: bad argument");
   const int slot = ticket % SRTB_B200_RING_SLOTS;
   if (!ctx->slot_busy[slot] || ctx->slot_ticket[slot] != ticket)
     return fail(ctx, SRTB_B200_E_INVALID, "collect_block: nothing submitted under this ticket");
+  if (events && !ctx->slot_events[slot])
+    return fail(ctx, SRTB_B200_E_INVALID, "collect_block_events: the block was not submitted with submit_block_events");
+  if (events && !h_events && ctx->slot_max_events[slot] > 0)
+    return fail(ctx, SRTB_B200_E_INVALID, "collect_block_events: h_events is null and the block lists events");
   CK(cudaSetDevice(ctx->device));
   {
     const cudaEvent_t e0 = ctx->slot_done[slot], e1 = ctx->slot_alt_used[slot] ? ctx->slot_done_alt[slot] : nullptr;
@@ -3163,8 +3269,24 @@ extern "C" int srtb_b200_collect_block_ex(srtb_b200_ctx* ctx, int ticket, srtb_b
   if (h_series) *h_series = ctx->slot_out_series[slot];
   if (d_spectrum)
     for (int s = 0; s < 4; s++) d_spectrum[s] = s < streams ? ctx->slot_out_spectrum[slot][s] : nullptr;
+  if (events) {
+    const unsigned long long* counts = reinterpret_cast<const unsigned long long*>(ctx->slot_ev[slot].p);
+    for (int r = 0; r < streams + (ctx->slot_sum[slot] ? 1 : 0); r++) n_events[r] = counts[r];
+    if (h_events) *h_events = reinterpret_cast<const srtb_b200_event*>(ctx->slot_ev[slot].p + LANE_EV_HEAD);
+  }
   ctx->slot_busy[slot] = false;
   return streams;
+}
+
+extern "C" int srtb_b200_collect_block_ex(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result* h_results,
+                                          const float** h_series, const void** d_spectrum) {
+  return collect_ring(ctx, ticket, h_results, h_series, d_spectrum, false, nullptr, nullptr);
+}
+
+extern "C" int srtb_b200_collect_block_events(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result* h_results,
+                                              const float** h_series, const void** d_spectrum,
+                                              const srtb_b200_event** h_events, uint64_t* n_events) {
+  return collect_ring(ctx, ticket, h_results, h_series, d_spectrum, true, h_events, n_events);
 }
 
 extern "C" int srtb_b200_collect_block(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result* h_results) {

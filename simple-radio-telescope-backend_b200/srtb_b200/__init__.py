@@ -16,6 +16,7 @@ LIB_PATH = _HERE.parent / "csrc" / os.environ.get("SRTB_B200_LIB", "libsrtb_b200
 FORMAT_SIMPLE, FORMAT_INTERLEAVED_2, FORMAT_NAOCPSR_SNAP1, FORMAT_GZNUPSR_A1_2, FORMAT_GZNUPSR_A1_4 = range(5)
 WINDOW_RECTANGLE, WINDOW_HANN, WINDOW_HAMMING = range(3)
 MAX_BOXCARS = 32
+RING_SLOTS = 3  # SRTB_B200_RING_SLOTS: blocks the ring keeps in flight
 
 # names follow the reference's registry (io/backend_registry.hpp:36-181; unpack_pipe.hpp:392-413)
 FORMAT_BY_NAME = {
@@ -182,6 +183,9 @@ SYMBOLS = {
     "srtb_b200_process_block_dm_sweep_events": (_I, [_P, _P, _P, _SZ, _I, C.POINTER(C.c_float), _SZ,
                                                      C.POINTER(DetectResult), _P, _P, _SZ, C.POINTER(C.c_uint64)]),
     "srtb_b200_cluster_events": (_I, [_P, _SZ, C.POINTER(C.c_float), _SZ, _P, _SZ, C.POINTER(C.c_uint64)]),
+    "srtb_b200_submit_block_events": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ, _I, C.POINTER(BlockOutputs), _SZ]),
+    "srtb_b200_collect_block_events": (_I, [_P, _I, C.POINTER(DetectResult), C.POINTER(_P), C.POINTER(_P),
+                                            C.POINTER(_P), C.POINTER(C.c_uint64)]),
     "srtb_b200_fold_phase": (_I, [C.c_double, C.c_double, C.c_double, C.c_uint64, C.c_uint64,
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "srtb_b200_fold": (_I, [_P, C.POINTER(_P), _I, _SZ, _SZ, _SZ, C.c_double, C.c_double, C.c_double, _SZ, _SZ,
@@ -240,6 +244,7 @@ class Context:
         self.h = h
         self.device = device
         self._sum_tickets = {}  # ring ticket -> submitted with signal_detect_sum_streams
+        self._event_caps = {}  # ring ticket -> max_events of submit_block_events
 
     def close(self):
         if getattr(self, "h", None):
@@ -527,6 +532,47 @@ class Context:
         spec = (C.c_void_p * 4)()
         n = self._ck(self.lib.srtb_b200_collect_block_ex(self.h, ticket, res, C.byref(series), spec))
         return [res[i] for i in range(n + self._sum_result(ticket))], series.value, [spec[i] for i in range(n)]
+
+    def submit_block_events(self, cfg: BlockConfig, baseband, nbytes: int, max_events: int, on_device: bool = False,
+                            d_spectrum=None, h_series=None) -> int:
+        """submit_block_ex that also lists every detector's events (srtb_b200_event), at most max_events per stream
+        (and per sum)"""
+        out = BlockOutputs()
+        for i, t in enumerate(d_spectrum or []):
+            out.d_spectrum[i] = _ptr(t)
+        out.h_series = _ptr(h_series)
+        ticket = self._ck(self.lib.srtb_b200_submit_block_events(self.h, C.byref(cfg), _ptr(baseband), nbytes,
+                                                                  int(on_device), C.byref(out), max_events))
+        self._event_caps[ticket] = max_events
+        return self._submitted(cfg, ticket)
+
+    def collect_block_events(self, ticket: int):
+        """collect_block_ex's (results, series pointer, spectra) plus (events, n_events, sum_events, sum_n_events):
+        events[s] a numpy structured array (Event's dtype) of stream s's first min(n_events[s], max_events) events, a
+        copy of the slot's list; sum_events / sum_n_events the total intensity's (None / 0 without the sum)"""
+        import numpy as np
+        res = (DetectResult * 5)()
+        series = C.c_void_p()
+        spec = (C.c_void_p * 4)()
+        ev_p = C.c_void_p()
+        n_ev = (C.c_uint64 * 5)()
+        n = self._ck(self.lib.srtb_b200_collect_block_events(self.h, ticket, res, C.byref(series), spec,
+                                                              C.byref(ev_p), n_ev))
+        cap = self._event_caps.pop(ticket, 0)
+        rows = n + self._sum_result(ticket)
+        dt = _dtype_of(Event)
+        lists = []
+        for r in range(rows):
+            k = min(int(n_ev[r]), cap)
+            if k:
+                buf = (C.c_char * (k * dt.itemsize)).from_address(ev_p.value + r * cap * dt.itemsize)
+                lists.append(np.frombuffer(buf, dt, k).copy())
+            else:
+                lists.append(np.zeros(0, dt))
+        totals = [int(n_ev[r]) for r in range(rows)]
+        results = [res[i] for i in range(rows)]
+        sum_events, sum_total = (lists[n], totals[n]) if rows > n else (None, 0)
+        return (results, series.value, [spec[i] for i in range(n)], lists[:n], totals[:n], sum_events, sum_total)
 
     def debug_set_submit_count(self, value: int):
         self._ck(self.lib.srtb_b200_debug_set_submit_count(self.h, value))

@@ -232,6 +232,7 @@ int main(int argc, char** argv) {
         cfg, srtb::io::backend_registry::get_data_stream_count(cfg.baseband_format_type));
     srtb::program_options::check_fold(cfg);
     srtb::program_options::check_dm_search_candidates(cfg);
+    srtb::program_options::check_signal_detect_candidates(cfg);
   } catch (const std::exception& e) {
     std::fprintf(stderr, "srtb_b200: %s\n", e.what());
     return 2;
