@@ -98,6 +98,26 @@ inline std::vector<srtb::work::time_series_holder> positive_series(const srtb_b2
   return out;
 }
 
+/** one summary per trial of stream s: results and peaks are [n_dm][stride] (stride: the DM sweep's streams, 1 for the
+ *  incoherent search) */
+inline std::vector<srtb::work::dm_trial_summary> dm_trials(const srtb_b200_detect_result* results,
+                                                           const srtb_b200_peak* peaks,
+                                                           const std::vector<srtb::real>& dms, size_t stride, int s) {
+  std::vector<srtb::work::dm_trial_summary> out;
+  for (size_t j = 0; j < dms.size(); j++) {
+    const srtb_b200_detect_result& t = results[j * stride + s];
+    const srtb_b200_peak& pk = peaks[j * stride + s];
+    srtb::work::dm_trial_summary d;
+    d.dm = dms[j];
+    d.detect_enabled = t.detect_enabled != 0;
+    for (int b = 0; b < t.n_boxcars; b++)
+      d.boxcars.push_back({t.boxcar_length[b], t.series_length[b], t.signal_count[b], t.threshold[b], pk.snr[b],
+                           pk.peak_index[b]});
+    out.push_back(std::move(d));
+  }
+  return out;
+}
+
 /** the block's own share of candidate windows (series indices): min(step, valid_samples) / 2C, step = fold_block_step(),
  *  or step / 2C for a block without a first_sample (UDP). Consecutive blocks start step samples apart, so a pulse in the
  *  coherent sweep's overlap is listed by one block only; the incoherent search's series are step / 2C long, so it keeps
@@ -342,15 +362,7 @@ class baseband_chain_pipe {
     const srtb_b200_detect_result& r = tr[best];
     w.time_series = positive_series(r, h_inc, s, p.L, r.time_series_count);
     w.dm = dms[best];
-    for (size_t j = 0; j < n_dm; j++) {
-      srtb::work::dm_trial_summary d;
-      d.dm = dms[j];
-      d.detect_enabled = tr[j].detect_enabled != 0;
-      for (int b = 0; b < tr[j].n_boxcars; b++)
-        d.boxcars.push_back({tr[j].boxcar_length[b], tr[j].series_length[b], tr[j].signal_count[b],
-                             tr[j].threshold[b], peaks[j].snr[b], peaks[j].peak_index[b]});
-      w.dm_trials.push_back(std::move(d));
-    }
+    w.dm_trials = dm_trials(tr.data(), peaks.data(), dms, 1, 0);
   }
 };
 

@@ -85,17 +85,7 @@ class dm_sweep_chain_pipe {
       w.ptr = d_spectrum[s];
       w.time_series = positive_series(r, h_series, s, L);
       w.dm = dms[best[s]];
-      for (size_t j = 0; j < n_dm; j++) {
-        const srtb_b200_detect_result& t = res[j * streams + s];
-        const srtb_b200_peak& pk = peaks[j * streams + s];
-        srtb::work::dm_trial_summary d;
-        d.dm = dms[j];
-        d.detect_enabled = t.detect_enabled != 0;
-        for (int b = 0; b < t.n_boxcars; b++)
-          d.boxcars.push_back({t.boxcar_length[b], t.series_length[b], t.signal_count[b], t.threshold[b], pk.snr[b],
-                               pk.peak_index[b]});
-        w.dm_trials.push_back(std::move(d));
-      }
+      w.dm_trials = dm_trials(res.data(), peaks.data(), dms, (size_t)streams, s);
       if (candidates)
         attach_candidates(w, events.data() + (size_t)s * candidate_event_cap, n_events[s], candidate_event_cap, dms, 0);
       out.push_back(std::move(w));

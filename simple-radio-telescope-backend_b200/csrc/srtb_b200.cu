@@ -35,8 +35,12 @@ static thread_local std::string g_last_error;
 
 // result headers per block: one per data stream (at most 4), then the total-intensity sum's (signal_detect_sum_streams)
 constexpr int RES_GROUP = 5, SUM_SLOT = 4;
-// head of a lane's block-path event scratch and of a slot's pinned event list: the counts [RES_GROUP] (and the ticket)
-constexpr size_t LANE_EV_HEAD = 256;
+// the device's records are the ABI's structs, copied byte for byte
+static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
+static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
+static_assert(sizeof(ev_event) == sizeof(srtb_b200_event) && sizeof(ev_event) == 40, "event layout");
+// head of a lane's event scratch and of a pinned event list: the counts [RES_GROUP] (and the scratch's ticket)
+constexpr size_t EV_HEAD = 256;
 
 // an allocation the context owns, device memory or (PINNED) pinned host memory, freed with its owner. grow() sizes it;
 // move-only, so a lane_state holding some stays swappable (lane_swap)
@@ -79,9 +83,44 @@ struct lane_state {
   // long waterfall rows: per-tile SK statistics of the last sweep, per-row zap flags
   buffer<float2> long_stats;
   buffer<unsigned char> long_zap;
-  // block-path events (srtb_b200_submit_block_events): the running event counts [RES_GROUP] and the count kernel's
-  // ticket at the head (LANE_EV_HEAD bytes), then the tile summaries and scan offsets of one detector's rows
+  // events (events.cuh): the running event counts [RES_GROUP] and the count kernel's ticket at the head (EV_HEAD
+  // bytes), then the tile summaries, scan offsets and uploaded headers of one pass (ev_scratch_for)
   buffer<char> ev_work;
+};
+
+// a pinned event list: the counts [RES_GROUP] in an EV_HEAD-byte head, then [rows][max_events] events the emit kernel
+// writes through
+struct ev_list {
+  char* p = nullptr;
+  size_t max_events = 0;
+  unsigned long long* counts() const { return reinterpret_cast<unsigned long long*>(p); }
+  ev_event* row(size_t r) const { return reinterpret_cast<ev_event*>(p + EV_HEAD) + r * max_events; }
+};
+
+// one block in flight on the pipelined ingest ring (submit_ring / collect_ring)
+struct ring_slot {
+  buffer<void> baseband;  // the block's host baseband, copied on the copy stream
+  cudaEvent_t h2d = nullptr, done = nullptr, done_alt = nullptr;  // done_alt: the second lane's completion of the block
+  int streams = 0, ticket = 0;
+  bool busy = false, alt_used = false, sum = false;  // sum: the block carries the total-intensity sum's header
+  // outputs: ctx-owned working buffers / pinned series unless the caller supplied its own (submit_block_ex)
+  buffer<float> stream_buf[4];
+  buffer<float, true> h_series;
+  float* out_spectrum[4] = {};
+  float* out_series = nullptr;
+  // events (submit_block_events): the pinned list [streams (+1)][max_events], kept and grown like h_series; list is
+  // into it, or {null, 0} when the block lists no events
+  buffer<char, true> ev;
+  ev_list list;
+};
+
+// what the incoherent search needs of (C, band, dm, trials): incoherent_plan_for
+struct incoherent_plan {
+  std::vector<int64_t> shifts;       // [n_dm][C]
+  uint64_t s_plus = 0, s_minus = 0;
+  std::vector<int> order;            // [n_dm] trial at each sorted position
+  std::vector<int2> groups, gspan;   // [groups] (first, count); [groups][C] (min, max) of a group's s + S-
+  unsigned spread = 0;               // largest max - min of any group and channel
 };
 
 struct srtb_b200_ctx {
@@ -109,7 +148,7 @@ struct srtb_b200_ctx {
   buffer<float> series[RES_GROUP];
   detect_dev_result* d_res = nullptr;  // RES_GROUP slots
   detect_dev_result* h_res = nullptr;  // pinned, RES_GROUP slots for process_block, then RES_GROUP per ring slot
-  size_t slot_time_count[RES_GROUP] = {};
+  size_t series_len[RES_GROUP] = {};  // time_count of the slot's last detector run: the row stride of its series
   // total-intensity sum: the streams' raw column sums [1 + RING_SLOTS][4][L] (group 0: process_block, 1 + slot: the
   // ring; slot-owned, so a lane's next block cannot overwrite what the sum of this one still reads), and the mask
   // kernel's output (mask float2[C], mismatched channels uint2[C], their count)
@@ -117,24 +156,7 @@ struct srtb_b200_ctx {
   buffer<float2> sum_mask;
   // pipelined ingest ring
   cudaStream_t copy_stream = nullptr;
-  buffer<void> slot_baseband[SRTB_B200_RING_SLOTS];
-  cudaEvent_t slot_h2d[SRTB_B200_RING_SLOTS] = {nullptr}, slot_done[SRTB_B200_RING_SLOTS] = {nullptr};
-  int slot_streams[SRTB_B200_RING_SLOTS] = {0};
-  bool slot_busy[SRTB_B200_RING_SLOTS] = {false};
-  cudaEvent_t slot_done_alt[SRTB_B200_RING_SLOTS] = {nullptr};  // second lane's completion of the slot's block
-  bool slot_alt_used[SRTB_B200_RING_SLOTS] = {false};
-  bool slot_sum[SRTB_B200_RING_SLOTS] = {false};  // the slot's block carries the total-intensity sum's header
-  int slot_ticket[SRTB_B200_RING_SLOTS] = {0};
-  // per-slot outputs: ctx-owned working buffers / pinned series unless the caller supplied its own (submit_block_ex)
-  buffer<float> slot_stream_buf[SRTB_B200_RING_SLOTS][4];
-  buffer<float, true> slot_h_series[SRTB_B200_RING_SLOTS];
-  float* slot_out_spectrum[SRTB_B200_RING_SLOTS][4] = {};
-  float* slot_out_series[SRTB_B200_RING_SLOTS] = {nullptr};
-  // per-slot event lists (submit_block_events): pinned, the counts [RES_GROUP] at the head, then [streams (+1)][max]
-  // events the emit kernel writes through; kept and grown by the ctx like slot_h_series
-  buffer<char, true> slot_ev[SRTB_B200_RING_SLOTS];
-  bool slot_events[SRTB_B200_RING_SLOTS] = {false};
-  size_t slot_max_events[SRTB_B200_RING_SLOTS] = {0};
+  ring_slot ring[SRTB_B200_RING_SLOTS];
   uint64_t submit_count = 0;
   // DM sweep working copy of the spectrum, per-trial result headers
   buffer<float2> sweep_buf;
@@ -160,21 +182,19 @@ struct srtb_b200_ctx {
   buffer<float2> corr_rows;
   buffer<double2> corr_partial;
   unsigned* corr_tickets = nullptr;
-  // incoherent DM search: the shift tables of the last (geometry, dm, trial list), on the host and the device, and the
-  // per-trial series [n_dm][nb][T], scans [n_dm][T], result headers, peaks and tickets
-  std::vector<double> inc_key;
-  std::vector<int64_t> inc_shifts;  // [n_dm][C]
-  uint64_t inc_s_plus = 0, inc_s_minus = 0;
-  std::vector<int> inc_off, inc_order;            // [C][n_dm] s + S- in sorted order; [n_dm] trial of each sorted slot
-  std::vector<int2> inc_gspan, inc_groups;        // [groups][C] (min, max) of a group's offsets; [groups] (first, count)
-  unsigned inc_spread = 0;                         // largest max - min of any group and channel
-  bool inc_tab_uploaded = false;
+  // incoherent DM search: the plan of the last (geometry, dm, trial list) and its key, the kernel's offsets [C][n_dm]
+  // (s + S- in sorted order) and whether inc_tab holds them; the device tables, and the per-trial series
+  // [n_dm][nb][T], scans [n_dm][T], result headers, peaks and tickets
+  struct {
+    std::vector<double> key;
+    incoherent_plan plan;
+    std::vector<int> off;
+    bool uploaded = false;
+  } inc;
   buffer<char> inc_tab, inc_work;
   // fold: the sorted bin plan, hits, profile and kept, and the per-CTA rows fold_finish_kernel adds (srtb_b200_fold)
   buffer<char> fold_work;
-  // events (events.cuh): tile summaries, scan offsets, per-stream event counts, ticket and uploaded headers on the
-  // device; the counts, then [streams][max_events] events in pinned memory the emit kernel writes through
-  buffer<char> ev_work;
+  // the DM searches' and series_events' event list (their scratch is the first lane's)
   buffer<char, true> ev_host;
 };
 
@@ -387,10 +407,10 @@ int srtb_b200_ctx_destroy(srtb_b200_ctx* ctx) {
   cudaFree(ctx->corr_tickets);
   if (ctx->lane_fork) cudaEventDestroy(ctx->lane_fork);
   if (ctx->lane_join) cudaEventDestroy(ctx->lane_join);
-  for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) {
-    if (ctx->slot_h2d[i]) cudaEventDestroy(ctx->slot_h2d[i]);
-    if (ctx->slot_done[i]) cudaEventDestroy(ctx->slot_done[i]);
-    if (ctx->slot_done_alt[i]) cudaEventDestroy(ctx->slot_done_alt[i]);
+  for (ring_slot& rs : ctx->ring) {
+    if (rs.h2d) cudaEventDestroy(rs.h2d);
+    if (rs.done) cudaEventDestroy(rs.done);
+    if (rs.done_alt) cudaEventDestroy(rs.done_alt);
   }
   if (ctx->copy_stream) cudaStreamDestroy(ctx->copy_stream);
   for (auto& ev : ctx->stat_ev)
@@ -1566,7 +1586,7 @@ static int detect_tail(srtb_b200_ctx* ctx, const detect_out& out, const float* p
   CK(launch(ctx, true, boxcar, boxcar_ctas(max_boxcar, ts_count), 1024, 0, ctx->series[slot].p, time_count,
             (const float*)ctx->lane.acc.p, ts_count, snr, ctx->d_res + slot, out.host_series, out.peak, (size_t)0,
             (size_t)0));
-  ctx->slot_time_count[slot] = time_count;
+  ctx->series_len[slot] = time_count;
   return 0;
 }
 
@@ -1755,10 +1775,9 @@ static int watfft_long_fused(srtb_b200_ctx* ctx, const detect_out& out, float2* 
 
 static int detect_collect(srtb_b200_ctx* ctx, int slot, srtb_b200_detect_result* h_result, float* h_series,
                           int copy_all) {
-  static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
   std::memcpy(h_result, ctx->h_res + slot, sizeof(srtb_b200_detect_result));
   if (h_series && h_result->detect_enabled) {
-    const size_t stride = ctx->slot_time_count[slot];
+    const size_t stride = ctx->series_len[slot];
     bool any = false;
     for (int b = 0; b < h_result->n_boxcars; b++) {
       if (copy_all || h_result->signal_count[b] > 0) {
@@ -1959,6 +1978,10 @@ struct block_params {
     return {(double)f_min, (double)df, 1.0 / (double)f_c, (double)f_c, (D * 1e6) * (double)dm,
             mean, cfg->mitigate_rfi_average_method_threshold, coef, 0};
   }
+  // row s (a stream, or the sum after the streams) of a block's pinned series [rows][MAX_BOXCARS][L], or null without
+  float* series_row(float* h_series, int s) const {
+    return h_series ? h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * L : nullptr;
+  }
 };
 
 static int block_params_for(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const char* who, block_params* p) {
@@ -2137,58 +2160,76 @@ static int sum_tail(srtb_b200_ctx* ctx, const block_params& p, float* const* buf
             (const unsigned*)n_mis, ctx->series[SUM_SLOT].p));
   // the tail counts the mask's zeros (stride 1): the union count. The first lane's ticket and scan buffer are free here:
   // its own stream's tail has finished in stream order.
-  const detect_out out{SUM_SLOT, host_series ? host_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * L : nullptr,
-                       nullptr, nullptr, /*header_zeroed=*/true};
+  const detect_out out{SUM_SLOT, p.series_row(host_series, p.streams), nullptr, nullptr, /*header_zeroed=*/true};
   return detect_tail(ctx, out, nullptr, mask, L, C, ts, 0, cfg->signal_detect_signal_noise_threshold,
                      cfg->signal_detect_channel_threshold, cfg->signal_detect_max_boxcar_length, /*zero_stride=*/1);
 }
 
-// ---- events of the block path (srtb_b200_submit_block_events): every detector's series of a block searched for
-// above-threshold runs (events.cuh) at the end of its own chain, on its lane, into the ring slot's pinned list. The
-// lane's scratch serves one detector at a time in stream order; the two lanes never share it.
-struct block_events {
-  char* list;         // the slot's pinned list: counts [RES_GROUP] at the head, then [streams (+1)][max_events] events
-  size_t max_events;
-  unsigned max_nb;    // boxcar rows per detector the launches cover
-  size_t tiles;       // tiles of EV_TILE samples per row of L
+// ---- events: every above-threshold run of a detector's series (events.cuh), found by two launches that write into a
+// pinned ev_list through a lane's scratch. The block path (srtb_b200_submit_block_events) runs them at the end of every
+// detector's own chain, on its lane, into the ring slot's list; the DM searches and series_events run them on the
+// first lane into ctx->ev_host. A lane's scratch serves one pass at a time in stream order.
+struct ev_scratch {
+  unsigned long long* count;   // [RES_GROUP] running counts, at the head
+  unsigned* ticket;            // the count kernel's, at the head
+  ev_tile* tile;               // [n_rec][max_nb][tiles] tile summaries
+  unsigned long long* offset;  // their scan offsets
+  detect_dev_result* headers;  // uploaded headers
+  unsigned max_nb;             // boxcar rows per record the launches cover
+  size_t tiles;                // tiles of EV_TILE samples per row
 };
 
-// the tile summaries of one detector's rows, then their scan offsets, after the lane scratch's head
-static size_t lane_ev_offsets_at(const block_events& ev) {
-  return LANE_EV_HEAD + (((size_t)ev.max_nb * ev.tiles * sizeof(ev_tile) + 255) & ~(size_t)255);
+// lane l's scratch for n_rec records of max_nb rows of at most row_len samples, and n_headers uploaded headers: the
+// head (EV_HEAD bytes), the tile summaries, their offsets and the headers, each 256-byte aligned
+static int ev_scratch_for(srtb_b200_ctx* ctx, lane_state& l, const char* who, size_t n_rec, unsigned max_nb,
+                          size_t row_len, size_t n_headers, ev_scratch* sc) {
+  const size_t tiles = std::max<size_t>(1, (row_len + EV_TILE - 1) / EV_TILE);
+  const size_t nt = n_rec * max_nb * tiles;
+  if (n_rec > 65535 || tiles > 0x7fffffffu || nt >= ((size_t)1 << 32))
+    return fail(ctx, SRTB_B200_E_SIZE, std::string(who) + ": too many tiles for the event pass");
+  const size_t off_o = EV_HEAD + ((nt * sizeof(ev_tile) + 255) & ~(size_t)255);
+  const size_t hdr_o = off_o + ((nt * sizeof(unsigned long long) + 255) & ~(size_t)255);
+  if (int rc = grow(ctx, l.ev_work, hdr_o + n_headers * sizeof(detect_dev_result))) return rc;
+  char* const w = l.ev_work.p;
+  *sc = ev_scratch{reinterpret_cast<unsigned long long*>(w),
+                   reinterpret_cast<unsigned*>(w + RES_GROUP * sizeof(unsigned long long)),
+                   reinterpret_cast<ev_tile*>(w + EV_HEAD), reinterpret_cast<unsigned long long*>(w + off_o),
+                   reinterpret_cast<detect_dev_result*>(w + hdr_o), max_nb, tiles};
+  return 0;
 }
 
-// zeroes the current lane's counts and ticket: at the head of a chain, never between two of its kernels
-static int lane_ev_zero(srtb_b200_ctx* ctx) {
-  CK(cudaMemsetAsync(ctx->lane.ev_work.p, 0, LANE_EV_HEAD, ctx->lane.stream));
+// zeroes the scratch's counts and ticket on the current lane: at the head of a chain, never between two of its kernels
+static int ev_zero(srtb_b200_ctx* ctx, const ev_scratch& sc) {
+  CK(cudaMemsetAsync(sc.count, 0, EV_HEAD, ctx->lane.stream));
+  return 0;
+}
+
+// b holds a list of `rows` rows of max_events afterwards
+static int ev_list_for(srtb_b200_ctx* ctx, buffer<char, true>& b, size_t rows, size_t max_events, ev_list* list) {
+  if (int rc = grow(ctx, b, EV_HEAD + rows * std::max<size_t>(max_events, 1) * sizeof(ev_event))) return rc;
+  *list = ev_list{b.p, max_events};
   return 0;
 }
 
 // the two event launches over n_rec records (rows as r describes them), counting from *count (the ticket zero), into
-// list (max_events per stream). Shared by the DM searches' scratch (events_enqueue) and the lanes' (lane_ev_enqueue).
-static int events_launch(srtb_b200_ctx* ctx, const ev_rows& r, size_t n_rec, ev_tile* tile, unsigned long long* offset,
-                         unsigned* ticket, unsigned long long* count, ev_event* list, size_t max_events) {
+// list row r.stream
+static int events_enqueue(srtb_b200_ctx* ctx, const ev_scratch& sc, const ev_rows& r, size_t n_rec,
+                          unsigned long long* count, const ev_list& list) {
   const dim3 grid((unsigned)r.tiles, r.max_nb, (unsigned)n_rec);
-  CK(launch(ctx, false, ev_count_kernel, grid, EV_THREADS, 0, r, tile, offset, ticket, count));
-  CK(launch(ctx, false, ev_emit_kernel, grid, EV_THREADS, 0, r, (const ev_tile*)tile, (const unsigned long long*)offset,
-            list, (unsigned long long)max_events));
+  CK(launch(ctx, false, ev_count_kernel, grid, EV_THREADS, 0, r, sc.tile, sc.offset, sc.ticket, count));
+  CK(launch(ctx, false, ev_emit_kernel, grid, EV_THREADS, 0, r, (const ev_tile*)sc.tile,
+            (const unsigned long long*)sc.offset, list.row(r.stream), (unsigned long long)list.max_events));
   return 0;
 }
 
-// after detector `slot` (a stream, or SUM_SLOT) has run on the current lane: its events, as list row `row` with
-// stream = row, and their count into the list's head
-static int lane_ev_enqueue(srtb_b200_ctx* ctx, const block_events& ev, int slot, size_t L, unsigned row) {
-  char* const w = ctx->lane.ev_work.p;
-  unsigned long long* const count = reinterpret_cast<unsigned long long*>(w) + slot;
-  unsigned* const ticket = reinterpret_cast<unsigned*>(w + RES_GROUP * sizeof(unsigned long long));
-  const ev_rows r{ctx->series[slot].p, L, 0, ctx->d_res + slot, ev.max_nb, ev.tiles, 0u, row};
-  ev_event* const list = reinterpret_cast<ev_event*>(ev.list + LANE_EV_HEAD) + (size_t)row * ev.max_events;
-  if (int rc = events_launch(ctx, r, 1, reinterpret_cast<ev_tile*>(w + LANE_EV_HEAD),
-                             reinterpret_cast<unsigned long long*>(w + lane_ev_offsets_at(ev)), ticket, count, list,
-                             ev.max_events))
-    return rc;
-  CK(cudaMemcpyAsync(reinterpret_cast<unsigned long long*>(ev.list) + row, count, sizeof(unsigned long long),
-                     cudaMemcpyDeviceToHost, ctx->lane.stream));
+// after detector `slot` (a stream, or SUM_SLOT) has run on the current lane, whose scratch is sc: its events, as list
+// row `row` with stream = row, and their count into the list's head
+static int block_ev_enqueue(srtb_b200_ctx* ctx, const ev_scratch& sc, const ev_list& list, int slot, size_t L,
+                            unsigned row) {
+  const ev_rows r{ctx->series[slot].p, L, 0, ctx->d_res + slot, sc.max_nb, sc.tiles, 0u, row};
+  if (int rc = events_enqueue(ctx, sc, r, 1, sc.count + slot, list)) return rc;
+  CK(cudaMemcpyAsync(list.counts() + row, sc.count + slot, sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                     ctx->lane.stream));
   return 0;
 }
 
@@ -2198,11 +2239,11 @@ static int lane_ev_enqueue(srtb_b200_ctx* ctx, const block_events& ev, int slot,
 // that receives positive series. join_lanes: the first lane waits for the second at the end (process_block); the ring
 // leaves the lanes free-running (each copies its own result headers back, *alt_used tells the caller to record a
 // completion event on both). With cfg->signal_detect_sum_streams the first lane then waits for the second on the device
-// and runs sum_tail; its header lands in h_res[res_base + SUM_SLOT]. ev (the ring's events entry, or null): every
-// detector's events after its tail, on its lane (two launches and a count copy per stream, and per sum).
+// and runs sum_tail; its header lands in h_res[res_base + SUM_SLOT]. ev (the ring slot's list for the events entry, or
+// null): every detector's events after its tail, on its lane (two launches and a count copy per stream, and per sum).
 static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* d_baseband, size_t baseband_bytes,
                          int res_base, float* const* bufs, float* host_series, bool join_lanes = true,
-                         bool* alt_used = nullptr, const block_events* ev = nullptr) {
+                         bool* alt_used = nullptr, const ev_list* ev = nullptr) {
   struct pdl_scope {  // launch reads ctx->pdl_auto; it is only meaningful inside this call
     srtb_b200_ctx* c;
     ~pdl_scope() { c->pdl_auto = false; }
@@ -2222,18 +2263,19 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
   if (two_lanes) {
     if (int rc = ensure_alt_lane(ctx)) return rc;
   }
+  ev_scratch evs[2] = {};  // the first lane's event scratch, the second's: one detector's rows of L
   if (ev) {
-    const size_t bytes = lane_ev_offsets_at(*ev) + (size_t)ev->max_nb * ev->tiles * sizeof(unsigned long long);
-    if (int rc = grow(ctx, ctx->lane.ev_work, bytes)) return rc;
+    const unsigned max_nb = boxcar_ctas(p.cfg->signal_detect_max_boxcar_length, p.L);
+    if (int rc = ev_scratch_for(ctx, ctx->lane, "submit_block_events", 1, max_nb, p.L, 0, &evs[0])) return rc;
     if (two_lanes)
-      if (int rc = grow(ctx, ctx->alt.ev_work, bytes)) return rc;
+      if (int rc = ev_scratch_for(ctx, ctx->alt, "submit_block_events", 1, max_nb, p.L, 0, &evs[1])) return rc;
   }
   if (!two_lanes) {
     // result headers zeroed before the first kernel (a memset between kernels would break the dependent-launch chain);
     // with two lanes every stream zeroes its own header at the head of its chain, on its lane. The event counts alike.
     CK(cudaMemsetAsync(ctx->d_res, 0, sizeof(detect_dev_result) * p.streams, ctx->lane.stream));
     if (ev)
-      if (int rc = lane_ev_zero(ctx)) return rc;
+      if (int rc = ev_zero(ctx, evs[0])) return rc;
   }
   block_input in{d_baseband, baseband_bytes, bufs};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
@@ -2245,10 +2287,10 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     if (two_lanes) {
       CK(cudaMemsetAsync(ctx->d_res + s, 0, sizeof(detect_dev_result), ctx->lane.stream));
       if (ev)
-        if (int rc = lane_ev_zero(ctx)) return rc;
+        if (int rc = ev_zero(ctx, evs[s & 1])) return rc;
     }
-    const detect_out out{s, host_series ? host_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
-                         raw ? raw + (size_t)s * p.L : nullptr, nullptr, /*header_zeroed=*/true};
+    const detect_out out{s, p.series_row(host_series, s), raw ? raw + (size_t)s * p.L : nullptr, nullptr,
+                         /*header_zeroed=*/true};
     if (sweep_order) {
       {
         stage_scope stats_(ctx, SRTB_B200_STAGE_FUSED_R2C,
@@ -2273,7 +2315,7 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
     if (alt) lane_swap(ctx);
     int rc = enqueue_stream(s);
     // every route of stream_tail ends in detect_tail, which leaves series[s] and d_res[s] for the event pass
-    if (!rc && ev) rc = lane_ev_enqueue(ctx, *ev, s, p.L, (unsigned)s);
+    if (!rc && ev) rc = block_ev_enqueue(ctx, evs[alt], *ev, s, p.L, (unsigned)s);
     if (!rc && two_lanes) {
       const cudaError_t e = cudaMemcpyAsync(ctx->h_res + res_base + s, ctx->d_res + s, sizeof(detect_dev_result),
                                             cudaMemcpyDeviceToHost, ctx->lane.stream);
@@ -2291,12 +2333,46 @@ static int block_enqueue(srtb_b200_ctx* ctx, const block_params& p, const void* 
                        ctx->lane.stream));
   if (sum) {
     if (ev)  // the sum's chain head, next to sum_tail's header memset
-      if (int rc = lane_ev_zero(ctx)) return rc;
+      if (int rc = ev_zero(ctx, evs[0])) return rc;
     if (int rc = sum_tail(ctx, p, bufs, raw, host_series)) return rc;
     if (ev)
-      if (int rc = lane_ev_enqueue(ctx, *ev, SUM_SLOT, p.L, (unsigned)p.streams)) return rc;
+      if (int rc = block_ev_enqueue(ctx, evs[0], *ev, SUM_SLOT, p.L, (unsigned)p.streams)) return rc;
     CK(cudaMemcpyAsync(ctx->h_res + res_base + SUM_SLOT, ctx->d_res + SUM_SLOT, sizeof(detect_dev_result),
                        cudaMemcpyDeviceToHost, ctx->lane.stream));
+  }
+  return 0;
+}
+
+// the caller's spectra (d_spectrum of the block or sweep outputs, or null): given for every stream or for none, each
+// 16-byte aligned. *given: they are.
+static int caller_spectra(srtb_b200_ctx* ctx, const char* who, float* const* d_spectrum, int streams, bool* given) {
+  *given = d_spectrum && d_spectrum[0];
+  for (int s = 0; d_spectrum && s < streams; s++) {
+    if (!d_spectrum[s] == *given)
+      return fail(ctx, SRTB_B200_E_INVALID, std::string(who) + ": d_spectrum given for some streams only");
+    if (*given && !aligned16(d_spectrum[s]))
+      return fail(ctx, SRTB_B200_E_INVALID,
+                  std::string(who) + ": d_spectrum[" + std::to_string(s) + "] is not 16-byte aligned");
+  }
+  return 0;
+}
+
+// the block's baseband on the device: the caller's (on_device), else the host bytes copied into ctx->d_baseband on the
+// current lane
+static int device_baseband(srtb_b200_ctx* ctx, const void* baseband, size_t bytes, int on_device, const void** d) {
+  *d = baseband;
+  if (on_device) return 0;
+  if (int rc = grow(ctx, ctx->d_baseband, bytes)) return rc;
+  CK(cudaMemcpyAsync(ctx->d_baseband.p, baseband, bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
+  *d = ctx->d_baseband.p;
+  return 0;
+}
+
+// bufs[s]: stream s's working buffer of N + 2 floats from own[s] (the ctx's, or a ring slot's), grown for the block
+static int own_stream_bufs(srtb_b200_ctx* ctx, const block_params& p, buffer<float>* own, float** bufs) {
+  for (int s = 0; s < p.streams; s++) {
+    if (int rc = grow(ctx, own[s], (p.N + 2) * sizeof(float))) return rc;
+    bufs[s] = own[s].p;
   }
   return 0;
 }
@@ -2311,19 +2387,13 @@ extern "C" int srtb_b200_process_block_device(srtb_b200_ctx* ctx, const srtb_b20
   block_params p;
   if (int rc = block_params_for(ctx, cfg, "process_block", &p)) return rc;
   float* bufs[4] = {};
-  for (int s = 0; s < p.streams; s++) {
-    if (int rc = grow(ctx, ctx->stream_buf[s], (p.N + 2) * sizeof(float))) return rc;
-    bufs[s] = ctx->stream_buf[s].p;
-  }
+  if (int rc = own_stream_bufs(ctx, p, ctx->stream_buf, bufs)) return rc;
   if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, 0, bufs, nullptr)) return rc;
   CK(cudaStreamSynchronize(ctx->lane.stream));
   for (int s = 0; s < p.streams; s++)
-    if (int rc = detect_collect(ctx, s, h_results + s, h_series ? h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr,
-                                copy_all))
-      return rc;
+    if (int rc = detect_collect(ctx, s, h_results + s, p.series_row(h_series, s), copy_all)) return rc;
   if (cfg->signal_detect_sum_streams)
-    if (int rc = detect_collect(ctx, SUM_SLOT, h_results + p.streams,
-                                h_series ? h_series + (size_t)p.streams * SRTB_B200_MAX_BOXCARS * p.L : nullptr, copy_all))
+    if (int rc = detect_collect(ctx, SUM_SLOT, h_results + p.streams, p.series_row(h_series, p.streams), copy_all))
       return rc;
   return p.streams;
 }
@@ -2334,13 +2404,12 @@ extern "C" int srtb_b200_process_block(srtb_b200_ctx* ctx, const srtb_b200_block
   API_LOCK(ctx);
   if (!ctx || !cfg || !h_baseband) return fail(ctx, SRTB_B200_E_INVALID, "process_block: null argument");
   CK(cudaSetDevice(ctx->device));
-  if (int rc = grow(ctx, ctx->d_baseband, baseband_bytes)) return rc;
-  CK(cudaMemcpyAsync(ctx->d_baseband.p, h_baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
-  return srtb_b200_process_block_device(ctx, cfg, ctx->d_baseband.p, baseband_bytes, h_results, h_series, copy_all);
+  const void* d_baseband = nullptr;
+  if (int rc = device_baseband(ctx, h_baseband, baseband_bytes, /*on_device=*/0, &d_baseband)) return rc;
+  return srtb_b200_process_block_device(ctx, cfg, d_baseband, baseband_bytes, h_results, h_series, copy_all);
 }
 
 // ---- events: every above-threshold run of the detector's series (events.cuh) -----------------------------------------
-static_assert(sizeof(ev_event) == sizeof(srtb_b200_event) && sizeof(ev_event) == 40, "event layout");
 
 // where a DM search's events go: max_events per stream into h_events, the totals into n_events[streams]
 struct ev_request {
@@ -2349,60 +2418,28 @@ struct ev_request {
   uint64_t* n_events;
 };
 
-// the device scratch of the event launches of one call: tile summaries and offsets for n_rec records of max_nb rows of at
-// most row_len samples, the streams' running counts (zeroed) and the ticket, and room for n_headers uploaded headers;
-// the pinned list holds the counts, then max_events per stream. Grows before any launch of the call.
-struct ev_scratch {
-  ev_tile* tile;
-  unsigned long long* offset;
-  unsigned long long* count;  // [4]
-  unsigned* ticket;
-  detect_dev_result* headers;
-  size_t tiles;
-};
+// the event pass of one synchronous call, before any of its launches: the first lane's scratch (ev_scratch_for), with its
+// counts zeroed, and ctx->ev_host as the list of `streams` rows of max_events
 static int events_prepare(srtb_b200_ctx* ctx, const char* who, size_t n_rec, unsigned max_nb, size_t row_len,
-                          int streams, size_t max_events, size_t n_headers, ev_scratch* sc) {
-  sc->tiles = std::max<size_t>(1, (row_len + EV_TILE - 1) / EV_TILE);
-  const size_t nt = n_rec * max_nb * sc->tiles;
-  if (n_rec > 65535 || sc->tiles > 0x7fffffffu || nt >= ((size_t)1 << 32))
-    return fail(ctx, SRTB_B200_E_SIZE, std::string(who) + ": too many tiles for the event pass");
-  const size_t off_o = (nt * sizeof(ev_tile) + 255) & ~(size_t)255;
-  const size_t cnt_o = (off_o + nt * sizeof(unsigned long long) + 255) & ~(size_t)255;
-  const size_t hdr_o = cnt_o + 256;
-  if (int rc = grow(ctx, ctx->ev_work, hdr_o + n_headers * sizeof(detect_dev_result))) return rc;
-  const size_t list_b = 256 + (size_t)streams * std::max<size_t>(max_events, 1) * sizeof(ev_event);
-  if (int rc = grow(ctx, ctx->ev_host, list_b)) return rc;
-  char* w = ctx->ev_work.p;
-  sc->tile = reinterpret_cast<ev_tile*>(w);
-  sc->offset = reinterpret_cast<unsigned long long*>(w + off_o);
-  sc->count = reinterpret_cast<unsigned long long*>(w + cnt_o);
-  sc->ticket = reinterpret_cast<unsigned*>(w + cnt_o + 4 * sizeof(unsigned long long));
-  sc->headers = reinterpret_cast<detect_dev_result*>(w + hdr_o);
-  CK(cudaMemsetAsync(w + cnt_o, 0, 256, ctx->lane.stream));
-  return 0;
+                          int streams, size_t max_events, size_t n_headers, ev_scratch* sc, ev_list* list) {
+  if (int rc = ev_scratch_for(ctx, ctx->lane, who, n_rec, max_nb, row_len, n_headers, sc)) return rc;
+  if (int rc = ev_list_for(ctx, ctx->ev_host, (size_t)streams, max_events, list)) return rc;
+  return ev_zero(ctx, *sc);
 }
 
-// the two event launches over n_rec records (rows as r describes them), into stream r.stream's list
-static int events_enqueue(srtb_b200_ctx* ctx, const ev_scratch& sc, const ev_rows& r, size_t n_rec, size_t max_events) {
-  ev_event* list = reinterpret_cast<ev_event*>(ctx->ev_host.p + 256) + (size_t)r.stream * max_events;
-  return events_launch(ctx, r, n_rec, sc.tile, sc.offset, sc.ticket, sc.count + r.stream, list, max_events);
-}
-
-// enqueued before the call's synchronisation: the streams' counts into the pinned list's head
-static int events_fetch_counts(srtb_b200_ctx* ctx, const ev_scratch& sc, int streams) {
-  CK(cudaMemcpyAsync(ctx->ev_host.p, sc.count, streams * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+// enqueued before the call's synchronisation: the streams' counts into the list's head
+static int events_fetch_counts(srtb_b200_ctx* ctx, const ev_scratch& sc, const ev_list& list, int streams) {
+  CK(cudaMemcpyAsync(list.counts(), sc.count, streams * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
                      ctx->lane.stream));
   return 0;
 }
 
 // after the synchronisation: the counts and the written events to the caller
-static void events_collect(srtb_b200_ctx* ctx, int streams, const ev_request& ev) {
-  const unsigned long long* counts = reinterpret_cast<const unsigned long long*>(ctx->ev_host.p);
-  const ev_event* list = reinterpret_cast<const ev_event*>(ctx->ev_host.p + 256);
+static void events_collect(const ev_list& list, int streams, const ev_request& ev) {
   for (int s = 0; s < streams; s++) {
-    ev.n_events[s] = counts[s];
-    const size_t k = (size_t)std::min<unsigned long long>(counts[s], ev.max_events);
-    if (k) std::memcpy(ev.h_events + (size_t)s * ev.max_events, list + (size_t)s * ev.max_events, k * sizeof(ev_event));
+    ev.n_events[s] = list.counts()[s];
+    const size_t k = (size_t)std::min<unsigned long long>(list.counts()[s], ev.max_events);
+    if (k) std::memcpy(ev.h_events + (size_t)s * ev.max_events, list.row(s), k * sizeof(ev_event));
   }
 }
 
@@ -2437,18 +2474,19 @@ extern "C" int srtb_b200_series_events(srtb_b200_ctx* ctx, const float* d_series
   }
   CK(cudaSetDevice(ctx->device));
   ev_scratch sc;
-  if (int rc = events_prepare(ctx, "series_events", n_trials, std::max(max_nb, 1u), row_len, 1, max_events, n_trials, &sc))
+  ev_list list;
+  if (int rc = events_prepare(ctx, "series_events", n_trials, std::max(max_nb, 1u), row_len, 1, max_events, n_trials,
+                              &sc, &list))
     return rc;
-  static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
   CK(cudaMemcpyAsync(sc.headers, h_results, n_trials * sizeof(detect_dev_result), cudaMemcpyHostToDevice,
                      ctx->lane.stream));
   if (max_nb > 0) {
     const ev_rows r{d_series, boxcar_stride, trial_stride, sc.headers, max_nb, sc.tiles, 0u, 0u};
-    if (int rc = events_enqueue(ctx, sc, r, n_trials, max_events)) return rc;
+    if (int rc = events_enqueue(ctx, sc, r, n_trials, sc.count, list)) return rc;
   }
-  if (int rc = events_fetch_counts(ctx, sc, 1)) return rc;
+  if (int rc = events_fetch_counts(ctx, sc, list, 1)) return rc;
   CK(cudaStreamSynchronize(ctx->lane.stream));
-  events_collect(ctx, 1, ev);
+  events_collect(list, 1, ev);
   return 0;
 }
 
@@ -2618,28 +2656,13 @@ static int dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const
   CK(cudaSetDevice(ctx->device));
   block_params p;
   if (int rc = block_params_for(ctx, cfg, "dm_sweep", &p)) return rc;
-  const bool user_spec = outputs && outputs->d_spectrum[0];
-  if (outputs) {
-    for (int s = 0; s < p.streams; s++) {
-      if (user_spec && !outputs->d_spectrum[s])
-        return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum given for some streams only");
-      if (!user_spec && outputs->d_spectrum[s])
-        return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum given for some streams only");
-      if (user_spec && !aligned16(outputs->d_spectrum[s]))
-        return fail(ctx, SRTB_B200_E_INVALID, "dm_sweep: d_spectrum[" + std::to_string(s) + "] is not 16-byte aligned");
-    }
-  }
-  const void* d_baseband = baseband;
-  if (!on_device) {
-    if (int rc = grow(ctx, ctx->d_baseband, baseband_bytes)) return rc;
-    CK(cudaMemcpyAsync(ctx->d_baseband.p, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->lane.stream));
-    d_baseband = ctx->d_baseband.p;
-  }
+  bool user_spec = false;
+  if (int rc = caller_spectra(ctx, "dm_sweep", outputs ? outputs->d_spectrum : nullptr, p.streams, &user_spec))
+    return rc;
+  const void* d_baseband = nullptr;
+  if (int rc = device_baseband(ctx, baseband, baseband_bytes, on_device, &d_baseband)) return rc;
   float* bufs[4] = {};
-  for (int s = 0; s < p.streams; s++) {
-    if (int rc = grow(ctx, ctx->stream_buf[s], (p.N + 2) * sizeof(float))) return rc;
-    bufs[s] = ctx->stream_buf[s].p;
-  }
+  if (int rc = own_stream_bufs(ctx, p, ctx->stream_buf, bufs)) return rc;
   if (int rc = grow(ctx, ctx->sweep_buf, (p.Nc + 1) * sizeof(float2))) return rc;
   float2* W = ctx->sweep_buf.p;
   // every trial's result header is parked on the device and fetched once at the end: no host sync per trial. With
@@ -2657,9 +2680,10 @@ static int dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const
   if (outputs) CK(cudaMemsetAsync(d_peaks, 0, n_rec * sizeof(detect_dev_peak), ctx->lane.stream));
   // events: rows of at most L samples and boxcar_ctas(max, L) boxcars per trial, one trial per launch pair
   ev_scratch sc{};
+  ev_list list;
   const unsigned ev_nb = boxcar_ctas(cfg->signal_detect_max_boxcar_length, p.L);
   if (ev)
-    if (int rc = events_prepare(ctx, "dm_sweep", 1, ev_nb, p.L, p.streams, ev->max_events, 0, &sc)) return rc;
+    if (int rc = events_prepare(ctx, "dm_sweep", 1, ev_nb, p.L, p.streams, ev->max_events, 0, &sc, &list)) return rc;
   block_input in{d_baseband, baseband_bytes, bufs};
   if (int rc = block_input_init(ctx, p, &in)) return rc;
   for (int s = 0; s < p.streams; s++) {
@@ -2676,25 +2700,21 @@ static int dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const
                          ctx->lane.stream));
       if (ev) {  // the trial's series and header, before the next trial overwrites them
         const ev_rows r{ctx->series[0].p, p.L, 0, ctx->d_res, ev_nb, sc.tiles, (unsigned)j, (unsigned)s};
-        if (int rc = events_enqueue(ctx, sc, r, 1, ev->max_events)) return rc;
+        if (int rc = events_enqueue(ctx, sc, r, 1, sc.count + s, list)) return rc;
       }
     }
   }
   if (ev)
-    if (int rc = events_fetch_counts(ctx, sc, p.streams)) return rc;
-  static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
-  static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
+    if (int rc = events_fetch_counts(ctx, sc, list, p.streams)) return rc;
   CK(cudaMemcpyAsync(h_results, d_sweep, n_rec * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, ctx->lane.stream));
-  if (!outputs) {
-    CK(cudaStreamSynchronize(ctx->lane.stream));
-    if (ev) events_collect(ctx, p.streams, *ev);
-    return p.streams;
-  }
-  std::vector<detect_dev_peak> own_peaks(outputs->h_peaks ? 0 : n_rec);
-  detect_dev_peak* h_peaks = outputs->h_peaks ? reinterpret_cast<detect_dev_peak*>(outputs->h_peaks) : own_peaks.data();
-  CK(cudaMemcpyAsync(h_peaks, d_peaks, n_rec * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, ctx->lane.stream));
+  std::vector<detect_dev_peak> own_peaks(outputs && !outputs->h_peaks ? n_rec : 0);
+  detect_dev_peak* h_peaks =
+      outputs && outputs->h_peaks ? reinterpret_cast<detect_dev_peak*>(outputs->h_peaks) : own_peaks.data();
+  if (outputs)
+    CK(cudaMemcpyAsync(h_peaks, d_peaks, n_rec * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, ctx->lane.stream));
   CK(cudaStreamSynchronize(ctx->lane.stream));
-  if (ev) events_collect(ctx, p.streams, *ev);
+  if (ev) events_collect(list, p.streams, *ev);
+  if (!outputs) return p.streams;
   int best[4] = {0, 0, 0, 0};
   for (int s = 0; s < p.streams; s++) {
     best[s] = best_trial(h_results, h_peaks, n_dm, p.streams, s);
@@ -2704,7 +2724,7 @@ static int dm_sweep(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, const
   // the best trial once more per stream, from the kept spectrum: its spectrum to d_spectrum[s], its positive series
   // straight from the detector kernel to h_series' row of the stream, its header to h_res[s]
   for (int s = 0; s < p.streams; s++) {
-    const detect_out out{0, outputs->h_series ? outputs->h_series + (size_t)s * SRTB_B200_MAX_BOXCARS * p.L : nullptr};
+    const detect_out out{0, p.series_row(outputs->h_series, s)};
     float2* dst = user_spec ? reinterpret_cast<float2*>(outputs->d_spectrum[s]) : W;
     CK(cudaMemcpyAsync(ctx->lane.mean, d_means + s, sizeof(float), cudaMemcpyDeviceToDevice, ctx->lane.stream));
     if (int rc = stream_tail(ctx, p, out, dst, reinterpret_cast<float2*>(bufs[s]), h_dms[best[s]], /*phase_table=*/false))
@@ -2742,15 +2762,19 @@ extern "C" int srtb_b200_process_block_dm_sweep_events(srtb_b200_ctx* ctx, const
 // ---- incoherent DM search on one stream's dynamic spectrum (incoherent.cuh): every trial's series in one kernel, then
 // the detector's scan and boxcars batched over the trials, the best trial chosen on the host by best_trial().
 
-// s[d][c] = llround(K (DM_d - dm) (1/f(c)^2 - 1/f_ref^2) sample_rate / (2C)), f_ref = float(freq_low + bandwidth) (the
-// chirp's f_c), f(c) = freq_low + bandwidth (c + 0.5) / C, all in double; S+ / S- = max(0, max s) / max(0, -min s)
-static int incoherent_shift_table(size_t C, float freq_low, float bandwidth, float sample_rate, float dm,
-                                  const float* dms, size_t n_dm, std::vector<int64_t>* shifts, uint64_t* s_plus,
-                                  uint64_t* s_minus) {
+// the incoherent search's plan of (C, band, dm, trials). The shifts: s[d][c] = llround(K (DM_d - dm) (1/f(c)^2 -
+// 1/f_ref^2) sample_rate / (2C)), f_ref = float(freq_low + bandwidth) (the chirp's f_c), f(c) = freq_low + bandwidth
+// (c + 0.5) / C, all in double; S+ / S- = max(0, max s) / max(0, -min s). Then the trials sorted by DM (stable) and cut
+// greedily into groups of at most INC_GROUP whose spread over every channel is at most INC_SPREAD_MAX (a single trial
+// has none), so neighbouring trials share a group whatever order they came in. Returns SRTB_B200_E_INVALID for a shift
+// that is not finite, SRTB_B200_E_SIZE for one out of range.
+static int incoherent_plan_for(size_t C, float freq_low, float bandwidth, float sample_rate, float dm, const float* dms,
+                               size_t n_dm, incoherent_plan* pl) {
   constexpr double D = 4.148808e3;
   const double f_ref = (double)(float)(freq_low + bandwidth);
   const double scale = (double)sample_rate / (2.0 * (double)C);
-  shifts->assign(n_dm * C, 0);
+  std::vector<int64_t>& sh = pl->shifts;
+  sh.assign(n_dm * C, 0);
   int64_t hi = 0, lo = 0;
   for (size_t c = 0; c < C; c++) {
     const double f = (double)freq_low + (double)bandwidth * ((double)c + 0.5) / (double)C;
@@ -2759,52 +2783,29 @@ static int incoherent_shift_table(size_t C, float freq_low, float bandwidth, flo
       const double v = ((double)dms[d] - (double)dm) * k;
       if (!std::isfinite(v)) return SRTB_B200_E_INVALID;
       if (std::fabs(v) > 4.0e18) return SRTB_B200_E_SIZE;
-      const int64_t sh = std::llround(v);
-      (*shifts)[d * C + c] = sh;
-      hi = std::max(hi, sh);
-      lo = std::min(lo, sh);
+      const int64_t s = std::llround(v);
+      sh[d * C + c] = s;
+      hi = std::max(hi, s);
+      lo = std::min(lo, s);
     }
   }
-  *s_plus = (uint64_t)hi;
-  *s_minus = (uint64_t)(-lo);
-  return 0;
-}
-
-extern "C" int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, float bandwidth, float sample_rate,
-                                           float dm, const float* h_dms, size_t n_dm, int64_t* shifts,
-                                           uint64_t* s_plus, uint64_t* s_minus) {
-  if (chan_count == 0 || !h_dms || n_dm == 0)
-    return fail(nullptr, SRTB_B200_E_INVALID, "incoherent_shifts: bad argument");
-  std::vector<int64_t> tab;
-  uint64_t sp = 0, sm = 0;
-  if (int rc = incoherent_shift_table(chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm, &tab, &sp, &sm))
-    return fail(nullptr, rc, "incoherent_shifts: a shift is not finite or out of range");
-  if (shifts) std::memcpy(shifts, tab.data(), tab.size() * sizeof(int64_t));
-  if (s_plus) *s_plus = sp;
-  if (s_minus) *s_minus = sm;
-  return 0;
-}
-
-// the trials sorted by DM (stable) and cut greedily into groups of at most INC_GROUP whose spread over every channel is at
-// most INC_SPREAD_MAX (a single trial has none), so neighbouring trials share a group whatever order they came in.
-// sh: the shift table [n_dm][C]. order: trial of each sorted slot; groups: (first sorted slot, count); gspan:
-// [groups][C] (min, max) of s + S- over the group's trials; spread: the largest max - min of any group and channel.
-static void incoherent_grouping(const std::vector<int64_t>& sh, size_t C, const float* dms, size_t n_dm,
-                                int64_t s_minus, std::vector<int>* order, std::vector<int2>* groups,
-                                std::vector<int2>* gspan, unsigned* spread) {
-  order->resize(n_dm);
-  for (size_t d = 0; d < n_dm; d++) (*order)[d] = (int)d;
-  std::stable_sort(order->begin(), order->end(), [&](int a, int b) { return dms[a] < dms[b]; });
-  groups->clear();
-  gspan->clear();
-  *spread = 0;
+  pl->s_plus = (uint64_t)hi;
+  pl->s_minus = (uint64_t)(-lo);
+  const int64_t s_minus = -lo;
+  std::vector<int>& order = pl->order;
+  order.resize(n_dm);
+  for (size_t d = 0; d < n_dm; d++) order[d] = (int)d;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return dms[a] < dms[b]; });
+  pl->groups.clear();
+  pl->gspan.clear();
+  pl->spread = 0;
   std::vector<int64_t> gmin(C), gmax(C), nmin(C), nmax(C);
   size_t first = 0;
   while (first < n_dm) {
-    for (size_t c = 0; c < C; c++) gmin[c] = gmax[c] = sh[(size_t)(*order)[first] * C + c];
+    for (size_t c = 0; c < C; c++) gmin[c] = gmax[c] = sh[(size_t)order[first] * C + c];
     size_t count = 1;
     while (first + count < n_dm && count < (size_t)INC_GROUP) {
-      const size_t d = (size_t)(*order)[first + count];
+      const size_t d = (size_t)order[first + count];
       bool fits = true;
       for (size_t c = 0; c < C && fits; c++) {
         nmin[c] = std::min(gmin[c], sh[d * C + c]);
@@ -2816,13 +2817,28 @@ static void incoherent_grouping(const std::vector<int64_t>& sh, size_t C, const 
       gmax.swap(nmax);
       count++;
     }
-    groups->push_back(make_int2((int)first, (int)count));
+    pl->groups.push_back(make_int2((int)first, (int)count));
     for (size_t c = 0; c < C; c++) {
-      gspan->push_back(make_int2((int)(gmin[c] + s_minus), (int)(gmax[c] + s_minus)));
-      *spread = std::max(*spread, (unsigned)(gmax[c] - gmin[c]));
+      pl->gspan.push_back(make_int2((int)(gmin[c] + s_minus), (int)(gmax[c] + s_minus)));
+      pl->spread = std::max(pl->spread, (unsigned)(gmax[c] - gmin[c]));
     }
     first += count;
   }
+  return 0;
+}
+
+extern "C" int srtb_b200_incoherent_shifts(size_t chan_count, float freq_low, float bandwidth, float sample_rate,
+                                           float dm, const float* h_dms, size_t n_dm, int64_t* shifts,
+                                           uint64_t* s_plus, uint64_t* s_minus) {
+  if (chan_count == 0 || !h_dms || n_dm == 0)
+    return fail(nullptr, SRTB_B200_E_INVALID, "incoherent_shifts: bad argument");
+  incoherent_plan pl;
+  if (int rc = incoherent_plan_for(chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm, &pl))
+    return fail(nullptr, rc, "incoherent_shifts: a shift is not finite or out of range");
+  if (shifts) std::memcpy(shifts, pl.shifts.data(), pl.shifts.size() * sizeof(int64_t));
+  if (s_plus) *s_plus = pl.s_plus;
+  if (s_minus) *s_minus = pl.s_minus;
+  return 0;
 }
 
 extern "C" int srtb_b200_incoherent_groups(size_t chan_count, float freq_low, float bandwidth, float sample_rate,
@@ -2830,43 +2846,34 @@ extern "C" int srtb_b200_incoherent_groups(size_t chan_count, float freq_low, fl
                                            int32_t* gspan, uint64_t* n_groups, uint32_t* spread) {
   if (chan_count == 0 || !h_dms || n_dm == 0 || !n_groups)
     return fail(nullptr, SRTB_B200_E_INVALID, "incoherent_groups: bad argument");
-  std::vector<int64_t> tab;
-  uint64_t sp = 0, sm = 0;
-  if (int rc = incoherent_shift_table(chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm, &tab, &sp, &sm))
+  incoherent_plan pl;
+  if (int rc = incoherent_plan_for(chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm, &pl))
     return fail(nullptr, rc, "incoherent_groups: a shift is not finite or out of range");
-  std::vector<int> ord;
-  std::vector<int2> grp, gsp;
-  unsigned spr = 0;
-  incoherent_grouping(tab, chan_count, h_dms, n_dm, (int64_t)sm, &ord, &grp, &gsp, &spr);
-  *n_groups = grp.size();
-  if (order) std::memcpy(order, ord.data(), ord.size() * sizeof(int));
-  if (groups) std::memcpy(groups, grp.data(), grp.size() * sizeof(int2));
-  if (gspan) std::memcpy(gspan, gsp.data(), gsp.size() * sizeof(int2));
-  if (spread) *spread = spr;
+  *n_groups = pl.groups.size();
+  if (order) std::memcpy(order, pl.order.data(), pl.order.size() * sizeof(int));
+  if (groups) std::memcpy(groups, pl.groups.data(), pl.groups.size() * sizeof(int2));
+  if (gspan) std::memcpy(gspan, pl.gspan.data(), pl.gspan.size() * sizeof(int2));
+  if (spread) *spread = pl.spread;
   return 0;
 }
 
-// the shift tables of (C, band, dm, trials), cached: the host table, and the kernel's sorted offsets and groups
-// (incoherent_grouping)
+// the plan of (C, band, dm, trials), cached with the kernel's offsets s + S- in sorted order [C][n_dm]
 static int incoherent_tables(srtb_b200_ctx* ctx, size_t C, float freq_low, float bandwidth, float sample_rate,
                              float dm, const float* dms, size_t n_dm) {
   std::vector<double> key = {(double)C, freq_low, bandwidth, sample_rate, dm};
   key.reserve(key.size() + n_dm);  // no reallocating insert: g++ 13 warns falsely on it once this is inlined
   key.insert(key.end(), dms, dms + n_dm);
-  if (key == ctx->inc_key) return 0;
-  ctx->inc_key.clear();
-  if (int rc = incoherent_shift_table(C, freq_low, bandwidth, sample_rate, dm, dms, n_dm, &ctx->inc_shifts,
-                                      &ctx->inc_s_plus, &ctx->inc_s_minus))
+  if (key == ctx->inc.key) return 0;
+  ctx->inc.key.clear();
+  const incoherent_plan& pl = ctx->inc.plan;
+  if (int rc = incoherent_plan_for(C, freq_low, bandwidth, sample_rate, dm, dms, n_dm, &ctx->inc.plan))
     return fail(ctx, rc, "incoherent_dm_search: a shift is not finite or out of range");
-  const std::vector<int64_t>& sh = ctx->inc_shifts;
-  const int64_t s_minus = (int64_t)ctx->inc_s_minus;
-  const std::vector<int>& order = ctx->inc_order;
-  incoherent_grouping(sh, C, dms, n_dm, s_minus, &ctx->inc_order, &ctx->inc_groups, &ctx->inc_gspan, &ctx->inc_spread);
-  ctx->inc_off.resize(C * n_dm);
+  ctx->inc.off.resize(C * n_dm);
   for (size_t c = 0; c < C; c++)
-    for (size_t i = 0; i < n_dm; i++) ctx->inc_off[c * n_dm + i] = (int)(sh[(size_t)order[i] * C + c] + s_minus);
-  ctx->inc_tab_uploaded = false;
-  ctx->inc_key = std::move(key);
+    for (size_t i = 0; i < n_dm; i++)
+      ctx->inc.off[c * n_dm + i] = (int)(pl.shifts[(size_t)pl.order[i] * C + c] + (int64_t)pl.s_minus);
+  ctx->inc.uploaded = false;
+  ctx->inc.key = std::move(key);
   return 0;
 }
 
@@ -2890,18 +2897,19 @@ static int incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size
   CK(cudaSetDevice(ctx->device));
   if (int rc = incoherent_tables(ctx, chan_count, freq_low, bandwidth, sample_rate, dm, h_dms, n_dm)) return rc;
   const size_t ts = time_count - time_reserved_count;
-  const uint64_t span = ctx->inc_s_plus + ctx->inc_s_minus;
+  const incoherent_plan& pl = ctx->inc.plan;
+  const uint64_t span = pl.s_plus + pl.s_minus;
   if (span + 2 > ts)
     return fail(ctx, SRTB_B200_E_SIZE, "incoherent_dm_search: T = ts - S+ - S- = " +
                                            std::to_string((long long)ts - (long long)span) + " < 2");
   const size_t T = ts - span;
   const unsigned max_nb = boxcar_ctas(max_boxcar_length, T);
-  const size_t n_groups = ctx->inc_groups.size();
+  const size_t n_groups = pl.groups.size();
   // device tables: off [C][n_dm] int, order [n_dm] int, gspan [groups][C] int2, groups [groups] int2
   const size_t off_b = chan_count * n_dm * sizeof(int), order_b = n_dm * sizeof(int);
   const size_t gspan_o = (off_b + order_b + 15) & ~(size_t)15, gspan_b = n_groups * chan_count * sizeof(int2);
   const size_t groups_o = gspan_o + gspan_b, tab_b = groups_o + n_groups * sizeof(int2);
-  if (ctx->inc_tab.bytes < tab_b) ctx->inc_tab_uploaded = false;
+  if (ctx->inc_tab.bytes < tab_b) ctx->inc.uploaded = false;
   if (int rc = grow(ctx, ctx->inc_tab, tab_b)) return rc;
   // work: series [n_dm][max_nb][T], scans [n_dm][T], headers [n_dm], peaks [n_dm], tickets [n_dm]
   const size_t series_stride = (size_t)max_nb * T;
@@ -2912,8 +2920,10 @@ static int incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size
   const size_t work_b = ticket_o + n_dm * sizeof(unsigned);
   if (int rc = grow(ctx, ctx->inc_work, work_b)) return rc;
   ev_scratch sc{};
+  ev_list list;
   if (ev)
-    if (int rc = events_prepare(ctx, "incoherent_dm_search", n_dm, max_nb, T, 1, ev->max_events, 0, &sc)) return rc;
+    if (int rc = events_prepare(ctx, "incoherent_dm_search", n_dm, max_nb, T, 1, ev->max_events, 0, &sc, &list))
+      return rc;
   char* tab = ctx->inc_tab.p;
   char* work = ctx->inc_work.p;
   float* d_series = reinterpret_cast<float*>(work);
@@ -2922,15 +2932,15 @@ static int incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size
   detect_dev_peak* d_peak = reinterpret_cast<detect_dev_peak*>(work + peak_o);
   unsigned* d_ticket = reinterpret_cast<unsigned*>(work + ticket_o);
   cudaStream_t st = ctx->lane.stream;
-  if (!ctx->inc_tab_uploaded) {  // the host vectors live in the ctx, so the copies may complete after we return
-    CK(cudaMemcpyAsync(tab, ctx->inc_off.data(), off_b, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(tab + off_b, ctx->inc_order.data(), order_b, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(tab + gspan_o, ctx->inc_gspan.data(), gspan_b, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(tab + groups_o, ctx->inc_groups.data(), n_groups * sizeof(int2), cudaMemcpyHostToDevice, st));
-    ctx->inc_tab_uploaded = true;
+  if (!ctx->inc.uploaded) {  // the host vectors live in the ctx, so the copies may complete after we return
+    CK(cudaMemcpyAsync(tab, ctx->inc.off.data(), off_b, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tab + off_b, pl.order.data(), order_b, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tab + gspan_o, pl.gspan.data(), gspan_b, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(tab + groups_o, pl.groups.data(), n_groups * sizeof(int2), cudaMemcpyHostToDevice, st));
+    ctx->inc.uploaded = true;
   }
   CK(cudaMemsetAsync(work + res_o, 0, work_b - res_o, st));  // headers (zero_count is atomically added), peaks, tickets
-  const unsigned spread = ctx->inc_spread;
+  const unsigned spread = pl.spread;
   const size_t smem = incoherent_smem_bytes(spread);
   if (smem > 48 * 1024)  // once, for the largest spread any group may have
     if (int rc = set_smem_max(ctx, incoherent_dedisperse_kernel, incoherent_smem_bytes(INC_SPREAD_MAX))) return rc;
@@ -2948,17 +2958,15 @@ static int incoherent_dm_search(srtb_b200_ctx* ctx, const void* d_spectrum, size
             d_res, nullptr, d_peak, series_stride, T));
   if (ev) {
     const ev_rows r{d_series, T, series_stride, d_res, max_nb, sc.tiles, 0u, 0u};
-    if (int rc = events_enqueue(ctx, sc, r, n_dm, ev->max_events)) return rc;
-    if (int rc = events_fetch_counts(ctx, sc, 1)) return rc;
+    if (int rc = events_enqueue(ctx, sc, r, n_dm, sc.count, list)) return rc;
+    if (int rc = events_fetch_counts(ctx, sc, list, 1)) return rc;
   }
-  static_assert(sizeof(detect_dev_result) == sizeof(srtb_b200_detect_result), "result layout");
-  static_assert(sizeof(detect_dev_peak) == sizeof(srtb_b200_peak), "peak layout");
   std::vector<srtb_b200_peak> own_peaks(h_peaks ? 0 : n_dm);
   srtb_b200_peak* peaks = h_peaks ? h_peaks : own_peaks.data();
   CK(cudaMemcpyAsync(h_results, d_res, n_dm * sizeof(detect_dev_result), cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(peaks, d_peak, n_dm * sizeof(detect_dev_peak), cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  if (ev) events_collect(ctx, 1, *ev);
+  if (ev) events_collect(list, 1, *ev);
   const int best = best_trial(h_results, reinterpret_cast<const detect_dev_peak*>(peaks), n_dm, 1, 0);
   if (h_best_trial) *h_best_trial = best;
   if (!h_series) return 0;
@@ -3129,8 +3137,8 @@ static inline int ring_ticket(uint64_t submit_count) {
 extern "C" int srtb_b200_debug_set_submit_count(srtb_b200_ctx* ctx, uint64_t value) {
   API_LOCK(ctx);
   if (!ctx) return fail(nullptr, SRTB_B200_E_INVALID, "debug_set_submit_count: ctx is null");
-  for (int i = 0; i < SRTB_B200_RING_SLOTS; i++)
-    if (ctx->slot_busy[i]) return fail(ctx, SRTB_B200_E_INVALID, "debug_set_submit_count: ring not empty");
+  for (const ring_slot& rs : ctx->ring)
+    if (rs.busy) return fail(ctx, SRTB_B200_E_INVALID, "debug_set_submit_count: ring not empty");
   ctx->submit_count = value;
   return 0;
 }
@@ -3147,74 +3155,63 @@ static int submit_ring(srtb_b200_ctx* ctx, const srtb_b200_block_config* cfg, co
   if (max_events && *max_events > ((size_t)1 << 32))
     return fail(ctx, SRTB_B200_E_INVALID, "submit_block_events: max_events above 2^32");
   CK(cudaSetDevice(ctx->device));
-  const int slot = (int)(ctx->submit_count % SRTB_B200_RING_SLOTS);
-  if (ctx->slot_busy[slot]) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: ring full, collect a block first");
+  const int k = (int)(ctx->submit_count % SRTB_B200_RING_SLOTS);
+  ring_slot& rs = ctx->ring[k];
+  if (rs.busy) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: ring full, collect a block first");
   block_params p;
   if (int rc = block_params_for(ctx, cfg, "process_block", &p)) return rc;
-  if (!ctx->slot_done[slot])
-    for (int i = 0; i < SRTB_B200_RING_SLOTS; i++)
-      if (!ctx->slot_done[i]) CK(cudaEventCreateWithFlags(&ctx->slot_done[i], cudaEventDisableTiming));
+  if (!rs.done)
+    for (ring_slot& r : ctx->ring)
+      if (!r.done) CK(cudaEventCreateWithFlags(&r.done, cudaEventDisableTiming));
   // outputs: the caller's buffers (the work's own buffer, as in the reference) or this slot's ctx-owned ones
   float* bufs[4] = {nullptr, nullptr, nullptr, nullptr};
-  bool user_spec = outputs && outputs->d_spectrum[0];
+  bool user_spec = false;
+  if (int rc = caller_spectra(ctx, "submit_block", outputs ? outputs->d_spectrum : nullptr, p.streams, &user_spec))
+    return rc;
   if (user_spec) {
-    for (int s = 0; s < p.streams; s++) {
-      if (!outputs->d_spectrum[s]) return fail(ctx, SRTB_B200_E_INVALID, "submit_block: d_spectrum given for some streams only");
-      if (!aligned16(outputs->d_spectrum[s]))
-        return fail(ctx, SRTB_B200_E_INVALID, "submit_block: d_spectrum[" + std::to_string(s) + "] is not 16-byte aligned");
-      bufs[s] = outputs->d_spectrum[s];
-    }
-  } else {
-    for (int s = 0; s < p.streams; s++) {
-      if (int rc = grow(ctx, ctx->slot_stream_buf[slot][s], (p.N + 2) * sizeof(float))) return rc;
-      bufs[s] = ctx->slot_stream_buf[slot][s].p;
-    }
+    for (int s = 0; s < p.streams; s++) bufs[s] = outputs->d_spectrum[s];
+  } else if (int rc = own_stream_bufs(ctx, p, rs.stream_buf, bufs)) {
+    return rc;
   }
+  const size_t rows = (size_t)p.streams + (cfg->signal_detect_sum_streams ? 1 : 0);  // of the series and the events
   float* h_series = outputs ? outputs->h_series : nullptr;
   if (!h_series) {
-    const size_t need = (size_t)(p.streams + (cfg->signal_detect_sum_streams ? 1 : 0)) * SRTB_B200_MAX_BOXCARS * p.L;
-    if (int rc = grow(ctx, ctx->slot_h_series[slot], need * sizeof(float))) return rc;
-    h_series = ctx->slot_h_series[slot].p;
+    if (int rc = grow(ctx, rs.h_series, rows * SRTB_B200_MAX_BOXCARS * p.L * sizeof(float))) return rc;
+    h_series = rs.h_series.p;
   }
   const void* d_baseband = baseband;
   if (!on_device) {
     if (!ctx->copy_stream) {
       CK(cudaStreamCreateWithFlags(&ctx->copy_stream, cudaStreamNonBlocking));
-      for (int i = 0; i < SRTB_B200_RING_SLOTS; i++) CK(cudaEventCreateWithFlags(&ctx->slot_h2d[i], cudaEventDisableTiming));
+      for (ring_slot& r : ctx->ring) CK(cudaEventCreateWithFlags(&r.h2d, cudaEventDisableTiming));
     }
-    if (int rc = grow(ctx, ctx->slot_baseband[slot], baseband_bytes)) return rc;
-    CK(cudaMemcpyAsync(ctx->slot_baseband[slot].p, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
-    CK(cudaEventRecord(ctx->slot_h2d[slot], ctx->copy_stream));
-    CK(cudaStreamWaitEvent(ctx->lane.stream, ctx->slot_h2d[slot], 0));
-    d_baseband = ctx->slot_baseband[slot].p;
+    if (int rc = grow(ctx, rs.baseband, baseband_bytes)) return rc;
+    CK(cudaMemcpyAsync(rs.baseband.p, baseband, baseband_bytes, cudaMemcpyHostToDevice, ctx->copy_stream));
+    CK(cudaEventRecord(rs.h2d, ctx->copy_stream));
+    CK(cudaStreamWaitEvent(ctx->lane.stream, rs.h2d, 0));
+    d_baseband = rs.baseband.p;
   }
-  block_events ev{};
-  if (max_events) {
-    const size_t rows = (size_t)p.streams + (cfg->signal_detect_sum_streams ? 1 : 0);
-    if (int rc = grow(ctx, ctx->slot_ev[slot], LANE_EV_HEAD + rows * std::max<size_t>(*max_events, 1) * sizeof(ev_event)))
-      return rc;
-    ev = block_events{ctx->slot_ev[slot].p, *max_events, boxcar_ctas(cfg->signal_detect_max_boxcar_length, p.L),
-                      std::max<size_t>(1, (p.L + EV_TILE - 1) / EV_TILE)};
-  }
+  ev_list list;
+  if (max_events)
+    if (int rc = ev_list_for(ctx, rs.ev, rows, *max_events, &list)) return rc;
   bool alt_used = false;
-  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, RES_GROUP * (1 + slot), bufs, h_series, /*join_lanes=*/false,
-                             &alt_used, max_events ? &ev : nullptr))
+  if (int rc = block_enqueue(ctx, p, d_baseband, baseband_bytes, RES_GROUP * (1 + k), bufs, h_series, /*join_lanes=*/false,
+                             &alt_used, max_events ? &list : nullptr))
     return rc;
-  ctx->slot_events[slot] = max_events != nullptr;
-  ctx->slot_max_events[slot] = max_events ? *max_events : 0;
-  ctx->slot_streams[slot] = p.streams;
-  ctx->slot_sum[slot] = cfg->signal_detect_sum_streams != 0;
-  CK(cudaEventRecord(ctx->slot_done[slot], ctx->lane.stream));
-  ctx->slot_alt_used[slot] = alt_used;
+  rs.list = list;
+  rs.streams = p.streams;
+  rs.sum = cfg->signal_detect_sum_streams != 0;
+  CK(cudaEventRecord(rs.done, ctx->lane.stream));
+  rs.alt_used = alt_used;
   if (alt_used) {
-    if (!ctx->slot_done_alt[slot]) CK(cudaEventCreateWithFlags(&ctx->slot_done_alt[slot], cudaEventDisableTiming));
-    CK(cudaEventRecord(ctx->slot_done_alt[slot], ctx->alt.stream));
+    if (!rs.done_alt) CK(cudaEventCreateWithFlags(&rs.done_alt, cudaEventDisableTiming));
+    CK(cudaEventRecord(rs.done_alt, ctx->alt.stream));
   }
-  for (int s = 0; s < 4; s++) ctx->slot_out_spectrum[slot][s] = bufs[s];
-  ctx->slot_out_series[slot] = h_series;
-  ctx->slot_busy[slot] = true;
+  for (int s = 0; s < 4; s++) rs.out_spectrum[s] = bufs[s];
+  rs.out_series = h_series;
+  rs.busy = true;
   const int ticket = ring_ticket(ctx->submit_count);
-  ctx->slot_ticket[slot] = ticket;
+  rs.ticket = ticket;
   ctx->submit_count++;
   return ticket;
 }
@@ -3247,34 +3244,34 @@ static int collect_ring(srtb_b200_ctx* ctx, int ticket, srtb_b200_detect_result*
   API_LOCK(ctx);
   if (!ctx || !h_results || ticket < 0 || (events && !n_events))
     return fail(ctx, SRTB_B200_E_INVALID, "collect_block: bad argument");
-  const int slot = ticket % SRTB_B200_RING_SLOTS;
-  if (!ctx->slot_busy[slot] || ctx->slot_ticket[slot] != ticket)
+  const int k = ticket % SRTB_B200_RING_SLOTS;
+  ring_slot& rs = ctx->ring[k];
+  if (!rs.busy || rs.ticket != ticket)
     return fail(ctx, SRTB_B200_E_INVALID, "collect_block: nothing submitted under this ticket");
-  if (events && !ctx->slot_events[slot])
+  if (events && !rs.list.p)
     return fail(ctx, SRTB_B200_E_INVALID, "collect_block_events: the block was not submitted with submit_block_events");
-  if (events && !h_events && ctx->slot_max_events[slot] > 0)
+  if (events && !h_events && rs.list.max_events > 0)
     return fail(ctx, SRTB_B200_E_INVALID, "collect_block_events: h_events is null and the block lists events");
   CK(cudaSetDevice(ctx->device));
   {
-    const cudaEvent_t e0 = ctx->slot_done[slot], e1 = ctx->slot_alt_used[slot] ? ctx->slot_done_alt[slot] : nullptr;
+    const cudaEvent_t e0 = rs.done, e1 = rs.alt_used ? rs.done_alt : nullptr;
     api_lock_.unlock();  // the wait runs unlocked (a ticket is collected once, by one thread)
     CK(cudaEventSynchronize(e0));
     if (e1) CK(cudaEventSynchronize(e1));
     api_lock_.lock();
   }
-  const int streams = ctx->slot_streams[slot];
-  std::memcpy(h_results, ctx->h_res + RES_GROUP * (1 + slot), sizeof(srtb_b200_detect_result) * streams);
-  if (ctx->slot_sum[slot])
-    std::memcpy(h_results + streams, ctx->h_res + RES_GROUP * (1 + slot) + SUM_SLOT, sizeof(srtb_b200_detect_result));
-  if (h_series) *h_series = ctx->slot_out_series[slot];
+  const int streams = rs.streams;
+  const detect_dev_result* res = ctx->h_res + RES_GROUP * (1 + k);
+  std::memcpy(h_results, res, sizeof(srtb_b200_detect_result) * streams);
+  if (rs.sum) std::memcpy(h_results + streams, res + SUM_SLOT, sizeof(srtb_b200_detect_result));
+  if (h_series) *h_series = rs.out_series;
   if (d_spectrum)
-    for (int s = 0; s < 4; s++) d_spectrum[s] = s < streams ? ctx->slot_out_spectrum[slot][s] : nullptr;
+    for (int s = 0; s < 4; s++) d_spectrum[s] = s < streams ? rs.out_spectrum[s] : nullptr;
   if (events) {
-    const unsigned long long* counts = reinterpret_cast<const unsigned long long*>(ctx->slot_ev[slot].p);
-    for (int r = 0; r < streams + (ctx->slot_sum[slot] ? 1 : 0); r++) n_events[r] = counts[r];
-    if (h_events) *h_events = reinterpret_cast<const srtb_b200_event*>(ctx->slot_ev[slot].p + LANE_EV_HEAD);
+    for (int r = 0; r < streams + (rs.sum ? 1 : 0); r++) n_events[r] = rs.list.counts()[r];
+    if (h_events) *h_events = reinterpret_cast<const srtb_b200_event*>(rs.list.row(0));
   }
-  ctx->slot_busy[slot] = false;
+  rs.busy = false;
   return streams;
 }
 
