@@ -68,6 +68,10 @@ struct configs {
   // run of every stream's boxcar series grouped friends-of-friends over width and time (<prefix><counter>.<id>.candidates
   // .csv), and the total intensity's with signal_detect_sum_polarizations (<prefix><counter>.sum.candidates.csv)
   bool signal_detect_candidates = false;
+  // with signal_detect_candidates or dm_search_candidates: cut out the N highest-S/N candidates of each candidate file
+  // (0 = off): the dedispersed frequency-time image and the DM-time plane of each (<prefix><counter>.<id>.cutout_ft.npy,
+  // .cutout_dmt.npy, .cutouts.csv), from the block's spectra on the device; not with dm_list
+  int64_t candidate_cutouts = 0;
   std::vector<std::string> udp_receiver_address = {"10.0.1.2"};
   std::vector<unsigned short> udp_receiver_port = {12004};
   std::vector<uint32_t> udp_receiver_cpu_preferred = {0};

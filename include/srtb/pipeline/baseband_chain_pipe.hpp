@@ -9,6 +9,8 @@
 // Throughput across blocks: start several of these pipes on their own cuda_queue (one CUDA stream + context each)
 // popping from one MPMC work queue — blocks then alternate over contexts and overlap on the GPU.
 #pragma once
+#include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <deque>
@@ -156,6 +158,64 @@ inline void attach_candidates(srtb::work::write_signal_work& w, const srtb_b200_
   w.candidate_sample_offset = sample_offset;
 }
 
+/** candidate_cutouts' fixed geometry: W = n_rows = 256, nsub = the largest divisor of C up to 256 */
+constexpr size_t cutout_width = 256, cutout_rows = 256;
+inline size_t cutout_nsub(size_t C) {
+  for (size_t d = std::min<size_t>(C, 256); d > 1; d--)
+    if (C % d == 0) return d;
+  return 1;
+}
+
+/** max_c |k[c]|: the largest residual delay per unit DM over the band, in spectrum samples (k[c] as
+ *  srtb_b200_candidate_cutouts defines it, the same expression and order) */
+inline double cutout_k_max(size_t C, float freq_low, float bandwidth, float sample_rate) {
+  const double f_ref = (double)(float)(freq_low + bandwidth);
+  const double scale = (double)sample_rate / (2.0 * (double)C);
+  double k_max = 0;
+  for (size_t c = 0; c < C; c++) {
+    const double f = (double)freq_low + (double)bandwidth * ((double)c + 0.5) / (double)C;
+    k_max = std::max(k_max, std::fabs((1.0 / (f * f) - 1.0 / (f_ref * f_ref)) * scale * 4.148808e3));
+  }
+  return k_max;
+}
+
+/** the plane's DM half-width: (W/2) q / max_c |k[c]|, the DM offset whose residual sweep across the band fills half the
+ *  image, so the bow tie of a pulse at the candidate's DM spans the plane (0 for a band without dispersion) */
+inline float cutout_halfwidth(size_t W, uint32_t q, double k_max) {
+  return k_max > 0 ? (float)((double)(W / 2) * (double)q / k_max) : 0.f;
+}
+
+/** the rows of a candidate file (those below share, in file order) to cut out: the n highest-S/N, highest first, ties
+ *  in file order. Returns (row in the file, index into candidates) */
+inline std::vector<std::pair<uint64_t, size_t>> cutout_selection(const std::vector<srtb::work::dm_candidate>& candidates,
+                                                                 uint64_t share, size_t n) {
+  std::vector<std::pair<uint64_t, size_t>> rows;
+  for (size_t i = 0; i < candidates.size(); i++)
+    if (candidates[i].window < share) rows.push_back({rows.size(), i});
+  std::stable_sort(rows.begin(), rows.end(),
+                   [&](const auto& a, const auto& b) { return candidates[a.second].snr > candidates[b.second].snr; });
+  if (rows.size() > n) rows.resize(n);
+  return rows;
+}
+
+/** the cut-out requests of a selection: q = max(1, boxcar_length / 2), center = window + offset + boxcar_length / 2,
+ *  the candidate's DM, half-width by cutout_halfwidth */
+inline std::vector<srtb_b200_cutout_request> cutout_requests(const std::vector<srtb::work::dm_candidate>& candidates,
+                                                             const std::vector<std::pair<uint64_t, size_t>>& sel,
+                                                             uint64_t sample_offset, double k_max) {
+  std::vector<srtb_b200_cutout_request> out;
+  for (const auto& [row, i] : sel) {
+    const srtb::work::dm_candidate& c = candidates[i];
+    srtb_b200_cutout_request r{};
+    r.decimation = (uint32_t)std::max<uint64_t>(1, c.boxcar_length / 2);
+    r.center = (int64_t)(c.window + sample_offset + c.boxcar_length / 2);
+    r.dm = c.dm;
+    r.dm_halfwidth = cutout_halfwidth(cutout_width, r.decimation, k_max);
+    out.push_back(r);
+  }
+  return out;
+}
+
 /** events per stream and block a DM search lists for its candidates (dm_search_candidates) */
 constexpr size_t candidate_event_cap = (size_t)1 << 18;
 
@@ -283,9 +343,13 @@ class baseband_chain_pipe {
       }
       if (p.events) {
         attach_candidates(w, ev_list + (size_t)s * cap, n_ev[s], cap, block_dm, 0);
+        w.cutouts = cut_out(p, w, w.candidates, {s}, p.L - res[s].time_series_count);
         if (p.sum && s == 0) {
           cluster_candidates(w.sum_candidates, ev_list + (size_t)n * cap, n_ev[n], cap, block_dm, "sum");
           w.has_sum_candidates = true;
+          std::vector<int> all(p.streams);
+          for (int t = 0; t < p.streams; t++) all[t] = t;
+          w.sum_cutouts = cut_out(p, w, w.sum_candidates, all, p.L - res[n].time_series_count);
         }
       }
       if (inc_dms.empty())
@@ -294,6 +358,37 @@ class baseband_chain_pipe {
         incoherent_search(w, p, s, res[s], inc_dms, h_inc);
       out.push_back(std::move(w));
     }
+  }
+
+  /** candidate_cutouts: the cut-outs of the highest-S/N candidates of `candidates` (those below w's share) on the
+   *  spectra of `streams` (stream indices into p.d_spectrum), or null when the key is off or none is listed */
+  std::shared_ptr<const srtb::work::cutout_set> cut_out(const pending_block& p, const srtb::work::write_signal_work& w,
+                                                        const std::vector<srtb::work::dm_candidate>& candidates,
+                                                        const std::vector<int>& streams, size_t time_reserved_count) {
+    const int64_t N = srtb::config.candidate_cutouts;
+    if (N <= 0) return nullptr;
+    const auto sel = cutout_selection(candidates, w.candidate_share, (size_t)N);
+    if (sel.empty()) return nullptr;
+    const auto& cfg = holder.cfg;
+    const double k_max = cutout_k_max(p.C, cfg.baseband_freq_low, cfg.baseband_bandwidth, cfg.baseband_sample_rate);
+    const auto req = cutout_requests(candidates, sel, w.candidate_sample_offset, k_max);
+    auto out = std::make_shared<srtb::work::cutout_set>();
+    out->width = cutout_width;
+    out->nsub = cutout_nsub(p.C);
+    out->n_rows = cutout_rows;
+    out->ft.resize(req.size() * out->nsub * out->width);
+    out->dmt.resize(req.size() * out->n_rows * out->width);
+    std::vector<float> row_dms(req.size() * out->n_rows);
+    std::vector<const void*> spectra;
+    for (int s : streams) spectra.push_back(p.d_spectrum[s].get());
+    q.check(srtb_b200_candidate_cutouts(q.ctx(), spectra.data(), (int)spectra.size(), p.L, p.C, time_reserved_count,
+                                        cfg.baseband_freq_low, cfg.baseband_bandwidth, cfg.baseband_sample_rate,
+                                        cfg.dm, req.data(), req.size(), out->width, out->nsub, out->n_rows,
+                                        out->ft.data(), out->dmt.data(), row_dms.data()));
+    for (size_t i = 0; i < req.size(); i++)
+      out->rows.push_back({sel[i].first, req[i].center, req[i].decimation, row_dms[i * out->n_rows],
+                           row_dms[i * out->n_rows + out->n_rows - 1]});
+    return out;
   }
 
   /** folds the block's streams at fold_period: the first min(block step, samples read) / (2C) spectrum samples */
@@ -351,6 +446,7 @@ class baseband_chain_pipe {
       q.check(srtb_b200_incoherent_shifts(p.C, cfg.baseband_freq_low, cfg.baseband_bandwidth, cfg.baseband_sample_rate,
                                           cfg.dm, dms.data(), n_dm, nullptr, nullptr, &s_minus));
       attach_candidates(w, events.data(), n_events, events.size(), dms, s_minus);
+      w.cutouts = cut_out(p, w, w.candidates, {s}, p.L - block_res.time_series_count);
     } else {
       q.check(srtb_b200_incoherent_dm_search(
           q.ctx(), p.d_spectrum[s].get(), p.L, p.C, p.L - block_res.time_series_count, cfg.baseband_freq_low,

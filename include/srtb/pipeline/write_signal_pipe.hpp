@@ -10,6 +10,9 @@
 // With dm_search_candidates, also <prefix><counter>.<id>.candidates.csv: the block's single-pulse candidates. With
 // signal_detect_candidates the block path writes the same file at its one DM, and <prefix><counter>.sum.candidates.csv
 // for the total intensity (signal_detect_sum_polarizations).
+// With candidate_cutouts = N, beside each candidate file: <stem>.<id>.cutout_ft.npy and .cutout_dmt.npy (float32
+// [N'][nsub][W] and [N'][n_rows][W]) and <stem>.<id>.cutouts.csv, the N' <= N highest-S/N candidates' cut-outs (.sum.
+// for the total intensity's file).
 // With signal_detect_sum_polarizations, a block whose total intensity is positive keeps every stream's work, and the
 // first stream's work writes the sum's series as <prefix><counter>.sum.<boxcar>.tim (once per block).
 // counter = udp_packet_counter, or the timestamp when there is none (:145-148).
@@ -144,6 +147,7 @@ class write_signal_pipe {
       // signal_detect_candidates: the block path's candidates, and the total intensity's on the first stream's work
       if (w.has_candidates) write_candidates(w, stem);
       if (w.has_sum_candidates) write_candidate_rows(w, w.sum_candidates, stem + ".sum.candidates.csv");
+      if (w.sum_cutouts) write_cutouts(w, *w.sum_cutouts, stem + ".sum");
       return;
     }
     std::ofstream f(stem + "." + std::to_string(w.data_stream_id) + ".dm_sweep.csv", std::ios::trunc);
@@ -166,6 +170,35 @@ class write_signal_pipe {
    *  (signal_detect_candidates) writes the same columns: dm = dm_low = dm_high = the block's dm, trial 0. */
   static void write_candidates(const srtb::work::write_signal_work& w, const std::string& stem) {
     write_candidate_rows(w, w.candidates, stem + "." + std::to_string(w.data_stream_id) + ".candidates.csv");
+    if (w.cutouts) write_cutouts(w, *w.cutouts, stem + "." + std::to_string(w.data_stream_id));
+  }
+
+  /** candidate_cutouts: <base>.cutout_ft.npy, <base>.cutout_dmt.npy and <base>.cutouts.csv, a header row, then one row
+   *  per cut-out: its row in the candidate file, center (spectrum sample at bin W/2), decimation, the time of bin 0
+   *  (spectrum sample center - (W/2) decimation, as candidates.csv defines time; empty without a first_sample) and the
+   *  DMs of the plane's first and last rows */
+  static void write_cutouts(const srtb::work::write_signal_work& w, const srtb::work::cutout_set& c,
+                            const std::string& base) {
+    const size_t n = c.rows.size();
+    srtb::io::npy_save(base + ".cutout_ft.npy", c.ft.data(), std::vector<size_t>{n, c.nsub, c.width});
+    srtb::io::npy_save(base + ".cutout_dmt.npy", c.dmt.data(), std::vector<size_t>{n, c.n_rows, c.width});
+    auto fmt = [](const char* f, double v) {
+      char buf[64];
+      std::snprintf(buf, sizeof buf, f, v);
+      return std::string{buf};
+    };
+    const uint64_t two_c = 2 * (uint64_t)w.batch_size;
+    const bool placed = w.first_sample != w.no_first_sample;
+    std::ofstream f(base + ".cutouts.csv", std::ios::trunc);
+    f << "candidate,center,decimation,time,dm_row_low,dm_row_high\n";
+    for (const auto& r : c.rows) {
+      const double bin0 = (double)r.center - (double)(c.width / 2) * (double)r.decimation;
+      const std::string time =
+          placed ? fmt("%.12g", ((double)w.first_sample + (double)two_c * bin0) / srtb::config.baseband_sample_rate) : "";
+      f << r.candidate << "," << r.center << "," << r.decimation << "," << time << "," << fmt("%.9g", r.dm_row_low)
+        << "," << fmt("%.9g", r.dm_row_high) << "\n";
+    }
+    if (!f) SRTB_LOGE << " [write_signal_pipe] " << "cannot write " << base << ".cutouts.csv";
   }
 
   /** write_candidates' file of `candidates` at `path`, under w's share, offset, geometry and first sample */

@@ -240,7 +240,7 @@ inline const std::vector<std::string>& known_options() {
       "signal_detect_signal_noise_threshold", "signal_detect_channel_threshold", "signal_detect_max_boxcar_length",
       "signal_detect_sum_polarizations", "fold_period", "fold_period_derivative", "fold_bin_count",
       "fold_subband_count", "fold_subintegration_blocks", "fold_coherence", "dm_search_candidates",
-      "signal_detect_candidates"};
+      "signal_detect_candidates", "candidate_cutouts"};
   return names;
 }
 
@@ -382,6 +382,7 @@ inline void evaluate_and_apply_changed_config(const std::string& name, const std
   SRTB_PARSE(fold_coherence)
   SRTB_PARSE(dm_search_candidates)
   SRTB_PARSE(signal_detect_candidates)
+  SRTB_PARSE(candidate_cutouts)
   SRTB_PARSE(thread_query_work_wait_time)
   SRTB_PARSE(gui_enable)
   SRTB_PARSE(gui_pixmap_width)
@@ -419,6 +420,22 @@ inline void check_signal_detect_candidates(const srtb::configs& config) {
   if (config.signal_detect_candidates && (!trim(config.dm_list).empty() || !trim(config.incoherent_dm_list).empty()))
     throw std::invalid_argument("[program_options] signal_detect_candidates lists the candidates of the block path at "
                                 "its one dm; with dm_list or incoherent_dm_list set, use dm_search_candidates instead");
+}
+
+/** candidate_cutouts cuts out candidates a candidate list names: it needs one (signal_detect_candidates or
+ *  dm_search_candidates), is a count (not negative), and needs the spectrum of each candidate's block, which the
+ *  coherent DM sweep (dm_list) keeps for no trial */
+inline void check_candidate_cutouts(const srtb::configs& config) {
+  if (config.candidate_cutouts < 0)
+    throw std::invalid_argument("[program_options] candidate_cutouts is a count of candidates per file: got " +
+                                std::to_string(config.candidate_cutouts));
+  if (config.candidate_cutouts == 0) return;
+  if (!config.signal_detect_candidates && !config.dm_search_candidates)
+    throw std::invalid_argument("[program_options] candidate_cutouts needs a candidate list: set "
+                                "signal_detect_candidates (the block path) or dm_search_candidates (a DM search)");
+  if (!trim(config.dm_list).empty())
+    throw std::invalid_argument("[program_options] candidate_cutouts is not available with dm_list: the coherent DM "
+                                "sweep keeps no trial's spectrum; use incoherent_dm_list");
 }
 
 /** signal_detect_sum_polarizations adds the streams of a block: it needs two or more (`streams`, the format's count),

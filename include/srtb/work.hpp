@@ -228,6 +228,20 @@ struct dm_candidate {
   uint32_t trial = 0;
 };
 
+/** candidate_cutouts: the cut-outs of one candidate file (srtb_b200_candidate_cutouts), in S/N order, highest first */
+struct cutout_set {
+  size_t width = 0, nsub = 0, n_rows = 0;
+  std::vector<float> ft;   // [n][nsub][width]
+  std::vector<float> dmt;  // [n][n_rows][width]
+  struct row {
+    uint64_t candidate = 0;  // 0-based row in the candidate file
+    int64_t center = 0;      // spectrum sample at bin width/2
+    uint32_t decimation = 0;
+    float dm_row_low = 0, dm_row_high = 0;  // the plane's first and last rows' DMs
+  };
+  std::vector<row> rows;
+};
+
 struct write_signal_work : public write_file_work {
   std::vector<time_series_holder> time_series;  // non-empty <=> has_signal
   size_t zero_count = 0;
@@ -250,6 +264,8 @@ struct write_signal_work : public write_file_work {
   // signal_detect_candidates with the total-intensity sum: the sum's candidates, on the first stream's work (same share)
   bool has_sum_candidates = false;
   std::vector<dm_candidate> sum_candidates;
+  // candidate_cutouts: the cut-outs of candidates' and of sum_candidates' files (null when off or empty)
+  std::shared_ptr<const cutout_set> cutouts, sum_cutouts;
   // fold_period: the block's fold (srtb_b200_fold), carried by the block's first stream
   std::shared_ptr<const fold_block> fold;
 };

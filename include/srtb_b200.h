@@ -443,6 +443,49 @@ typedef struct {
 } srtb_b200_candidate;
 int srtb_b200_cluster_events(const srtb_b200_event* h_events, size_t n_events, const float* h_dms, size_t n_dm,
                              srtb_b200_candidate* h_candidates, size_t max_candidates, uint64_t* n_candidates);
+/* ---- candidate cut-outs: the dedispersed frequency-time image and the DM-time plane around each candidate ------------
+ * Inputs: S (1..4) spectra x_s [C][L] (complex64, time contiguous, 8-byte aligned), coherently dedispersed at dm; only
+ * samples j < ts = L - time_reserved_count are data. Per request: center, DM dm_req, half-width, decimation q. Per call:
+ * width W (even), nsub (divides C), n_rows.
+ *   power        P(c, j) = sum_s |x_s[c][j]|^2 for 0 <= j < ts when channel c is kept, else 0. |x|^2 = x.x*x.x + x.y*x.y
+ *                in fp32 without contraction, the streams added in order. A channel is kept when |x_s[c][0]|^2 != 0 in
+ *                every stream (the detector's and the total-intensity sum's masking rule).
+ *   k[c]         the incoherent search's shift per unit DM: (1/f(c)^2 - 1/f_ref^2) sample_rate / (2C) 4.148808e3, in
+ *                double, f and f_ref as srtb_b200_incoherent_shifts defines them.
+ *   shift        s(delta, c) = llround((((double)delta - (double)dm) k[c]) / q) decimated bins, half away from zero
+ *                (with q = 1 the incoherent search's s[d][c]).
+ *   decimated    t0 = center - (W/2) q, D(c, m) = sum_{u<q} P(c, t0 + m q + u) in fp32, added in u order.
+ *   image        ft[k][i] = sum over the C/nsub channels c of subband k, in index order, of D(c, i + s(dm_req, c)), i < W.
+ *   row DMs      DM_r = (float)((double)dm_req + (double)halfwidth (double)(r - n_rows/2) / (double)(n_rows/2)), so row
+ *                n_rows/2 is dm_req; with n_rows == 1 the one row is dm_req.
+ *   plane        dmt[r][i] = sum_{c<C}, in index order, of D(c, i + s(DM_r, c)), fp32.
+ * Samples outside [0, ts) add 0: a cut-out near or past a block edge is zero-padded. Raw power sums, no scaling. So with
+ * q = 1, one stream and nsub = C, ft[c][i] is |x[c][t0 + i + s]|^2 bit for bit, and with q = 1, one stream and every
+ * channel kept, dmt[r] at a row DM equal to trial DM_d of srtb_b200_incoherent_dm_search is v_d[t0 + i - S-] bit for bit
+ * wherever that index lies in [0, T).
+ * Four kernel launches per call whatever n, S and n_rows (csrc/cutout.cuh): a plan, the decimation (reads each
+ * request's span of every channel once, at most min(ts, (W + spread) q) samples), the image and the plane. Stream-ordered
+ * on the ctx's stream, synchronised once; two calls write the same bytes.
+ * Before any launch: a null ctx, d_spectra, spectrum, h_requests, h_ft or h_dmt, a zero time_count or chan_count,
+ * streams outside 1..4, a spectrum not 8-byte aligned, n == 0, an odd W, nsub not dividing C, a decimation of 0, or a
+ * non-finite dm, request DM, half-width or shift returns SRTB_B200_E_INVALID; n > 65535, W outside 2..4096, n_rows
+ * outside 1..4096, a decimation above 2^20, time_reserved_count >= time_count, a shift above 2^24 bins or |center| >=
+ * 2^62 returns SRTB_B200_E_SIZE.
+ * Scratch the ctx grows on demand and keeps (each part rounded up to 256 bytes): 8 C + n (24 + 4 n_rows + 8 C + 8 G C +
+ * 4 C Wd + 4 nsub W + 4 n_rows W) bytes of device memory, G = ceil(n_rows / 64) or more row groups (fewer rows per
+ * group when a group's shifts spread over 1792 bins), Wd = W + the widest shift span of one channel over a request's
+ * rows (+ 2). */
+typedef struct {
+  int64_t center;      /* spectrum sample at the image's bin W/2 (before decimation) */
+  float dm;            /* the image's DM and the plane's centre row */
+  float dm_halfwidth;  /* the plane's rows span dm +- dm_halfwidth */
+  uint32_t decimation; /* q >= 1 samples per bin */
+} srtb_b200_cutout_request;
+int srtb_b200_candidate_cutouts(srtb_b200_ctx* ctx, const void* const* d_spectra /* [streams] */, int streams,
+                                size_t time_count, size_t chan_count, size_t time_reserved_count, float freq_low,
+                                float bandwidth, float sample_rate, float dm, const srtb_b200_cutout_request* h_requests,
+                                size_t n, size_t width, size_t nsub, size_t n_rows, float* h_ft /* [n][nsub][W] */,
+                                float* h_dmt /* [n][n_rows][W] */, float* h_row_dms /* [n][n_rows] or NULL */);
 /* Events of the block path: the ring (submit_block_ex / collect_block_ex) that also lists every single pulse of each
  * block at its one DM. Everything submit_block_ex / collect_block_ex hand out is the same, bit for bit. In addition
  * every stream's detector series is searched for events (the definition above) at the end of that stream's chain, on

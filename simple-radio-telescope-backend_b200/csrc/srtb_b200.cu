@@ -28,6 +28,7 @@
 #include "stream_sum.cuh"
 #include "fold.cuh"
 #include "events.cuh"
+#include "cutout.cuh"
 
 using namespace srtb_b200;
 
@@ -196,6 +197,8 @@ struct srtb_b200_ctx {
   buffer<char> fold_work;
   // the DM searches' and series_events' event list (their scratch is the first lane's)
   buffer<char, true> ev_host;
+  // candidate_cutouts: the tables, decimated power rows and images of one call (cutout_layout)
+  buffer<char> cut_work;
 };
 
 static void lane_swap(srtb_b200_ctx* ctx) {
@@ -2768,17 +2771,22 @@ extern "C" int srtb_b200_process_block_dm_sweep_events(srtb_b200_ctx* ctx, const
 // greedily into groups of at most INC_GROUP whose spread over every channel is at most INC_SPREAD_MAX (a single trial
 // has none), so neighbouring trials share a group whatever order they came in. Returns SRTB_B200_E_INVALID for a shift
 // that is not finite, SRTB_B200_E_SIZE for one out of range.
-static int incoherent_plan_for(size_t C, float freq_low, float bandwidth, float sample_rate, float dm, const float* dms,
-                               size_t n_dm, incoherent_plan* pl) {
+// k[c] of the shifts below: channel c's residual delay per unit DM, in spectrum samples (double; the cut-outs use it too)
+static double dispersion_k(size_t C, float freq_low, float bandwidth, float sample_rate, size_t c) {
   constexpr double D = 4.148808e3;
   const double f_ref = (double)(float)(freq_low + bandwidth);
   const double scale = (double)sample_rate / (2.0 * (double)C);
+  const double f = (double)freq_low + (double)bandwidth * ((double)c + 0.5) / (double)C;
+  return (1.0 / (f * f) - 1.0 / (f_ref * f_ref)) * scale * D;
+}
+
+static int incoherent_plan_for(size_t C, float freq_low, float bandwidth, float sample_rate, float dm, const float* dms,
+                               size_t n_dm, incoherent_plan* pl) {
   std::vector<int64_t>& sh = pl->shifts;
   sh.assign(n_dm * C, 0);
   int64_t hi = 0, lo = 0;
   for (size_t c = 0; c < C; c++) {
-    const double f = (double)freq_low + (double)bandwidth * ((double)c + 0.5) / (double)C;
-    const double k = (1.0 / (f * f) - 1.0 / (f_ref * f_ref)) * scale * D;
+    const double k = dispersion_k(C, freq_low, bandwidth, sample_rate, c);
     for (size_t d = 0; d < n_dm; d++) {
       const double v = ((double)dms[d] - (double)dm) * k;
       if (!std::isfinite(v)) return SRTB_B200_E_INVALID;
@@ -3005,6 +3013,163 @@ extern "C" int srtb_b200_incoherent_dm_search_events(srtb_b200_ctx* ctx, const v
   return incoherent_dm_search(ctx, d_spectrum, time_count, chan_count, time_reserved_count, freq_low, bandwidth,
                               sample_rate, dm, h_dms, n_dm, snr, channel_threshold, max_boxcar_length, h_results,
                               h_peaks, h_best_trial, h_series, &ev);
+}
+
+// ---- candidate cut-outs (cutout.cuh): the frequency-time image and DM-time plane of every request in four launches.
+
+// the scratch of one call, each part 256-byte aligned: k [C] double, requests [n], row DMs [n][n_rows], bases and image
+// offsets [n][C], group spans [n][groups][C], decimated power [n][C][Wd], then the images ft [n][nsub][W] and dmt
+// [n][n_rows][W]
+struct cutout_layout {
+  size_t k, req, row_dms, base, ft_off, gspan, d, ft, dmt, bytes;
+  cutout_layout(size_t n, size_t C, size_t Wd, size_t W, size_t nsub, size_t n_rows, size_t groups) {
+    size_t o = 0;
+    auto take = [&](size_t b) {
+      const size_t at = o;
+      o += (b + 255) & ~(size_t)255;
+      return at;
+    };
+    k = take(C * sizeof(double));
+    req = take(n * sizeof(cut_request));
+    row_dms = take(n * n_rows * sizeof(float));
+    base = take(n * C * sizeof(int));
+    ft_off = take(n * C * sizeof(int));
+    gspan = take(n * groups * C * sizeof(int2));
+    d = take(n * C * Wd * sizeof(float));
+    ft = take(n * nsub * W * sizeof(float));
+    dmt = take(n * n_rows * W * sizeof(float));
+    bytes = o;
+  }
+};
+
+// an upper bound of |llround(a) - llround(b)| over the shifts of two DMs lo, hi in any channel, k_max = max |k[c]|: the
+// difference of the real shifts plus one for the rounding, with room for their float64 and float32 rounding errors
+static double cutout_shift_bound(float lo, float hi, double k_max, unsigned q) {
+  const double d = std::fabs((double)hi - (double)lo) + std::ldexp(std::fabs((double)hi) + std::fabs((double)lo), -20);
+  return std::floor(d * k_max / (double)q * (1.0 + 1e-9)) + 2.0;
+}
+
+extern "C" int srtb_b200_candidate_cutouts(srtb_b200_ctx* ctx, const void* const* d_spectra, int streams,
+                                           size_t time_count, size_t chan_count, size_t time_reserved_count,
+                                           float freq_low, float bandwidth, float sample_rate, float dm,
+                                           const srtb_b200_cutout_request* h_requests, size_t n, size_t width,
+                                           size_t nsub, size_t n_rows, float* h_ft, float* h_dmt, float* h_row_dms) {
+  API_LOCK(ctx);
+  const std::string who = "candidate_cutouts: ";
+  if (!ctx || !d_spectra || !h_requests || !h_ft || !h_dmt || time_count == 0 || chan_count == 0)
+    return fail(ctx, SRTB_B200_E_INVALID, who + "bad argument");
+  if (streams < 1 || streams > 4) return fail(ctx, SRTB_B200_E_INVALID, who + "streams must be 1 to 4");
+  for (int s = 0; s < streams; s++) {
+    if (!d_spectra[s]) return fail(ctx, SRTB_B200_E_INVALID, who + "a spectrum is null");
+    if (!aligned8(d_spectra[s])) return fail(ctx, SRTB_B200_E_INVALID, who + "a spectrum is not 8-byte aligned");
+  }
+  if (n == 0) return fail(ctx, SRTB_B200_E_INVALID, who + "no requests");
+  if (n > 65535) return fail(ctx, SRTB_B200_E_SIZE, who + "more than 65535 requests");
+  if (width % 2) return fail(ctx, SRTB_B200_E_INVALID, who + "width must be even");
+  if (width < 2 || width > 4096) return fail(ctx, SRTB_B200_E_SIZE, who + "width outside 2 .. 4096");
+  if (n_rows < 1 || n_rows > 4096) return fail(ctx, SRTB_B200_E_SIZE, who + "n_rows outside 1 .. 4096");
+  if (nsub == 0 || chan_count % nsub) return fail(ctx, SRTB_B200_E_INVALID, who + "nsub must divide chan_count");
+  if (!std::isfinite(dm)) return fail(ctx, SRTB_B200_E_INVALID, who + "dm is not finite");
+  for (size_t i = 0; i < n; i++) {
+    const srtb_b200_cutout_request& r = h_requests[i];
+    if (r.decimation == 0) return fail(ctx, SRTB_B200_E_INVALID, who + "a decimation is 0");
+    if (r.decimation > (1u << 20)) return fail(ctx, SRTB_B200_E_SIZE, who + "a decimation above 2^20");
+    if (!std::isfinite(r.dm) || !std::isfinite(r.dm_halfwidth))
+      return fail(ctx, SRTB_B200_E_INVALID, who + "a request's dm or dm_halfwidth is not finite");
+  }
+  if (time_reserved_count >= time_count)
+    return fail(ctx, SRTB_B200_E_SIZE, who + "time_reserved_count >= time_count");
+  const size_t C = chan_count, W = width, R = n_rows;
+  std::vector<double> k(C);
+  double k_max = 0;
+  for (size_t c = 0; c < C; c++) {
+    k[c] = dispersion_k(C, freq_low, bandwidth, sample_rate, c);
+    if (!std::isfinite(k[c])) return fail(ctx, SRTB_B200_E_INVALID, who + "a shift is not finite");
+    k_max = std::max(k_max, std::fabs(k[c]));
+  }
+  // every shift fits 2^24 decimated bins and every sample index int64 (|center| < 2^62): each request's row DMs span
+  // [first, last] (monotone in the row), its own DM among them. The window of decimated bins is W + the widest span
+  // of one channel's shifts; groups of rows_per_group rows spread at most INC_SPREAD_MAX bins in any channel
+  std::vector<cut_request> req(n);
+  double wspan = 0;
+  for (size_t i = 0; i < n; i++) {
+    const srtb_b200_cutout_request& r = h_requests[i];
+    const float first = cut_row_dm(r.dm, r.dm_halfwidth, 0, (unsigned)R);
+    const float last = cut_row_dm(r.dm, r.dm_halfwidth, (unsigned)R - 1, (unsigned)R);
+    for (float d : {first, last, r.dm}) {
+      const double v = ((double)d - (double)dm) * k_max / (double)r.decimation;
+      if (!std::isfinite(v)) return fail(ctx, SRTB_B200_E_INVALID, who + "a shift is not finite");
+      if (std::fabs(v) > (double)(1 << 24)) return fail(ctx, SRTB_B200_E_SIZE, who + "a shift out of range (2^24 bins)");
+    }
+    if (r.center >= ((int64_t)1 << 62) || r.center <= -((int64_t)1 << 62))
+      return fail(ctx, SRTB_B200_E_SIZE, who + "a center out of range (2^62)");
+    wspan = std::max(wspan, cutout_shift_bound(first, last, k_max, r.decimation));
+    req[i] = cut_request{(long long)r.center - (long long)(W / 2) * (long long)r.decimation, r.decimation, r.dm,
+                         r.dm_halfwidth};
+  }
+  unsigned rows_per_group = INC_GROUP;
+  for (;; rows_per_group /= 2) {
+    bool fits = true;
+    for (size_t i = 0; i < n && fits && rows_per_group > 1; i++) {
+      const srtb_b200_cutout_request& r = h_requests[i];
+      for (size_t r0 = 0; r0 < R && fits; r0 += rows_per_group) {
+        const size_t r1 = std::min(r0 + rows_per_group, R) - 1;
+        fits = cutout_shift_bound(cut_row_dm(r.dm, r.dm_halfwidth, (unsigned)r0, (unsigned)R),
+                                  cut_row_dm(r.dm, r.dm_halfwidth, (unsigned)r1, (unsigned)R), k_max,
+                                  r.decimation) <= INC_SPREAD_MAX;
+      }
+    }
+    if (fits) break;
+  }
+  const unsigned groups = (unsigned)((R + rows_per_group - 1) / rows_per_group);
+  const unsigned spread = rows_per_group > 1 ? INC_SPREAD_MAX : 0;
+  const size_t Wd = W + (size_t)wspan;
+  const unsigned d_tiles = (unsigned)((Wd + CUT_THREADS - 1) / CUT_THREADS);
+  const unsigned w_tiles = (unsigned)((W + CUT_THREADS - 1) / CUT_THREADS);
+  const unsigned p_tiles = (unsigned)((W + INC_TILE - 1) / INC_TILE);
+  if ((double)C * d_tiles > 2147483647.0 || (double)nsub * w_tiles > 2147483647.0)
+    return fail(ctx, SRTB_B200_E_SIZE, who + "a shift out of range (grid)");
+  CK(cudaSetDevice(ctx->device));
+  const cutout_layout lay(n, C, Wd, W, nsub, R, groups);
+  if (int rc = grow(ctx, ctx->cut_work, lay.bytes)) return rc;
+  char* w = ctx->cut_work.p;
+  cudaStream_t st = ctx->lane.stream;
+  // pageable sources: each copy returns once its bytes are staged, so the host vectors may go when we return
+  CK(cudaMemcpyAsync(w + lay.k, k.data(), C * sizeof(double), cudaMemcpyHostToDevice, st));
+  CK(cudaMemcpyAsync(w + lay.req, req.data(), n * sizeof(cut_request), cudaMemcpyHostToDevice, st));
+  const auto* d_req = reinterpret_cast<const cut_request*>(w + lay.req);
+  const auto* d_k = reinterpret_cast<const double*>(w + lay.k);
+  auto* d_row_dms = reinterpret_cast<float*>(w + lay.row_dms);
+  auto* d_base = reinterpret_cast<int*>(w + lay.base);
+  auto* d_ft_off = reinterpret_cast<int*>(w + lay.ft_off);
+  auto* d_gspan = reinterpret_cast<int2*>(w + lay.gspan);
+  auto* d_D = reinterpret_cast<float*>(w + lay.d);
+  auto* d_ft = reinterpret_cast<float*>(w + lay.ft);
+  auto* d_dmt = reinterpret_cast<float*>(w + lay.dmt);
+  cut_spectra sp{};
+  for (int s = 0; s < streams; s++) sp.x[s] = static_cast<const float2*>(d_spectra[s]);
+  sp.streams = streams;
+  sp.L = time_count;
+  sp.C = C;
+  sp.ts = time_count - time_reserved_count;
+  const unsigned plan_x = (unsigned)((std::max(C, R) + CUT_THREADS - 1) / CUT_THREADS);
+  CK(launch(ctx, false, cutout_plan_kernel, dim3(plan_x, (unsigned)n), CUT_THREADS, 0, d_req, d_k, C, (double)dm,
+            (unsigned)R, rows_per_group, groups, d_row_dms, d_base, d_ft_off, d_gspan));
+  CK(launch(ctx, false, cutout_decimate_kernel, dim3((unsigned)(C * d_tiles), (unsigned)n), CUT_THREADS, 0, sp, d_req,
+            static_cast<const int*>(d_base), Wd, d_tiles, d_D));
+  CK(launch(ctx, false, cutout_ft_kernel, dim3((unsigned)(nsub * w_tiles), (unsigned)n), CUT_THREADS, 0,
+            static_cast<const float*>(d_D), static_cast<const int*>(d_ft_off), C, Wd, (unsigned)W, (unsigned)nsub,
+            w_tiles, d_ft));
+  CK(launch(ctx, false, cutout_plane_kernel, dim3(groups * p_tiles, (unsigned)n), INC_THREADS,
+            cutout_plane_smem_bytes(spread), static_cast<const float*>(d_D), C, Wd,
+            static_cast<const int2*>(d_gspan), static_cast<const int*>(d_base), d_k,
+            static_cast<const float*>(d_row_dms), d_req, (double)dm, (unsigned)R, rows_per_group, groups,
+            (unsigned)W, (unsigned)(INC_TILE + spread), d_dmt));
+  CK(cudaMemcpyAsync(h_ft, d_ft, n * nsub * W * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CK(cudaMemcpyAsync(h_dmt, d_dmt, n * R * W * sizeof(float), cudaMemcpyDeviceToHost, st));
+  if (h_row_dms) CK(cudaMemcpyAsync(h_row_dms, d_row_dms, n * R * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CK(cudaStreamSynchronize(st));
+  return 0;
 }
 
 // ---- fold at a pulsar period (fold.cuh): the bin plan of each time tile, one read of the spectra into per-CTA bin

@@ -99,6 +99,12 @@ class Candidate(C.Structure):
                 ("trial", C.c_uint32), ("stream", C.c_uint32)]
 
 
+class CutoutRequest(C.Structure):
+    """srtb_b200_cutout_request: one candidate's cut-out (srtb_b200_candidate_cutouts): the spectrum sample at the
+    image's bin W/2, the image's DM, the plane's DM half-width and the decimation q"""
+    _fields_ = [("center", C.c_int64), ("dm", C.c_float), ("dm_halfwidth", C.c_float), ("decimation", C.c_uint32)]
+
+
 def _dtype_of(struct):
     """the numpy structured dtype with struct's field names, offsets and size"""
     import numpy as np
@@ -186,6 +192,8 @@ SYMBOLS = {
     "srtb_b200_submit_block_events": (_I, [_P, C.POINTER(BlockConfig), _P, _SZ, _I, C.POINTER(BlockOutputs), _SZ]),
     "srtb_b200_collect_block_events": (_I, [_P, _I, C.POINTER(DetectResult), C.POINTER(_P), C.POINTER(_P),
                                             C.POINTER(_P), C.POINTER(C.c_uint64)]),
+    "srtb_b200_candidate_cutouts": (_I, [_P, _P, _I, _SZ, _SZ, _SZ, _F, _F, _F, _F, C.POINTER(CutoutRequest), _SZ,
+                                         _SZ, _SZ, _SZ, _P, _P, _P]),
     "srtb_b200_fold_phase": (_I, [C.c_double, C.c_double, C.c_double, C.c_uint64, C.c_uint64,
                                   C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "srtb_b200_fold": (_I, [_P, C.POINTER(_P), _I, _SZ, _SZ, _SZ, C.c_double, C.c_double, C.c_double, _SZ, _SZ,
@@ -459,6 +467,27 @@ class Context:
             return results, (snr_a, idx_a), int(best.value), h_series
         return (results, (snr_a, idx_a), int(best.value), h_series, ev[:min(n_ev.value, max_events)].copy(),
                 int(n_ev.value))
+
+    def candidate_cutouts(self, d_spectra, time_count: int, chan_count: int, time_reserved_count: int,
+                          freq_low: float, bandwidth: float, sample_rate: float, dm: float, requests, width: int,
+                          nsub: int, n_rows: int):
+        """the frequency-time image and DM-time plane of each request (CutoutRequest, or (center, dm, dm_halfwidth,
+        decimation)) on the [chan_count][time_count] complex64 spectra d_spectra (1 to 4 streams, coherently dedispersed
+        at dm). Returns numpy float32 arrays (ft [n][nsub][width], dmt [n][n_rows][width], row_dms [n][n_rows])"""
+        import numpy as np
+        reqs = [r if isinstance(r, CutoutRequest) else CutoutRequest(int(r[0]), float(r[1]), float(r[2]), int(r[3]))
+                for r in requests]
+        n = len(reqs)
+        arr = (CutoutRequest * max(n, 1))(*reqs)
+        streams = len(d_spectra)
+        sp = (C.c_void_p * max(streams, 1))(*[_ptr(d) for d in d_spectra])
+        ft = np.zeros((n, nsub, width), np.float32)
+        dmt = np.zeros((n, n_rows, width), np.float32)
+        row_dms = np.zeros((n, n_rows), np.float32)
+        self._ck(self.lib.srtb_b200_candidate_cutouts(
+            self.h, C.cast(sp, C.c_void_p), streams, time_count, chan_count, time_reserved_count, freq_low, bandwidth,
+            sample_rate, dm, arr, n, width, nsub, n_rows, ft.ctypes.data, dmt.ctypes.data, row_dms.ctypes.data))
+        return ft, dmt, row_dms
 
     def _submitted(self, cfg: BlockConfig, ticket: int) -> int:
         self._sum_tickets[ticket] = bool(cfg.signal_detect_sum_streams)

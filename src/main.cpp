@@ -233,6 +233,7 @@ int main(int argc, char** argv) {
     srtb::program_options::check_fold(cfg);
     srtb::program_options::check_dm_search_candidates(cfg);
     srtb::program_options::check_signal_detect_candidates(cfg);
+    srtb::program_options::check_candidate_cutouts(cfg);
   } catch (const std::exception& e) {
     std::fprintf(stderr, "srtb_b200: %s\n", e.what());
     return 2;
